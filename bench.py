@@ -90,7 +90,7 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler:
@@ -241,12 +241,12 @@ def run_reference_arm(args):
         return run_reference_model_arm(args)
     wl = args.workload
     cores, avail = pick_cpu_threads()
-    steps = max(1, min(args.steps, 3))  # bounded: each step is a full fwd+bwd of the workload (~10 s of CPU work)
-    t = cpu_reference_steps(wl, steps, min(args.warmup, 1))
+    steps = args.steps
+    t = cpu_reference_steps(wl, steps, args.warmup)
     val = 1.0 / t
     line = {
         "impl": "reference", "metric": "SFNO-block fwd+bwd samples/sec", "value": val, "unit": "samples/s", "n_gpus": args.gpus, "steps": steps,
-        "warmup": min(args.warmup, 1), "ms_per_step": t * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
+        "warmup": args.warmup, "ms_per_step": t * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
         "data": "synthetic", "config": {"workload": wl, "batch_per_gpu": 1, "activations": "bf16", "parallelism": "cpu"},
         "cpu_baseline": {"value": val, "unit": "samples/s", "cores": cores, "kind": "port",
                          "sample": f"{steps} full fwd+bwd steps of the workload through oracle/makani_oracle.py (torch.fft + torch.einsum, fp32, {cores} threads chosen by calibration of {avail} available)"},
@@ -257,7 +257,7 @@ def run_reference_arm(args):
 
 def run_reference_model_arm(args):
     """CPU arm of the full-model workloads: the same network (makani_b200.sfno, pinned against the reference's network class by
-    tests/golden/sfno_golden.npz) on the oracle transforms / SpectralConv, bf16 autocast off (CPU), one bounded step."""
+    tests/golden/sfno_golden.npz) on the oracle transforms / SpectralConv, bf16 autocast off (CPU); --warmup and --steps as given."""
     from makani_b200.sfno import SphericalFourierNeuralOperatorNet
     from oracle.sfno_backend import OracleBackend
 
@@ -266,17 +266,24 @@ def run_reference_model_arm(args):
     torch.manual_seed(333)
     net = SphericalFourierNeuralOperatorNet(**cfg, backend=OracleBackend())
     x = torch.randn(1, cfg["inp_chans"], *cfg["inp_shape"])
+
+    def step():
+        net.zero_grad(set_to_none=True)
+        net(x).float().square().mean().backward()
+
+    for _ in range(args.warmup):
+        step()
     t0 = time.perf_counter()
-    out = net(x)
-    out.float().square().mean().backward()
-    t = time.perf_counter() - t0
+    for _ in range(args.steps):
+        step()
+    t = (time.perf_counter() - t0) / args.steps
     val = 1.0 / t
     print(json.dumps({
-        "impl": "reference", "metric": "SFNO model fwd+bwd samples/sec", "value": val, "unit": "samples/s", "n_gpus": args.gpus, "steps": 1, "warmup": 0,
+        "impl": "reference", "metric": "SFNO model fwd+bwd samples/sec", "value": val, "unit": "samples/s", "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": t * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": args.workload, "batch_per_gpu": 1, "parallelism": "cpu"},
         "cpu_baseline": {"value": val, "unit": "samples/s", "cores": cores, "kind": "port",
-                         "sample": f"1 full fwd+bwd step of the network on oracle/ (torch.fft + torch.einsum, fp32, {cores} threads of {avail})"},
+                         "sample": f"{args.steps} full fwd+bwd steps of the network on oracle/ (torch.fft + torch.einsum, fp32, {cores} threads of {avail})"},
         "e2e": {"value": val, "unit": "samples/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}), flush=True)
 
 
@@ -388,7 +395,9 @@ def run_gpu_arm(args):
     x_dev = x_host.to(dev)
     gy = torch.randn(1, C, nlat_o, nlon_o, device=dev).to(act_dtype)
     gw_host = torch.empty(conv.weight.shape, dtype=torch.complex64).pin_memory()
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > the 50 MB L2 of an H100
+
+    last = {}   # what the last step returned to its caller (--dump-outputs)
 
     def step(xin):
         xin.requires_grad_(True)
@@ -398,6 +407,7 @@ def run_gpu_arm(args):
         g = xin.grad
         xin.grad = None
         xin.requires_grad_(False)
+        last["y"], last["dx"] = y.detach(), g
         return g
 
     def step_e2e():
@@ -555,6 +565,9 @@ def run_gpu_arm(args):
                 torch.cuda.synchronize()
         ms_dev = timed(dp_step, args.steps, args.warmup)
         host_ms = host_enqueue.get("ms_per_step")
+        if args.dump_outputs and rank == 0:
+            torch.cuda.synchronize()
+            dump_outputs(args.dump_outputs, {"y": last["y"], "dx": last["dx"], "dweight": torch.view_as_real(conv.weight.grad)})
         # the same step replayed from a CUDA graph, reported separately (`value` stays the eager step: it is what N > 1 and e2e run)
         if args.graph and world == 1:
             graph_info = try_cuda_graph()
@@ -674,7 +687,7 @@ def run_gpu_arm(args):
                          f"chosen by calibration of {avail} available), {t:.2f} s/step"}
 
     # The library path the reference runs on a GPU (cuFFT + cuBLAS einsum, allow_tf32=True as makani/train.py:87), timed on this
-    # B200 with the same restated modules (the real torch-harmonics is not installable): informational, never the product path.
+    # GPU with the same restated modules (the real torch-harmonics is not installable): informational, never the product path.
     lib = None
     if not args.no_cpu and world == 1:
         try:
@@ -687,7 +700,7 @@ def run_gpu_arm(args):
         "metric": "SFNO-block fwd+bwd samples/sec", "value": world * 1e3 / ms_dev, "unit": "samples/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_dev, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "tf32" if precision == "tf32" else ("f32 (3 x tf32 Legendre)" if precision == "fp32x3" else "f32"),
         "data": "synthetic",
-        "config": {"workload": wl, "shape": [1, C, nlat_i, nlon_i], "activations": args.act, "contraction": {"tf32": "tcgen05 kind::tf32, fp32 accumulate", "fp32x3": "Legendre: 3 x TF32 on tcgen05 (fp32 operands); mix, FFT: fp32 FMA"}.get(precision, "fp32 FMA (CUDA cores)"),
+        "config": {"workload": wl, "shape": [1, C, nlat_i, nlon_i], "activations": args.act, "contraction": {"tf32": "TF32 mma.sync, fp32 accumulate", "fp32x3": "Legendre: 3 x TF32 on the tensor cores (fp32 operands); mix, FFT: fp32 FMA"}.get(precision, "fp32 FMA (CUDA cores)"),
                    "batch_per_gpu": 1, "global_batch": world, "parallelism": f"dp{world}" if world > 1 else "single", "dp_allreduce": dp_mode if world > 1 else None, "operator": "dhconv", "lmax": L, "mmax": M,
                    "l2": f"256 MiB buffer written between timed iterations (L2 flush); input {x_host.numel() * x_host.element_size() / 1e6:.0f} MB",
                    "weight_relayout_in_step": True, "flops_fwd_bwd_nnz": flops_fwd_bwd(wl)},
@@ -695,7 +708,7 @@ def run_gpu_arm(args):
         "e2e": {"value": world * 1e3 / ms_e2e, "unit": "samples/s", "ms_per_step": ms_e2e, "h2d_bytes_per_step": x_bytes, "d2h_bytes_per_step": gw_host.numel() * 8,
                 "how": f"makani_b200.HostFeed: every step copies its {x_bytes / 1e6:.0f} MB input from pinned host memory and reads its weight gradient back; the "
                        "copy of step i+1 (side stream, second device buffer) and the read-back of step i-1 overlap the kernels of step i; K steps timed "
-                       "from the first copy to the last read-back; two input buffers + gradients exceed the 126 MB L2",
+                       "from the first copy to the last read-back; two input buffers + gradients exceed the 50 MB L2",
                 "serial_value": world * 1e3 / ms_e2e_serial, "serial_ms_per_step": ms_e2e_serial,
                 "serial_how": "copy -> fwd+bwd -> read-back in one stream, L2 flushed between steps"},
         "gpu_launches": launches_per_step,
@@ -873,6 +886,21 @@ def run_model_arm(args):
         dist.destroy_process_group()
 
 
+def dump_outputs(outdir, arrays, budget_bytes=64 << 20):
+    """Write each array as <outdir>/<name>.npy in float32.  An array larger than its share of the budget is replaced by a fixed sample:
+    the elements at sorted indices drawn from a generator seeded with 0, the same for every run with the same shapes."""
+    import numpy as np
+
+    os.makedirs(outdir, exist_ok=True)
+    per = budget_bytes // (4 * len(arrays))
+    for name, t in arrays.items():
+        flat = t.detach().float().reshape(-1).cpu()
+        if flat.numel() > per:
+            g = torch.Generator().manual_seed(0)
+            flat = flat[torch.randint(0, flat.numel(), (per,), generator=g).sort().values]
+        np.save(os.path.join(outdir, name + ".npy"), flat.numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -883,6 +911,8 @@ def main():
     ap.add_argument("--precision", default="best", choices=["best", "fp32", "tf32", "fp32x3"])
     ap.add_argument("--act", default="bf16", choices=["bf16", "fp32"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step returned (y, dx, dweight) as DIR/<name>.npy, float32, <= 64 MB in all")
     ap.add_argument("--no-stages", action="store_true", help="skip per-stage kernel timing")
     ap.add_argument("--no-hxw", action="store_true", help="N > 1: skip the additional h x w spatial-model-parallel measurement of the same block")
     ap.add_argument("--graph", action="store_true", default=True, help="also time the step replayed from a CUDA graph (N = 1; reported as cuda_graph_replay, never as `value`)")
@@ -891,11 +921,15 @@ def main():
                     help="N > 1: weight-gradient all-reduce after the backward pass on the compute stream (trailing, default: measured faster, DESIGN.md section 7) or on a "
                          "side stream behind the wgrad event with reserved SMs (overlap)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    if args.dump_outputs and (args.impl == "reference" or args.workload in MODEL_WORKLOADS):
+        ap.error("--dump-outputs is implemented for the SpectralConv block workloads of --impl b200 only")
     if args.impl == "reference":
         run_reference_arm(args)
     else:
         if not torch.cuda.is_available():
-            raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback); use --impl reference for the CPU arm")
+            raise SystemExit("bench.py: no CUDA device (the CUDA path has no CPU fallback); use --impl reference for the CPU arm")
         if args.workload in MODEL_WORKLOADS:
             run_model_arm(args)
         else:

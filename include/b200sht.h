@@ -1,5 +1,5 @@
 /*
- * b200sht -- C ABI of the B200-native spherical-harmonic hot path (RealSHT / InverseRealSHT / SpectralConv).
+ * b200sht -- C ABI of the H100-native (sm_90a) spherical-harmonic hot path (RealSHT / InverseRealSHT / SpectralConv).
  *
  * Nothing equivalent exists in the reference: NVIDIA/makani has no native code (SURVEY.md F2) and reaches this
  * arithmetic through the Python package torch-harmonics.  Each entry point below names the reference interface
@@ -52,8 +52,8 @@ typedef enum { B200SHT_F32 = 0, B200SHT_BF16 = 1 } b200sht_dtype;
 /* arithmetic of the Legendre / channel-mix contractions */
 typedef enum {
   B200SHT_PREC_FP32 = 0, /* fp32 FMA on CUDA cores (reference tests run with TF32 disabled)          */
-  B200SHT_PREC_TF32 = 1, /* tcgen05 kind::tf32, fp32 accumulate in TMEM (reference training: allow_tf32) */
-  B200SHT_PREC_FP32X3 = 2 /* fp32 operands on the tensor cores: Legendre stages as 3 x TF32 (hi.hi + hi.lo + lo.hi into one TMEM accumulator),
+  B200SHT_PREC_TF32 = 1, /* TF32 tensor-core MMA (mma.sync), fp32 accumulate (reference training: allow_tf32) */
+  B200SHT_PREC_FP32X3 = 2 /* fp32 operands on the tensor cores: Legendre stages as 3 x TF32 (hi.hi + hi.lo + lo.hi into one fp32 accumulator),
                              longitude transform and channel mix as in FP32.  Element errors stay inside rtol 1e-5 (atol = rtol max|ref|), relative
                              L2 ~ 1e-6 .. 8e-6 growing with nlat (the tensor core truncates its fp32 accumulator on every add; the CUDA-core FP32 mode
                              rounds to nearest and stays at ~ 3e-7): ~1.7 x the speed of FP32 at 721 x 1440.  Uses a per-device scratch buffer for the
@@ -89,7 +89,7 @@ int b200sht_plan_create(b200sht_plan** plan, int nlat, int nlon, int lmax, int m
 int b200sht_plan_create_ex(b200sht_plan** plan, int nlat, int nlon, int lmax, int mmax, int m_offset, int flags,
                            const double* cost, const double* quad_w, int csphase, void* stream);
 int b200sht_plan_destroy(b200sht_plan* plan);
-/* what: 0 nlat, 1 nlon, 2 lmax, 3 mmax, 4 kp, 5 table bytes, 6 tcgen05 path available (0/1), 7 m_offset,
+/* what: 0 nlat, 1 nlon, 2 lmax, 3 mmax, 4 kp, 5 table bytes, 6 tensor-core path available (0/1; sm_90 devices), 7 m_offset,
  *       8 tensor-core longitude DFT available for this grid (0/1) */
 int64_t b200sht_plan_query(const b200sht_plan* plan, int what);
 /* device pointer to the fp32 table [mmax][lmax][kp] (for tests) */
@@ -107,16 +107,16 @@ int64_t b200sht_spec_elems_lm(int L, int M, int B, int C);
  *   X[m][p][r][k] = row_scale[k] * mode_scale[m] * sum_j x[r][k][j] exp(-2 pi i m j / nlon)
  * scale_mode 0: SHT forward     (row_scale = quad_w[k] * 2 pi / nlon, mode_scale = 1)
  * scale_mode 1: adjoint of irfft (row_scale = 1, mode_scale = 1 for m = 0 and Nyquist, 2 otherwise)
- * scale_mode | 2: TF32 precision: the output is rounded to the nearest TF32 value (it is the operand of a kind::tf32 GEMM) and,
+ * scale_mode | 2: TF32 precision: the output is rounded to the nearest TF32 value (it is the operand of a TF32 GEMM) and,
  *                 for nlon = 8 * N2 <= 1520 and mmax <= 256, the transform itself runs on the tensor cores (radix-8 butterflies on
- *                 the CUDA cores x a [mmax/8 x nlon/16] DFT matrix as a kind::tf32 GEMM, csrc/dft.cu) */
+ *                 the CUDA cores x a [mmax/8 x nlon/16] DFT matrix as a TF32 GEMM, csrc/dft.cu) */
 int b200sht_fft_analysis(const b200sht_plan* plan, const void* x, int dtype, int B, int C,
                          float* latspec, int scale_mode, void* stream);
 /* Longitude synthesis: truncated half spectrum -> real rows (+ optional per-channel bias, cast to dtype).
  * scale_mode 0: irfft(norm="forward") semantics (imaginary part of m=0 / Nyquist ignored)
  * scale_mode 1: adjoint of the scale_mode-0 analysis (row_scale = quad_w[k] 2 pi/nlon, modes m>0 halved)
  * scale_mode | 2: `latspec` is in the TILED layout written by b200sht_legendre_synthesis_tiled and the transform runs on the tensor
- *                 cores (TF32; radix-8 butterflies on the CUDA cores x a [mmax/8 x nlon/16] DFT matrix as a kind::tf32 GEMM, csrc/dft.cu).
+ *                 cores (TF32; radix-8 butterflies on the CUDA cores x a [mmax/8 x nlon/16] DFT matrix as a TF32 GEMM, csrc/dft.cu).
  *                 Error unless b200sht_plan_query(plan, 8) == 1. */
 int b200sht_fft_synthesis(const b200sht_plan* plan, const float* latspec, void* y, int dtype, int B, int C,
                           const float* bias, int scale_mode, void* stream);
@@ -254,7 +254,7 @@ int b200sht_bias_gelu_forward(const void* x, const float* bias, void* y, int dty
 int b200sht_bias_gelu_backward(const void* x, const float* bias, const void* dy, void* dx, float* row_sums, float* workspace, int dtype, int B, int C, int64_t hw,
                                void* stream);
 
-/* Programmatic dependent launch between the tcgen05 kernels of a call sequence (prologue of kernel i+1 under the tail of kernel i; environment
+/* Programmatic dependent launch between the tensor-core kernels of a call sequence (prologue of kernel i+1 under the tail of kernel i; environment
  * B200SHT_PDL sets the initial value, default on).  Returns the previous setting.  Results do not depend on it. */
 int b200sht_debug_set_pdl(int on);
 /* Latitude chunks of the fused (longitude analysis -> Legendre analysis) pair inside b200sht_sht_forward / _inverse_adjoint and the

@@ -1,4 +1,4 @@
-"""makani_b200 -- B200-native (sm_100a) implementation of makani's spherical-harmonic hot path.
+"""makani_b200 -- H100-native (sm_90a) implementation of makani's spherical-harmonic hot path.
 
 Public surface (mirrors the reference, see INTEGRATION.md):
     RealSHT, InverseRealSHT                    <- torch_harmonics.{RealSHT, InverseRealSHT}

@@ -1,7 +1,7 @@
 """ctypes binding of the in-tree CUDA library `libb200sht.so` (C ABI: include/b200sht.h).
 
 The product path has no CPU or PyTorch fallback: if the library cannot be loaded, or a call fails, a
-`B200ShtError` is raised.  The library is built in-tree by `makani_b200/build.py` (nvcc, sm_100a).
+`B200ShtError` is raised.  The library is built in-tree by `makani_b200/build.py` (nvcc, sm_90a).
 """
 import ctypes
 import os
@@ -107,7 +107,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise B200ShtError(
-            f"{LIB_PATH} not found: build it with `python -m makani_b200.build` (nvcc, sm_100a). "
+            f"{LIB_PATH} not found: build it with `python -m makani_b200.build` (nvcc, sm_90a). "
             "makani_b200 has no CPU / PyTorch fallback for the spherical-harmonic path."
         )
     try:

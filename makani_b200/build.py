@@ -1,4 +1,4 @@
-"""Build the in-tree CUDA library makani_b200/libb200sht.so for sm_100a with nvcc (no GPU needed: cross-compiles)."""
+"""Build the in-tree CUDA library makani_b200/libb200sht.so for sm_90a (H100) with nvcc (no GPU needed: cross-compiles)."""
 import os
 import subprocess
 import sys
@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200sht.so")
 SOURCES = ["capi.cu", "fft.cu", "legendre.cu", "mix.cu", "act.cu", "umma.cu", "dft.cu", "norm.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 

@@ -37,7 +37,7 @@ int mix_backward_simt(const Plan* pl, int op, const float* x, const void* w, con
 int complex_relu_fwd(const Plan* pl, int mode, const float* x, const float* bias, float slope, float* y, int B, int C, cudaStream_t st);
 int complex_relu_bwd(const Plan* pl, int mode, const float* x, const float* bias, float slope, const float* gy, float* gx, float* gbias, int B,
                      int C, cudaStream_t st);
-// tcgen05 path (umma.cu)
+// tensor-core path (umma.cu)
 int umma_plan_init(Plan* pl);
 void umma_plan_destroy(Plan* pl);
 int dft_plan_init(Plan* pl);
@@ -202,7 +202,7 @@ int b200sht_fft_synthesis(const b200sht_plan* pl, const float* latspec, void* y,
 }
 
 // ---------------------------------------------------------------------------------- fp32 operands on the tensor cores
-// B200SHT_PREC_FP32X3: the Legendre stages run as 3 x TF32 (hi.hi + hi.lo + lo.hi with fp32 accumulation in TMEM) instead of the CUDA-core
+// B200SHT_PREC_FP32X3: the Legendre stages run as 3 x TF32 (hi.hi + hi.lo + lo.hi with fp32 accumulation in registers) instead of the CUDA-core
 // kernels.  The residual of the activation operand lives in a per-device scratch buffer that grows on demand: calls of this mode on one
 // device must be issued from one stream at a time (they are stream-ordered through the same buffer).
 static float* residual_scratch(size_t bytes) {
@@ -226,7 +226,7 @@ static int check_precision(int umma_ok, int precision, const char* who) {
   if (precision == B200SHT_PREC_FP32) return 0;
   if (precision == B200SHT_PREC_TF32 || precision == B200SHT_PREC_FP32X3) {
     if (!umma_ok) {
-      set_error("%s: the tcgen05 (TF32 / 3 x TF32) path is not available on this device/build; refusing to fall back silently", who);
+      set_error("%s: the tensor-core (TF32 / 3 x TF32) path is not available on this device/build (it needs sm_90); refusing to fall back silently", who);
       return B200SHT_ERR_UNSUPPORTED;
     }
     return 0;
@@ -279,12 +279,12 @@ int b200sht_legendre_synthesis_tiled(const b200sht_plan* pl, const float* spec, 
 }
 
 // Longitude analysis + Legendre analysis.  At TF32 with the tensor-core DFT the pair can run in latitude chunks: the DFT writes the latspec
-// rows of one chunk (tens of MB) and the Legendre kernel reduces over exactly those rows right away -- reading them from the 126 MB L2
-// instead of HBM -- and adds its partial sums to the coefficients of the earlier chunks (unrounded fp32; the last chunk rounds to TF32).
+// rows of one chunk (tens of MB) and the Legendre kernel reduces over exactly those rows right away -- reading them from L2 (50 MB on
+// an H100) instead of HBM -- and adds its partial sums to the coefficients of the earlier chunks (unrounded fp32; the last chunk rounds to TF32).
 // The Legendre table is sliced along latitude, so no byte of it is read twice.  B200SHT_LAT_CHUNKS = n forces n chunks (1 = off);
 // default: chunks of at most kLatChunkBytes of latspec when the whole tensor exceeds it.
-constexpr size_t kLatChunkBytes = 40u << 20;
-constexpr bool kLatChunkByDefault = false;   // see DESIGN.md section 10 for the measurement behind this
+constexpr size_t kLatChunkBytes = 16u << 20;   // a third of the H100's 50 MB L2: the chunk and its slice of the table stay resident
+constexpr bool kLatChunkByDefault = false;      // off until a measurement on the H100 shows a gain
 static int& lat_chunks_forced() {
   static int forced = [] { const char* e = getenv("B200SHT_LAT_CHUNKS"); return e ? atoi(e) : 0; }();
   return forced;
@@ -461,7 +461,7 @@ int b200sht_mix_weight_unpack(int op, const float* w_packed, void* w_native, int
 }
 
 static bool dense_op(int op) { return op == B200SHT_OP_DHCONV || op == B200SHT_OP_SHARED || op == B200SHT_OP_LDEP; }
-// The tcgen05 mix addresses operands with TMA: group slices must start on 16-byte boundaries and the batch must divide 32.
+// The tensor-core mix addresses operands with TMA: group slices must start on 16-byte boundaries and the batch must divide 32.
 // Other shapes (none of the shipped configs: G = 1, B = 1 per GPU) are served by the fp32 CUDA-core kernels.
 static bool umma_mix_shape(int B, int G, int Ci, int Co) {
   return B >= 1 && 32 % B == 0 && (G == 1 || ((Ci / G) % 4 == 0 && (Co / G) % 4 == 0));

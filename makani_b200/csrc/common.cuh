@@ -33,7 +33,7 @@ void set_error(const char* fmt, ...);
     }                                           \
   } while (0)
 
-// round-to-nearest conversion to TF32 (10-bit mantissa), as cuBLAS applies to its TF32 GEMM inputs; tcgen05 kind::tf32 itself
+// round-to-nearest conversion to TF32 (10-bit mantissa), as cuBLAS applies to its TF32 GEMM inputs; the TF32 MMA itself
 // truncates the low 13 mantissa bits of whatever it reads, so producers of tensor-core operands round first.
 __device__ __forceinline__ float tf32_rn(float x) {
   uint32_t u;
@@ -67,15 +67,15 @@ struct Plan {
   int no_table;         // FFT-only plan (latitude-sharded stage of the distributed SHT)
   int dense;            // dims-only plans: packed spec tensors store every (l, m) entry (no block triangle)
   float* d_table;       // [mmax][lmax][kp]
-  float* d_table_tf32;  // same, rounded to nearest TF32 (operand of the tcgen05 kernels); null when that path is unavailable
+  float* d_table_tf32;  // same, rounded to nearest TF32 (operand of the tensor-core kernels); null when that path is unavailable
   float* d_table_lo;    // d_table - d_table_tf32 (second term of the 3 x TF32 strict-fp32 mode); allocated at its first use
   float* d_rowscale;    // [kp]  quad_w[k] * 2 pi / nlon (0 in the padding)
   float2* d_twiddle;    // [nlon] exp(-2 pi i t / nlon)
   FftPlan fft;
   int sm_count;
-  int umma_ok;          // tcgen05 path usable on this device
+  int umma_ok;          // tensor-core path usable on this device (sm_90)
   void* umma_state;     // TMA descriptors etc. (owned by umma translation unit)
-  void* dft_state;      // tensor-core DFT tables (dft.cu); null when the grid is outside its range or tcgen05 is unavailable
+  void* dft_state;      // tensor-core DFT tables (dft.cu); null when the grid is outside its range or the tensor-core path is unavailable
 };
 
 // SMs left free by the persistent kernels launched from this thread (0 = use them all).  Set around the stages that are meant to run beside
@@ -100,7 +100,7 @@ inline cudaError_t ensure_dynamic_smem(K kernel, size_t bytes) {
 }
 // ---- programmatic dependent launch (PDL) ------------------------------------------------------------------------------------------
 // The hot kernels call pdl_trigger() first thing (their successor in the stream may be scheduled as soon as every CTA of this grid has done
-// so or exited) and pdl_wait() after their prologue (barrier init, TMEM allocation, tensor-map prefetch, resident constant tables), i.e.
+// so or exited) and pdl_wait() after their prologue (barrier init, tensor-map prefetch, resident constant tables), i.e.
 // before the first access to memory another kernel produces or still reads: the wait returns once all prerequisite grids have COMPLETED and
 // their writes are visible.  A successor launched with launch_pdl() therefore overlaps its launch latency and prologue with the tail of this
 // kernel; launched normally it serialises as always.  Both instructions are no-ops without a programmatic dependency.

@@ -1,23 +1,22 @@
 // Longitude transform on the tensor cores (B200SHT_PREC_TF32): the truncated real DFT of every latitude row as
-//   radix-8 butterflies + twiddles on the CUDA cores  x  one class-independent [M2 x N2/2] DFT matrix on tcgen05 (kind::tf32).
+//   radix-8 butterflies + twiddles on the CUDA cores  x  one class-independent [M2 x N2/2] DFT matrix on the tensor cores (mma.sync TF32).
 // Replaces the CUDA-core Stockham kernels of fft.cu for nlon = 8 * N2, N2 <= 190, mmax <= 256 (every shipped grid); see dft_math.cuh
 // for the factorisation.  Reference semantics: 2 pi * torch.fft.rfft(x, norm="forward")[..., :mmax] and torch.fft.irfft(Z, n=nlon,
 // norm="forward") inside torch_harmonics.RealSHT / InverseRealSHT (call sites makani/models/common/spectral_convolution.py:239,253).
 //
-// Why: the Stockham kernels were issue-bound on the CUDA cores (64.7 M warp instructions, 0.26-0.29 of HBM bandwidth, VERDICT r1 item 5):
-// a B200 has ~37 TFLOP/s of fp32 add/mul against 6.5 TB/s, and a 1440-point row is 34 kflop for 4.8 KB.  Here two of the three
-// radix stages (the 31 x 180 sub-transform, 86 % of the flops) run on the tensor pipe at TF32 and only one radix-8 stage stays on the
-// CUDA cores; no shared-memory exchange between stages is left.
+// Why: the Stockham kernels are issue-bound on the CUDA cores: a 1440-point row is 34 kflop for 4.8 KB, far above the fp32 FMA rate over
+// the HBM bandwidth of the GPU.  Here two of the three radix stages (the 31 x 180 sub-transform, 86 % of the flops) run on the tensor
+// pipe at TF32 and only one radix-8 stage stays on the CUDA cores; no shared-memory exchange between stages is left.
 //
-// synthesis kernel (latspec -> rows):   TMEM lane = column j2 (<= N2/2, replicated when N2/2 < 64 so that all four SM sub-partitions
-//   work), accumulator columns = (class c, latitude k) of an 8-row tile.  A = E^T resident in shared memory (32 KB), B = the raw
-//   latspec tile [m2][(c, k)] streamed by TMA (16 KB per 8 rows), four accumulators S1..S4 (cos/sin x re/im), double buffered.
-//   Epilogue warps: tcgen05.ld -> V(j2), V(N2-j2) -> twiddle -> radix-8 -> scale/bias -> bf16; a warp stores 32 consecutive
-//   longitudes of one row per instruction.
+// synthesis kernel (latspec -> rows):   D[j2][(class c, latitude k)] for the columns j2 <= N2/2 and an 8-row tile.  A = E^T resident in
+//   shared memory (32 KB), B = the raw latspec tile [m2][(c, k)] streamed by TMA (16 KB per 8 rows) through an mbarrier ring, four
+//   accumulators S1..S4 (cos/sin x re/im) in registers.  A warp owns 16 columns j2; its m16n8 fragments give each thread the two
+//   latitudes 2 (lane % 4), + 1 of the columns j2 = lane / 4 (+ 8) for all eight classes, i.e. the inputs of its own butterflies:
+//   S -> V(j2), V(N2-j2) -> twiddle -> radix-8 -> scale/bias -> bf16 without any exchange.
 // analysis kernel (rows -> latspec):    producer warps load the eight samples x[N2 j1 + j2] of a column (lanes = consecutive j2),
 //   butterfly + twiddle them and write the even/odd combinations (Ye, Yo) as K-major TF32 operand tiles [(c, k)][j2] (128-byte
-//   swizzle, conflict-free row stores); B = E resident (<= 24 KB); D[(c,k)][m2] in TMEM; epilogue scales and writes latspec
-//   (64-byte runs along k).
+//   swizzle, conflict-free row stores); B = E resident (<= 24 KB); four MMA warps accumulate D[(c,k)][m2] in registers over the K-blocks
+//   and write latspec straight from their fragments (32-byte runs along k).
 #include "umma_common.cuh"
 #include "dft_math.cuh"
 #include <cmath>
@@ -29,16 +28,17 @@ namespace b200sht {
 int umma_available();   // umma.cu
 
 constexpr int kDftMaxHalf = 95;    // N2 / 2 <= 95: three 32-lane quadrants (synthesis) / three K-blocks (analysis)
-constexpr int kDftSynThreads = 512;
+constexpr int kDftSynWorkers = 7;                        // MMA + epilogue warps of the synthesis kernel
+constexpr int kDftSynThreads = 32 * (kDftSynWorkers + 1);   // + one TMA warp
 constexpr int kDftSynStages = 8;   // 16 KB each
 
 struct DftTables {
-  float* et;      // synthesis A: [2][128 rows = lane -> j2][32 m2]  (cos, sin), TF32-rounded
+  float* et;      // synthesis A: [2][128 rows j2][32 m2]  (cos, sin), TF32-rounded; rows j2 > N2 / 2 are zero
   float* eb;      // analysis  B: [nkb][2][32 rows m2][32 j2 local]  (cos, sin), TF32-rounded
   float2* tw;     // [8][N2]  exp(+2 pi i c j2 / nlon)
   float* trash;   // 64 x (4 * nlon + 256) floats: store target of the synthesis rows / lanes without output (keeps the stores unconditional); one slab per CTA % 64
   float* zeros;   // 8 * N2 floats of zeros: load target of the analysis lanes / rows that carry no sample (keeps the loads unconditional)
-  int N2, half, M2, qpr, nrep, nkb;
+  int N2, half, M2, nkb;
 };
 
 bool dft_shape_ok(int nlon, int mmax) {
@@ -47,14 +47,13 @@ bool dft_shape_ok(int nlon, int mmax) {
   return N2 >= 2 && N2 / 2 <= kDftMaxHalf && (mmax + 7) / 8 <= 32 && mmax <= nlon / 2 + 1;
 }
 
-__global__ void dft_tables_kernel(float* et, float* eb, float2* tw, int N2, int half, int M2, int qpr, int nrep, int nkb, int nlon) {
+__global__ void dft_tables_kernel(float* et, float* eb, float2* tw, int N2, int half, int M2, int nkb, int nlon) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   // E^T tiles: [2][128][32]
   if (i < 2 * 128 * 32) {
-    const int m2 = i % 32, lane = (i / 32) % 128, p = i / (32 * 128);
-    const int rep = lane / (32 * qpr), j2 = lane - rep * 32 * qpr;
+    const int m2 = i % 32, j2 = (i / 32) % 128, p = i / (32 * 128);
     float v = 0.f;
-    if (rep < nrep && j2 <= half && m2 < M2) {
+    if (j2 <= half && m2 < M2) {
       const long long t = ((long long)m2 * j2) % N2;
       const double ang = 2.0 * M_PI * (double)t / (double)N2;
       v = tf32_rn((float)(p == 0 ? cos(ang) : sin(ang)));
@@ -86,9 +85,7 @@ int dft_plan_init(Plan* pl) {
   if (!dft_shape_ok(pl->nlon, pl->mmax)) return -1;
   DftTables* t = new DftTables();
   t->N2 = pl->nlon / 8; t->half = t->N2 / 2; t->M2 = (pl->mmax + 7) / 8;
-  t->qpr = (t->half + 1 + 31) / 32;
-  t->nrep = t->qpr == 1 ? 4 : (t->qpr == 2 ? 2 : 1);
-  t->nkb = t->qpr;
+  t->nkb = (t->half + 1 + 31) / 32;   // 32-column K-blocks of j2 = 0 .. N2 / 2 (analysis)
   t->et = nullptr; t->eb = nullptr; t->tw = nullptr; t->zeros = nullptr; t->trash = nullptr;
   const size_t neb = (size_t)t->nkb * 2 * 32 * 32;
   cudaError_t e = cudaMalloc(&t->et, sizeof(float) * 2 * 128 * 32);
@@ -99,7 +96,7 @@ int dft_plan_init(Plan* pl) {
   if (e == cudaSuccess) e = cudaMalloc(&t->trash, sizeof(float) * 64 * (4 * (size_t)pl->nlon + 256));   // + 256: idle lanes index up to j2 = 127 + 7 N2 past a row
   if (e == cudaSuccess) {
     const int n = 8192 > 8 * t->N2 ? 8192 : 8 * t->N2;
-    dft_tables_kernel<<<(n + 255) / 256, 256>>>(t->et, t->eb, t->tw, t->N2, t->half, t->M2, t->qpr, t->nrep, t->nkb, pl->nlon);
+    dft_tables_kernel<<<(n + 255) / 256, 256>>>(t->et, t->eb, t->tw, t->N2, t->half, t->M2, t->nkb, pl->nlon);
     e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(0);
   }
@@ -129,8 +126,8 @@ bool dft_usable(const Plan* pl) { return pl->dft_state != nullptr && dft_enabled
 // ----------------------------------------------------------------------------------------- wait-time profile
 // B200SHT_DFT_PROF=1: every role accumulates the SM clocks it spends in its mbarrier waits (one atomic per wait, lane 0 of the warp) into 16
 // counters, read back and cleared by b200sht_debug_dft_profile().  Slots -- analysis: 0 producers / raw samples, 1 producers / operand stage free,
-// 2 loader / raw stage free, 3 MMA / operand stage full, 4 MMA / accumulator free, 5 epilogue / accumulator full, 6 CTA lifetime, 7 producer items;
-// synthesis: 8 TMA / stage free, 9 MMA / stage full, 10 MMA / accumulator free, 11 epilogue / accumulator full, 12 CTA lifetime, 13 epilogue tiles.
+// 2 loader / raw stage free, 3 MMA warps / operand stage full, 5 MMA-warp tiles, 6 CTA lifetime, 7 producer items; synthesis: 8 TMA / stage free,
+// 9 MMA warps / stage full, 12 CTA lifetime, 13 MMA-warp tiles.
 static unsigned long long* g_dft_prof = nullptr;
 static unsigned long long* dft_prof_buffer() {
   static const int on = [] { const char* e = getenv("B200SHT_DFT_PROF"); return e ? atoi(e) : 0; }();
@@ -160,26 +157,6 @@ __device__ __forceinline__ void prof_wait(unsigned long long* prof, int slot, ui
   if (lead) atomicAdd(prof + slot, (unsigned long long)(clock64() - t0));
 }
 
-// ------------------------------------------------------------------------------------------------ small PTX
-__device__ __forceinline__ pr tmem_ld2(uint32_t taddr) {
-  uint32_t a, b;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0, %1}, [%2];" : "=r"(a), "=r"(b) : "r"(taddr) : "memory");
-  return make_pr(__uint_as_float(a), __uint_as_float(b));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, "
-      "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-        "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
 template <typename T> __device__ __forceinline__ void st_out(T* p, float v);
 template <> __device__ __forceinline__ void st_out<float>(float* p, float v) { *p = v; }
 template <> __device__ __forceinline__ void st_out<__nv_bfloat16>(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
@@ -188,8 +165,8 @@ template <typename T> __device__ __forceinline__ uint32_t ld_raw(const T* p);
 template <> __device__ __forceinline__ uint32_t ld_raw<float>(const float* p) { return __float_as_uint(__ldg(p)); }
 template <> __device__ __forceinline__ uint32_t ld_raw<__nv_bfloat16>(const __nv_bfloat16* p) { return (uint32_t)__ldg(reinterpret_cast<const unsigned short*>(p)); }
 
-// How the CUDA-core producers turn an fp32 value into a kind::tf32 operand (the MMA truncates the 13 low mantissa bits):
-//   0  cvt.rna.tf32.f32                 3 instructions on sm_100a (FSETP + IADD + LOP3)
+// How the CUDA-core producers turn an fp32 value into a TF32 operand (the MMA ignores the 13 low mantissa bits):
+//   0  cvt.rna.tf32.f32                 3 instructions (FSETP + IADD + LOP3)
 //   1  (bits + 0x1000) & ~0x1fff        2 instructions, same result for finite values
 //   2  bias-compensated truncation      0 instructions: the value is pre-scaled by (1 + 2^-10 / 3) -- folded into the twiddle
 //      factors -- so that the hardware truncation error x f - delta, delta ~ U[0, ulp), has zero mean over a binade; its rms is
@@ -241,12 +218,14 @@ struct DftSynParams {
   const float* bias;
   void* trash;
   unsigned long long* prof;
-  int R, C, nlat, nlon, kp, mmax, N2, half, M2, qpr, nrep, mode, ntiles, ktiles, has_nyq;
+  int R, C, nlat, nlon, kp, mmax, N2, half, M2, mode, ntiles, ktiles, has_nyq;
   int kt0, kt_all;   // latitude range of this launch: first 8-row tile, tiles per image in the whole tensor (ktiles = tiles per image in the range)
-  uint32_t idesc;
 };
 
 // shared memory: [A: cos 16 KB | sin 16 KB][B ring: kDftSynStages x 16 KB][tw table 8 x N2 float2][barriers]
+// warps 0..6: MMA + epilogue, in groups of `nmt` warps (one per 16 columns j2 <= N2 / 2); group i takes the tiles i, i + ngroups, ... of this
+// CTA.  Warp 7: TMA.  The m16n8 accumulator fragment of a warp holds, per thread, the columns j2 = 16 mt + lane / 4 (+ 8) and the latitude pair
+// 2 (lane % 4), + 1 for all eight classes: exactly the inputs of the radix-8 epilogue of those two columns.
 template <typename T, int N2T>
 __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const __grid_constant__ DftSynParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -261,33 +240,25 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
   uint64_t* bars = reinterpret_cast<uint64_t*>(gbase + 32768 + kDftSynStages * 16384 + ((8 * p.N2 * 8 + 15) & ~15));
   uint64_t* full = bars;
   uint64_t* empty = full + kDftSynStages;
-  uint64_t* acc_full = empty + kDftSynStages;
-  uint64_t* acc_empty = acc_full + 2;
-  uint64_t* e_full = acc_empty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(e_full + 1);
+  uint64_t* e_full = empty + kDftSynStages;
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
   pdl_trigger();
-  const int quad = warp & 3, sub = warp >> 2;
-  const int subs = 4 / p.nrep;                                  // k pairs per replica
-  const bool is_tma = (warp == 15), is_mma = (warp == 11);
-  const bool is_epi = !is_tma && !is_mma && quad < p.qpr * p.nrep && sub < subs;
-  const int n_epi = p.qpr * p.nrep * subs;
+  const int nmt = (p.half + 16) / 16;          // 16-column blocks of j2 = 0 .. N2 / 2
+  const int ngroups = kDftSynWorkers / nmt;
+  const bool is_tma = (warp == kDftSynWorkers);
+  const int grp = warp / nmt, mt = warp - grp * nmt;
+  const bool is_work = !is_tma && grp < ngroups;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kDftSynStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], n_epi); }
+    for (int s = 0; s < kDftSynStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], nmt); }
     mbar_init(e_full, 1);
     fence_barrier_init();
     prefetch_tmap(&p.tmZ);
     prefetch_tmap(&p.tmE);
   }
   for (int i = threadIdx.x; i < 8 * p.N2; i += blockDim.x) tws[i] = p.tw[i];
-  if (is_mma) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   const long long t_cta0 = (kDftProfile && p.prof && threadIdx.x == 0) ? clock64() : 0;
   pdl_wait();   // the prologue read plan constants only (twiddles); the latspec tiles, bias and y belong to other kernels until here
 
@@ -310,59 +281,23 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
       }
     }
     __syncwarp();
-  } else if (is_mma) {
-    {   // all 32 lanes run the loop (converged); the MMAs / commits are issued by an elected lane (umma_*_ws)
-      mbar_wait(e_full, 0);
-      const uint64_t dE0 = desc_kmajor(sA, 0), dZ0 = desc_mnmajor(sB, 0, 4096);
-      int n = 0;
-      for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
-        const int s = n % kDftSynStages, it = n / kDftSynStages;
-        const int buf = n & 1, use = n >> 1;
-        if (use > 0) { prof_wait(prof, 10, &acc_empty[buf], (use - 1) & 1, lane == 0); }
-        prof_wait(prof, 9, &full[s], it & 1, lane == 0);
-        tc_fence_after();
-        const uint64_t z0 = desc_advance(dZ0, (uint32_t)s * 16384u);
-        const uint32_t d = tmem + buf * 256;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const uint64_t ac = desc_advance(dE0, 32 * j), as = desc_advance(dE0, 16384 + 32 * j);
-          const uint64_t zr = desc_advance(z0, 1024 * j), zi = desc_advance(z0, 8192 + 1024 * j);
-          const uint32_t acc = j > 0 ? 1u : 0u;
-          umma_tf32_ws(d, ac, zr, p.idesc, acc);          // S1 = cos . Zr
-          umma_tf32_ws(d + 64, as, zi, p.idesc, acc);     // S2 = sin . Zi
-          umma_tf32_ws(d + 128, as, zr, p.idesc, acc);    // S3 = sin . Zr
-          umma_tf32_ws(d + 192, ac, zi, p.idesc, acc);    // S4 = cos . Zi
-        }
-        umma_commit_ws(&empty[s]);
-        umma_commit_ws(&acc_full[buf]);
-      }
-    }
-    __syncwarp();
-  } else if (is_epi) {
+  } else if (is_work) {
     const int N2 = N2T > 0 ? N2T : p.N2;
     const int nlon = 8 * N2;
-    const int rep = quad / p.qpr;
-    const int j2 = 32 * (quad - rep * p.qpr) + lane;
-    const bool valid = j2 <= p.half;
-    const bool paired = valid && j2 != 0 && 2 * j2 != N2;
-    const int jp = N2 - j2;
-    const int kpi = rep * subs + sub;
+    const int kpi = lane & 3;
     const bool n2odd = (N2 & 1) != 0;
     T* const y = static_cast<T*>(p.y);
     const float smul = p.mode == 0 ? 2.f : 1.f;
     const int nyq_m = nlon / 2;
     T* const trash = static_cast<T*>(p.trash) + (size_t)(blockIdx.x & 63) * (4 * nlon + 256);
-    float2 tw[8], tp[8];
-    tw[0] = make_float2(1.f, 0.f);
-#pragma unroll
-    for (int c = 1; c < 8; ++c) tw[c] = valid ? tws[c * N2 + j2] : make_float2(1.f, 0.f);
-    dft_partner_twiddles(tw, tp);
-    int n = 0;
-    for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
+    const uint8_t* const gE = gbase;
+    mbar_wait(e_full, 0);
+    int n = grp;
+    for (int ti = blockIdx.x + grp * gridDim.x; ti < p.ntiles; ti += ngroups * gridDim.x, n += ngroups) {
       const int r = ti / p.ktiles, k0 = (p.kt0 + ti - r * p.ktiles) * 8;
       const int ta = r * p.kt_all + p.kt0 + (ti - r * p.ktiles);   // tile index in the whole tensor
       const int ka = k0 + 2 * kpi;
-      const int buf = n & 1, use = n >> 1;
+      const int s = n % kDftSynStages, it = n / kDftSynStages;
       // per-row output factors:  out = x * sc + off(parity of the longitude)
       float rsa = 1.f, rsb = 1.f, z0a = 0.f, z0b = 0.f, zna = 0.f, znb = 0.f;
       if (p.mode == 1) {
@@ -382,66 +317,91 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
       const pr sc = make_pr(smul * rsa, smul * rsb);
       const pr off_e = make_pr(bias - rsa * (z0a + zna), bias - rsb * (z0b + znb));   // even longitude j
       const pr off_o = make_pr(bias - rsa * (z0a - zna), bias - rsb * (z0b - znb));   // odd longitude j
-      prof_wait(prof, 11, &acc_full[buf], use & 1, lane == 0);
+      prof_wait(prof, 9, &full[s], it & 1, lane == 0);
       if (prof && lane == 0) atomicAdd(prof + 13, 1ull);
-      tc_fence_after();
-      const uint32_t t0 = tmem + ((uint32_t)(quad * 32) << 16) + buf * 256 + 2 * kpi;
-      // rows beyond nlat (last tile of an image) are stored into a scratch row: no predicates / branches around the 32 stores
-      T* const pa = (valid && ka < p.nlat) ? y + ((size_t)r * p.nlat + ka) * nlon + j2 : trash + j2;
-      T* const pb = (valid && ka + 1 < p.nlat) ? y + ((size_t)r * p.nlat + ka + 1) * nlon + j2 : trash + nlon + j2;
-      const int dq = paired ? jp - j2 : 0;
-      // The four accumulators are read twice (TMEM reads are cheap) and reduced to V of one column right away, so that only 16 register
-      // pairs are live through each radix-8 pass: holding S1..S4 (64 registers) next to the twiddles made ptxas rematerialise the
-      // 64-bit store address for every one of the 32 stores (10 instructions each).
+      // S1 = cos . Zr, S2 = sin . Zi, S3 = sin . Zr, S4 = cos . Zi over the 32 orders m2 of the tile; rows j2, columns (class c, latitude)
+      float acc[4][8][4];
+#pragma unroll
+      for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int c = 0; c < 8; ++c) acc[a][c][0] = acc[a][c][1] = acc[a][c][2] = acc[a][c][3] = 0.f;
       {
-        pr vr[8], vi[8], x[8];
+        const uint8_t* const zs = gbase + 32768 + (size_t)s * 16384;
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const pr a1 = tmem_ld2(t0 + c * 8), a2 = tmem_ld2(t0 + 64 + c * 8), a3 = tmem_ld2(t0 + 128 + c * 8), a4 = tmem_ld2(t0 + 192 + c * 8);
-          tmem_ld_wait();
-          vr[c] = a1 - a2;
-          vi[c] = a3 + a4;
-        }
-        dft_syn_radix8<pr>(vr, vi, tw, x);
-        const pr o0 = (j2 & 1) ? off_o : off_e, o1 = (j2 & 1) ? off_e : off_o;
+        for (int kk = 0; kk < 32; kk += 8) {
+          uint32_t fc[4], fs[4];
+          frag_a<false>(gE, 16 * mt, kk, fc);
+          frag_a<false>(gE + 16384, 16 * mt, kk, fs);
 #pragma unroll
-        for (int j1 = 0; j1 < 8; ++j1) {
-          const pr o = rfma(x[j1], sc, (n2odd && (j1 & 1)) ? o1 : o0);
-          st_out<T>(pa + N2 * j1, o.v.x);
-          st_out<T>(pb + N2 * j1, o.v.y);
+          for (int c = 0; c < 8; ++c) {
+            uint32_t zr[2], zi[2];
+            frag_b<true>(zs, 8 * c, kk, zr);
+            frag_b<true>(zs + 8192, 8 * c, kk, zi);
+            mma_tf32(acc[0][c], fc, zr);
+            mma_tf32(acc[1][c], fs, zi);
+            mma_tf32(acc[2][c], fs, zr);
+            mma_tf32(acc[3][c], fc, zi);
+          }
         }
       }
-      {
-        pr vr[8], vi[8], x[8];
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);   // this warp's reads of the stage are done
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const pr a1 = tmem_ld2(t0 + c * 8), a2 = tmem_ld2(t0 + 64 + c * 8), a3 = tmem_ld2(t0 + 128 + c * 8), a4 = tmem_ld2(t0 + 192 + c * 8);
-          tmem_ld_wait();
-          vr[c] = a1 + a2;
-          vi[c] = a4 - a3;
+      for (int h = 0; h < 2; ++h) {
+        const int j2 = 16 * mt + (lane >> 2) + 8 * h;
+        const bool valid = j2 <= p.half;
+        const bool paired = valid && j2 != 0 && 2 * j2 != N2;
+        const int jp = N2 - j2;
+        float2 tw[8], tp[8];
+        tw[0] = make_float2(1.f, 0.f);
+#pragma unroll
+        for (int c = 1; c < 8; ++c) tw[c] = valid ? tws[c * N2 + j2] : make_float2(1.f, 0.f);
+        dft_partner_twiddles(tw, tp);
+        // rows beyond nlat (last tile of an image) are stored into a scratch row: no predicates / branches around the 32 stores
+        T* const pa = (valid && ka < p.nlat) ? y + ((size_t)r * p.nlat + ka) * nlon + j2 : trash + j2;
+        T* const pb = (valid && ka + 1 < p.nlat) ? y + ((size_t)r * p.nlat + ka + 1) * nlon + j2 : trash + nlon + j2;
+        const int dq = paired ? jp - j2 : 0;
+        {
+          pr vr[8], vi[8], x[8];
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            vr[c] = make_pr(acc[0][c][2 * h], acc[0][c][2 * h + 1]) - make_pr(acc[1][c][2 * h], acc[1][c][2 * h + 1]);
+            vi[c] = make_pr(acc[2][c][2 * h], acc[2][c][2 * h + 1]) + make_pr(acc[3][c][2 * h], acc[3][c][2 * h + 1]);
+          }
+          dft_syn_radix8<pr>(vr, vi, tw, x);
+          const pr o0 = (j2 & 1) ? off_o : off_e, o1 = (j2 & 1) ? off_e : off_o;
+#pragma unroll
+          for (int j1 = 0; j1 < 8; ++j1) {
+            const pr o = rfma(x[j1], sc, (n2odd && (j1 & 1)) ? o1 : o0);
+            st_out<T>(pa + N2 * j1, o.v.x);
+            st_out<T>(pb + N2 * j1, o.v.y);
+          }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[buf]);   // both reads done: release the accumulator set
-        dft_syn_radix8<pr>(vr, vi, tp, x);
-        T* const qa = paired ? pa + dq : trash + 2 * nlon + j2;     // unpaired columns (j2 = 0, N2 / 2) and idle lanes: scratch
-        T* const qb = paired ? pb + dq : trash + 3 * nlon + j2;
-        const pr o0 = (jp & 1) ? off_o : off_e, o1 = (jp & 1) ? off_e : off_o;
+        {
+          pr vr[8], vi[8], x[8];
 #pragma unroll
-        for (int j1 = 0; j1 < 8; ++j1) {
-          const pr o = rfma(x[j1], sc, (n2odd && (j1 & 1)) ? o1 : o0);
-          st_out<T>(qa + N2 * j1, o.v.x);
-          st_out<T>(qb + N2 * j1, o.v.y);
+          for (int c = 0; c < 8; ++c) {
+            vr[c] = make_pr(acc[0][c][2 * h], acc[0][c][2 * h + 1]) + make_pr(acc[1][c][2 * h], acc[1][c][2 * h + 1]);
+            vi[c] = make_pr(acc[3][c][2 * h], acc[3][c][2 * h + 1]) - make_pr(acc[2][c][2 * h], acc[2][c][2 * h + 1]);
+          }
+          dft_syn_radix8<pr>(vr, vi, tp, x);
+          T* const qa = paired ? pa + dq : trash + 2 * nlon + j2;     // unpaired columns (j2 = 0, N2 / 2) and idle rows: scratch
+          T* const qb = paired ? pb + dq : trash + 3 * nlon + j2;
+          const pr o0 = (jp & 1) ? off_o : off_e, o1 = (jp & 1) ? off_e : off_o;
+#pragma unroll
+          for (int j1 = 0; j1 < 8; ++j1) {
+            const pr o = rfma(x[j1], sc, (n2odd && (j1 & 1)) ? o1 : o0);
+            st_out<T>(qa + N2 * j1, o.v.x);
+            st_out<T>(qb + N2 * j1, o.v.y);
+          }
         }
       }
     }
   }
-  tc_fence_before();
   __syncthreads();
   if (kDftProfile && p.prof && threadIdx.x == 0) prof_s[12] = (unsigned long long)(clock64() - t_cta0);
   if (kDftProfile) __syncthreads();
   if (kDftProfile && p.prof && threadIdx.x < 16) atomicAdd(p.prof + threadIdx.x, prof_s[threadIdx.x]);
-  if (is_mma) tmem_dealloc(tmem, 512);
 }
 
 // k_begin / k_end: latitude range [k_begin, k_end) to produce (k_begin a multiple of 8; k_end < 0: all rows) -- the other rows of y are not touched
@@ -453,20 +413,19 @@ int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int
   memset(&p, 0, sizeof(p));
   p.Z = Z; p.y = y; p.tw = t->tw; p.rowscale = pl->d_rowscale; p.bias = bias; p.trash = t->trash; p.prof = dft_prof_buffer();
   p.R = R; p.C = C; p.nlat = pl->nlat; p.nlon = pl->nlon; p.kp = pl->kp; p.mmax = pl->mmax;
-  p.N2 = t->N2; p.half = t->half; p.qpr = t->qpr; p.nrep = t->nrep; p.mode = mode;
+  p.N2 = t->N2; p.half = t->half; p.mode = mode;
   if (k_end < 0 || k_end > pl->kp) k_end = pl->kp;
   B200_REQUIRE(k_begin >= 0 && k_begin % 8 == 0 && k_begin < k_end, "dft_synthesis: bad latitude range [%d, %d)", k_begin, k_end);
   p.kt_all = pl->kp / 8; p.kt0 = k_begin / 8;
   p.ktiles = (k_end - k_begin + 7) / 8; p.ntiles = R * p.ktiles;
   p.has_nyq = (pl->mmax == pl->nlon / 2 + 1) ? 1 : 0;
-  p.idesc = make_idesc(64, 0, 1, 0);
   p.M2 = t->M2;
   {
     // tiled latspec (written by legendre_synthesis_umma(tiled = 1)): [tile = r * ktiles + k / 8][plane][m2][c = m % 8][k % 8]; a tile is 16 KB
     // contiguous, the 128-byte rows of the TMA box are (4 classes x 8 latitudes) of one m2: the MN-major B operand, N = (c, k)
     long long d[5] = {32, 2, t->M2, 2, (long long)R * (pl->kp / 8)}, s[5] = {1, 32, 64, (long long)t->M2 * 64, 2ll * t->M2 * 64};
     int bx[5] = {32, 1, 32, 1, 1};
-    int rc = make_tmap(&p.tmZ, Z, 5, d, s, bx, true);
+    int rc = make_tmap(&p.tmZ, Z, 5, d, s, bx);
     if (rc) return rc;
   }
   {
@@ -475,8 +434,8 @@ int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int
     int rc = make_tmap(&p.tmE, t->et, 2, d, s, bx);
     if (rc) return rc;
   }
-  const size_t smem = 1024 + 32768 + (size_t)kDftSynStages * 16384 + ((8 * (size_t)t->N2 * 8 + 15) & ~(size_t)15) + (2 * kDftSynStages + 5) * 8 + 16;
-  const int sms = usable_sms(pl->sm_count > 0 ? pl->sm_count : 148);
+  const size_t smem = 1024 + 32768 + (size_t)kDftSynStages * 16384 + ((8 * (size_t)t->N2 * 8 + 15) & ~(size_t)15) + (2 * kDftSynStages + 1) * 8;
+  const int sms = usable_sms(pl->sm_count > 0 ? pl->sm_count : 132);
   const int ctas = p.ntiles < sms ? p.ntiles : sms;
 #define B200_LAUNCH_SYN(TT, NN)                                                                                                          \
   do {                                                                                                                                  \
@@ -540,18 +499,17 @@ struct DftAnaParams {
   unsigned long long* prof;
   int R, nlat, nlon, kp, mmax, N2, half, M2, nkb, mode, round_tf32, ntiles, ktiles, nraw, gs;
   int kt0;   // first 16-row tile of the latitude range this launch transforms (ktiles = tiles in the range; latitude-chunked analysis, capi.cu)
-  uint32_t idesc, idesc_neg;
 };
 
-// warps: 0..3 epilogue (TMEM quadrant = warp), 4 MMA issuer (+ TMEM owner, loads the resident B), 5 sample loader (TMA), 6.. producers
+// warps: 0..3 MMA + epilogue (rows 32 w .. + 31 of the tile = classes 2 w, 2 w + 1), 4 loads the resident B, 5 sample loader (TMA), 6.. producers
 // shared memory: [B resident: nkb x (cos 4 KB | sin 4 KB)][A ring: 2 x 4 planes x 16 KB][raw ring: nraw x 16 boxes][twiddles][barriers]
 //
 // Data flow of one (tile, K-block): the loader thread brings the 8 + 8 sample boxes the K-block needs -- for each j1 the 32 columns
 // j2 = 32 kb .. + 31 and their 32 partner columns N2 - j2, 16 rows each -- into a raw stage with 16 TMA boxes (deep asynchronous prefetch,
 // no registers: the first version's LDG -> register path stalled 2.1 cycles per issued instruction on the loads, with the 96-register cap
 // allowing only half an item of prefetch).  Eight producer warps (one row pair each) read their samples with LDS, run the two radix-8
-// butterflies + twiddles with the two rows packed in f32x2, and write Ye / Yo of the 8 classes into the operand stage; then the MMA thread
-// contracts the stage with E.  N2T > 0: nlon / 8 as a compile-time constant.
+// butterflies + twiddles on the two rows of a pair, and write Ye / Yo of the 8 classes into the operand stage; then the MMA warps contract
+// the stage with E.  N2T > 0: nlon / 8 as a compile-time constant.
 template <typename T, int N2T>
 __global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_constant__ DftAnaParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -575,12 +533,9 @@ __global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_const
   float2* twS = reinterpret_cast<float2*>(gbase + oT);   // [nkb][7][32] twiddles of the producer lanes
   uint64_t* full = reinterpret_cast<uint64_t*>(gbase + oBar);
   uint64_t* empty = full + kDftAnaStages;
-  uint64_t* acc_full = empty + kDftAnaStages;
-  uint64_t* acc_empty = acc_full + 4;
-  uint64_t* raw_full = acc_empty + 4;
+  uint64_t* raw_full = empty + kDftAnaStages;
   uint64_t* raw_empty = raw_full + 4;
   uint64_t* b_full = raw_empty + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(b_full + 1);
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
   pdl_trigger();
@@ -599,8 +554,7 @@ __global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_const
     twS[i] = w;
   }
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kDftAnaStages; ++s) { mbar_init(&full[s], 8); mbar_init(&empty[s], 1); }   // a K-block = 8 row pairs, one arrival each
-    for (int b = 0; b < 4; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 4); }
+    for (int s = 0; s < kDftAnaStages; ++s) { mbar_init(&full[s], 8); mbar_init(&empty[s], 4); }   // a K-block = 8 row pairs; 4 MMA warps
     for (int s = 0; s < p.nraw; ++s) { mbar_init(&raw_full[s], 1); mbar_init(&raw_empty[s], 8); }
     mbar_init(b_full, 1);
     fence_barrier_init();
@@ -613,12 +567,7 @@ __global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_const
     const int st = i >> 10, pl = (i >> 9) & 1, off = i & 511;
     reinterpret_cast<float*>(gA + (size_t)st * 65536)[(pl ? 12288 : 4096) + off] = 0.f;
   }
-  fence_proxy_async();
-  if (warp == 4) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   const long long t_cta0 = (kDftProfile && p.prof && threadIdx.x == 0) ? clock64() : 0;
   pdl_wait();   // the prologue read plan constants only (twiddles); samples and latspec belong to other kernels until here
 
@@ -628,36 +577,6 @@ __global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_const
       for (int kb = 0; kb < nkb; ++kb) {
         tma_load_2d(sBm + kb * 8192, &p.tmB, b_full, 0, kb * 64);
         tma_load_2d(sBm + kb * 8192 + 4096, &p.tmB, b_full, 0, kb * 64 + 32);
-      }
-    }
-    __syncwarp();
-    {   // all 32 lanes run the loop (converged); the MMAs / commits are issued by an elected lane (umma_*_ws)
-      mbar_wait(b_full, 0);
-      const uint64_t dA0 = desc_kmajor(sAr, 0), dB0 = desc_kmajor(sBm, 0);   // every other descriptor = one of these + a byte offset
-      int n = 0;
-      for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
-        const int buf = n & 3, use = n >> 2;
-        if (use > 0) prof_wait(prof, 4, &acc_empty[buf], (use - 1) & 1, lane == 0);
-        tc_fence_after();
-        const uint32_t d = tmem + buf * 64;
-        for (int kb = 0; kb < nkb; ++kb) {
-          const int g = n * nkb + kb, s = g % kDftAnaStages, it = g / kDftAnaStages;
-          prof_wait(prof, 3, &full[s], it & 1, lane == 0);   // precise wake-up: the stage is released (empty) only after these MMAs
-          tc_fence_after();
-          const uint64_t a0 = desc_advance(dA0, (uint32_t)s * 65536u);
-          const uint64_t bc = desc_advance(dB0, (uint32_t)kb * 8192u), bs = desc_advance(bc, 4096);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint32_t acc = (kb > 0 || j > 0) ? 1u : 0u;
-            const uint64_t bcj = desc_advance(bc, 32 * j), bsj = desc_advance(bs, 32 * j);
-            umma_tf32_ws(d, desc_advance(a0, 32 * j), bcj, p.idesc, acc);                       // Xre  = Ye_r cos
-            umma_tf32_ws(d, desc_advance(a0, 49152 + 32 * j), bsj, p.idesc, 1u);               // Xre += Yo_i sin
-            umma_tf32_ws(d + 32, desc_advance(a0, 16384 + 32 * j), bcj, p.idesc, acc);         // Xim  = Ye_i cos
-            umma_tf32_ws(d + 32, desc_advance(a0, 32768 + 32 * j), bsj, p.idesc_neg, 1u);      // Xim -= Yo_r sin
-          }
-          umma_commit_ws(&empty[s]);
-        }
-        umma_commit_ws(&acc_full[buf]);
       }
     }
     __syncwarp();
@@ -685,49 +604,83 @@ __global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_const
     }
     __syncwarp();
   } else if (warp < 4) {
-    // ------------------------------------------------------------------------------------------- epilogue
-    const int c = 2 * warp + (lane >> 4), kr = lane & 15;
+    // ------------------------------------------------------------------------------------------- MMA + epilogue
+    // D[(c, kr)][m2] = Xre: Ye_r cos + Yo_i sin,  Xim: Ye_i cos - Yo_r sin over the j2 of all K-blocks.  m16 tile mt of this warp is class
+    // c = 2 warp + mt, its fragment rows are the latitudes kr = lane / 4 (+ 8), its columns the orders m2 = 8 j + 2 (lane % 4) (+ 1).
     const size_t plane = (size_t)p.R * p.kp;
+    const float tcomp = p.round_tf32 ? kTruncComp : 1.f;
+    mbar_wait(b_full, 0);
     int n = 0;
     for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
       const int r = ti / p.ktiles, k0 = (p.kt0 + ti - r * p.ktiles) * 16;
-      const int k = k0 + kr;
-      const int buf = n & 3, use = n >> 2;
-      const bool kok = k < p.kp;
-      const float rs = (p.mode == 0) ? ((k < p.nlat) ? __ldg(p.rowscale + k) : 0.f) : 1.f;
-      const float tcomp = p.round_tf32 ? kTruncComp : 1.f;
-      {
-        const long long tw0 = prof ? clock64() : 0;
-        mbar_wait_relaxed(&acc_full[buf], use & 1, 1000);
-        if (prof && lane == 0) atomicAdd(prof + 5, (unsigned long long)(clock64() - tw0));
-      }
-      tc_fence_after();
-      float vr[32], vi[32];
-      const uint32_t t0 = tmem + ((uint32_t)(warp * 32) << 16) + buf * 64;
-      tmem_ld32_nowait(t0, vr);
-      tmem_ld32_nowait(t0 + 32, vi);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
-      if (!kok) continue;
-      float* xb = p.X + (size_t)r * p.kp + k;
+      float xr[2][4][4], xi[2][4][4];
 #pragma unroll
-      for (int m2 = 0; m2 < 32; ++m2) {
-        const int m = c + 8 * m2;
-        if (m >= p.mmax) break;
-        // round_tf32: the consumer is the kind::tf32 Legendre GEMM, which truncates its operands -> bias-compensated truncation folded
-        // into the scale factor (see B200_DFT_TF32_MODE above) instead of 3 instructions of cvt.rna per value
-        const float sc = ((p.mode == 0) ? rs : ((m == 0 || 2 * m == p.nlon) ? 1.f : 2.f)) * tcomp;
-        const float a = vr[m2] * sc, b = vi[m2] * sc;
-        float* dst = xb + (size_t)m * 2 * plane;
-        dst[0] = a;
-        dst[plane] = b;
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) { xr[mt][j][e] = 0.f; xi[mt][j][e] = 0.f; }
+      for (int kb = 0; kb < nkb; ++kb) {
+        const int g = n * nkb + kb, s = g % kDftAnaStages, it = g / kDftAnaStages;
+        prof_wait(prof, 3, &full[s], it & 1, lane == 0);
+        const uint8_t* const a0 = gA + (size_t)s * 65536;
+        const uint8_t* const bc = gbase + oB + kb * 8192;
+        const uint8_t* const bs = bc + 4096;
+#pragma unroll
+        for (int kk = 0; kk < 32; kk += 8) {
+          uint32_t fc[4][2], fs[4][2];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) { frag_b<false>(bc, 8 * j, kk, fc[j]); frag_b<false>(bs, 8 * j, kk, fs[j]); }
+#pragma unroll
+          for (int mt = 0; mt < 2; ++mt) {
+            const int row0 = 32 * warp + 16 * mt;
+            uint32_t er[4], ei[4], orr[4], oi[4];
+            frag_a<false>(a0, row0, kk, er);
+            frag_a<false>(a0 + 16384, row0, kk, ei);
+            frag_a<false>(a0 + 32768, row0, kk, orr);
+            frag_a<false>(a0 + 49152, row0, kk, oi);
+            frag_neg(orr, orr);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              mma_tf32(xr[mt][j], er, fc[j]);
+              mma_tf32(xr[mt][j], oi, fs[j]);
+              mma_tf32(xi[mt][j], ei, fc[j]);
+              mma_tf32(xi[mt][j], orr, fs[j]);
+            }
+          }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);   // this warp's reads of the stage are done
+      }
+      if (prof && lane == 0) atomicAdd(prof + 5, 1ull);
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt) {
+        const int c = 2 * warp + mt;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int k = k0 + (lane >> 2) + 8 * h;
+          if (k >= p.kp) continue;
+          const float rs = (p.mode == 0) ? ((k < p.nlat) ? __ldg(p.rowscale + k) : 0.f) : 1.f;
+          float* xb = p.X + (size_t)r * p.kp + k;
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int m = c + 8 * (8 * j + 2 * (lane & 3) + e);
+              if (m >= p.mmax) continue;
+              // round_tf32: the consumer is the TF32 Legendre GEMM, which truncates its operands -> bias-compensated truncation folded
+              // into the scale factor (see B200_DFT_TF32_MODE above) instead of 3 instructions of cvt.rna per value
+              const float sc = ((p.mode == 0) ? rs : ((m == 0 || 2 * m == p.nlon) ? 1.f : 2.f)) * tcomp;
+              float* dst = xb + (size_t)m * 2 * plane;
+              dst[0] = xr[mt][j][2 * h + e] * sc;
+              dst[plane] = xi[mt][j][2 * h + e] * sc;
+            }
+        }
       }
     }
   } else {
     // ------------------------------------------------------------------------------------------- producers
-    // Work item = (K-block kb, row pair q): rows 2q, 2q + 1 of the tile in the halves of packed f32x2 registers, lanes = the 32 columns of the
+    // Work item = (K-block kb, row pair q): rows 2q, 2q + 1 of the tile in the halves of register pairs (pr), lanes = the 32 columns of the
     // K-block.  Items are taken in K-block-major order (item = kb * 8 + q; warp w does w, w + nprod, ...): the MMAs of K-block kb run while
     // the warps work on kb + 1.  12 producer warps for three K-blocks (2 items per warp and tile), 8 otherwise: the kernel is bound by the
     // latency of the dependent butterfly chains, so the tile time is (items per warp) x (item latency).
@@ -823,12 +776,10 @@ __global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_const
       }
     }
   }
-  tc_fence_before();
   __syncthreads();
   if (kDftProfile && p.prof && threadIdx.x == 0) prof_s[6] = (unsigned long long)(clock64() - t_cta0);
   if (kDftProfile) __syncthreads();
   if (kDftProfile && p.prof && threadIdx.x < 16) atomicAdd(p.prof + threadIdx.x, prof_s[threadIdx.x]);
-  if (warp == 4) tmem_dealloc(tmem, 256);
 }
 
 // k_begin / k_end: latitude range [k_begin, k_end) to transform (k_begin a multiple of 16; k_end < 0: up to kp) -- the other rows of X are not touched
@@ -847,8 +798,6 @@ int dft_analysis(const Plan* pl, const void* x, int dtype, int B, int C, float* 
   p.ktiles = (k_end - k_begin + 15) / 16; p.ntiles = R * p.ktiles;
   const bool bf16 = (dtype == B200SHT_BF16);
   p.nraw = bf16 ? 3 : 2;   // raw stages of 20 / 34 KB
-  p.idesc = make_idesc(32, 0, 0, 0);
-  p.idesc_neg = make_idesc(32, 0, 0, 1);
   {
     long long d[2] = {32, (long long)t->nkb * 64}, s[2] = {1, 32};
     int bx[2] = {32, 32};
@@ -864,7 +813,7 @@ int dft_analysis(const Plan* pl, const void* x, int dtype, int B, int C, float* 
   }
   const size_t raw_bytes = bf16 ? (size_t)8 * 16 * (40 + 40) * 2 : (size_t)8 * 16 * (32 + 36) * 4;
   const size_t smem = 1024 + 3 * 8192 + (size_t)kDftAnaStages * 65536 + p.nraw * raw_bytes + 3 * 7 * 32 * 8 + 256;
-  const int sms = usable_sms(pl->sm_count > 0 ? pl->sm_count : 148);
+  const int sms = usable_sms(pl->sm_count > 0 ? pl->sm_count : 132);
   const int ctas = p.ntiles < sms ? p.ntiles : sms;
   const int threads = 32 * (6 + (t->nkb == 3 ? 12 : 8));
 #define B200_LAUNCH_ANA(TT, NN)                                                                                                          \

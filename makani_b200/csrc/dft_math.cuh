@@ -1,6 +1,6 @@
 // Radix-8 stage of the tensor-core longitude DFT (dft.cu), written once for three value types:
 //   float   host emulation (b200sht_debug_dft_host) and scalar device code
-//   pr      the same quantity of TWO latitude rows in one 64-bit register pair: packed FADD2 / FMUL2 / FFMA2 on sm_100a
+//   pr      the same quantity of TWO latitude rows in one 64-bit register pair: every operation acts on both rows
 //
 // Factorisation of the length-N real transform, N = 8 * N2 (reference semantics: torch.fft.rfft / irfft(norm="forward") as called
 // by torch_harmonics.RealSHT / InverseRealSHT; call sites makani/models/common/spectral_convolution.py:239,253):

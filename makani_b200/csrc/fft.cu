@@ -9,7 +9,7 @@
 //
 // Two kernel families share the butterflies (fft_butterfly.cuh):
 //   *_ct  : radix plan fixed at compile time (CT_PLANS): one half-length complex FFT per real row, two rows per 64-bit register
-//           pair (packed FADD2/FMUL2/FFMA2), persistent CTAs with register prefetch of the next tile, first stage fused with the
+//           pair (pr: each operation on both rows), persistent CTAs with register prefetch of the next tile, first stage fused with the
 //           global load, last stage of the inverse fused with the store, per-buffer conflict-free shared-memory layouts.
 //   *_rt  : any length whose prime factors are <= 13 (runtime plan), two real rows packed into one complex sequence.
 //
@@ -112,7 +112,7 @@ struct FftParams {
   int R;            // B*C image rows
   int C;            // channels (bias index = r % C)
   int scale_mode;
-  int round_tf32;   // analysis output feeds a tcgen05 kind::tf32 GEMM: round to nearest TF32 here
+  int round_tf32;   // analysis output feeds a TF32 tensor-core GEMM: round to nearest TF32 here
   const float2* twiddle;
   const float* rowscale;
   const float* bias;
@@ -136,9 +136,8 @@ __device__ __forceinline__ float mode_scale_analysis(const FftParams& prm, int m
 // as one 4- or 8-byte word), followed by the split  X[m] = E[m] + W_N^m O[m],  E = (Z[m] + conj Z[H-m])/2,
 // O = (Z[m] - conj Z[H-m])/(2i).  A CTA owns ROWS consecutive latitude rows; the threads form GROUPS groups of TPG threads, a
 // group owns RPT = ROWS/GROUPS rows.  One thread carries the same butterfly index of TWO adjacent rows in the two halves of 64-bit
-// registers (value type cpair): every arithmetic instruction is a packed FADD2 / FMUL2 / FFMA2.  The FMA pipe does the same work
-// either way (FFMA2 issues at half the FFMA rate, measured with scripts/micro/f32x2.cu); what is halved is the number of issue
-// slots and of index computations.
+// registers (value type cpair): every arithmetic operation acts on both rows, so the index computations
+// and shared-memory addressing are shared by two rows.
 //
 // Exchange buffers (shared memory, Stockham: stage s reads one buffer and writes the other).  A buffer holds PROWS = ROWS/2 row
 // pairs as two planes of 8-byte elements (real parts of both rows / imaginary parts of both rows), so every access is an 8-byte
@@ -761,7 +760,7 @@ static int launch_ct(const Plan* pl, int dir, const void* in, void* out, const F
   int per_sm = (int)((227 * 1024) / (smem + 1024));
   if (per_sm < 1) per_sm = 1;
   if (per_sm > 4) per_sm = 4;
-  const int sms = usable_sms(pl->sm_count > 0 ? pl->sm_count : 148);
+  const int sms = usable_sms(pl->sm_count > 0 ? pl->sm_count : 132);
   dim3 grid(ntiles < per_sm * sms ? ntiles : per_sm * sms);
   if (dir == 0) {
     auto k = fft_analysis_ct_kernel<T, ROWS, GROUPS, TPG, R0, R1, R2, MINB>;

@@ -1,7 +1,7 @@
 // In-register DFT butterflies of the longitude FFT (fft.cu), generic over the complex value type:
 //   float2  one complex number (host emulation, runtime-plan kernels)
-//   cpair   the same complex element of TWO latitude rows, real parts in one 64-bit register pair and imaginary parts in another,
-//           so that every add / mul / fma is one packed FADD2 / FMUL2 / FFMA2 (sm_100a) for both rows.
+//   cpair   the same complex element of TWO latitude rows, real parts in one register pair and imaginary parts in another; every
+//           add / mul / fma acts on both rows (two scalar instructions on sm_90a, which has no packed fp32 arithmetic).
 // Everything is written with explicit fused multiply-adds and "+ (-i) b" forms so that no negation or multiplication by 0 / 1
 // is ever materialised in either instantiation.
 #pragma once
@@ -19,49 +19,13 @@ struct pr { float2 v; };
 struct __align__(16) cpair { pr x, y; };   // (re row A, re row B), (im row A, im row B)
 
 HD pr make_pr(float a, float b) { pr r; r.v = make_float2(a, b); return r; }
-HD pr operator+(pr a, pr b) {
-#ifdef __CUDA_ARCH__
-  pr r; r.v = __fadd2_rn(a.v, b.v); return r;
-#else
-  return make_pr(a.v.x + b.v.x, a.v.y + b.v.y);
-#endif
-}
-HD pr operator-(pr a, pr b) {
-#ifdef __CUDA_ARCH__
-  pr r; r.v = __ffma2_rn(b.v, make_float2(-1.f, -1.f), a.v); return r;   // a - b in one FFMA2 (exact: b * -1 is exact)
-#else
-  return make_pr(a.v.x - b.v.x, a.v.y - b.v.y);
-#endif
-}
-HD pr operator*(pr a, pr b) {
-#ifdef __CUDA_ARCH__
-  pr r; r.v = __fmul2_rn(a.v, b.v); return r;
-#else
-  return make_pr(a.v.x * b.v.x, a.v.y * b.v.y);
-#endif
-}
+HD pr operator+(pr a, pr b) { return make_pr(a.v.x + b.v.x, a.v.y + b.v.y); }
+HD pr operator-(pr a, pr b) { return make_pr(a.v.x - b.v.x, a.v.y - b.v.y); }
+HD pr operator*(pr a, pr b) { return make_pr(a.v.x * b.v.x, a.v.y * b.v.y); }
 // a * s and a * s + c with a scalar factor shared by both rows
-HD pr rmul(pr a, float s) {
-#ifdef __CUDA_ARCH__
-  pr r; r.v = __fmul2_rn(a.v, make_float2(s, s)); return r;
-#else
-  return make_pr(a.v.x * s, a.v.y * s);
-#endif
-}
-HD pr rfma(pr a, float s, pr c) {
-#ifdef __CUDA_ARCH__
-  pr r; r.v = __ffma2_rn(a.v, make_float2(s, s), c.v); return r;
-#else
-  return make_pr(a.v.x * s + c.v.x, a.v.y * s + c.v.y);
-#endif
-}
-HD pr rfma(pr a, pr s, pr c) {
-#ifdef __CUDA_ARCH__
-  pr r; r.v = __ffma2_rn(a.v, s.v, c.v); return r;
-#else
-  return make_pr(a.v.x * s.v.x + c.v.x, a.v.y * s.v.y + c.v.y);
-#endif
-}
+HD pr rmul(pr a, float s) { return make_pr(a.v.x * s, a.v.y * s); }
+HD pr rfma(pr a, float s, pr c) { return make_pr(a.v.x * s + c.v.x, a.v.y * s + c.v.y); }
+HD pr rfma(pr a, pr s, pr c) { return make_pr(a.v.x * s.v.x + c.v.x, a.v.y * s.v.y + c.v.y); }
 HD float rmul(float a, float s) { return a * s; }
 HD float rfma(float a, float s, float c) { return a * s + c; }
 

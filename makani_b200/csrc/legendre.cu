@@ -43,7 +43,7 @@ __global__ void round_tf32_kernel(const float* __restrict__ src, float* __restri
   if (i < n) dst[i] = tf32_rn(src[i]);
 }
 
-// 3 x TF32: an fp32 operand v enters a kind::tf32 MMA as trunc(v) (the tensor core ignores the 13 low mantissa bits); the residual
+// 3 x TF32: an fp32 operand v enters a TF32 MMA as trunc(v) (the tensor core ignores the 13 low mantissa bits); the residual
 // v - trunc(v) is exact in fp32 and is fed to a second MMA, rounded to nearest TF32 here (its own truncation would add a 2^-21 bias).
 __global__ void tf32_residual_kernel(const float4* __restrict__ src, float4* __restrict__ dst, size_t n4) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;

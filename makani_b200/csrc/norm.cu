@@ -196,8 +196,17 @@ __global__ void norm_finalize_kernel(const float* __restrict__ partial, float* _
   }
 }
 
+// SMs of the current device (132 on an H100 SXM; also the value without a device, for the host-side workspace queries)
+static int device_sms() {
+  static int cached[64] = {0};
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  if (cached[dev] == 0) cached[dev] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 132;
+  return cached[dev];
+}
+
 int norm_splits(int rows, long long n) {
-  long long s = (8LL * 148 + rows - 1) / rows;          // >= 8 CTAs per SM's worth of blocks
+  long long s = (8LL * device_sms() + rows - 1) / rows;   // >= 8 CTAs per SM's worth of blocks
   const long long by_len = n / 2048 > 0 ? n / 2048 : 1;  // but not less than 2048 elements per CTA
   if (s > by_len) s = by_len;
   if (s > kNormMaxSplits) s = kNormMaxSplits;

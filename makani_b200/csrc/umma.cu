@@ -1,44 +1,113 @@
-// tcgen05 / TMA path (B200SHT_PREC_TF32): the Legendre contractions and the dense channel mix as TMA-fed tensor-core
-// GEMMs with fp32 accumulators in TMEM.
+// Tensor-core path (B200SHT_PREC_TF32): the Legendre contractions and the dense channel mix as TMA-fed TF32 GEMMs with fp32
+// accumulation.
 //
-//   one persistent engine (umma_kernel<Traits>, one CTA per SM walking the tile list): warp 0 lane 0 = TMA producer, warp 1
-//   lane 0 = tcgen05.mma issuer, warps 2..5 = epilogue (warp w owns TMEM lanes 32(w%4)..+31).  A ring of `stages` operand
-//   stages guarded by full/empty mbarriers runs continuously across tiles; two accumulator sets in TMEM (acc_full/acc_empty)
-//   let the epilogue of tile i overlap the main loop of tile i+1.
+//   one persistent engine (umma_kernel<Traits>, one CTA per SM walking the tile list): warp 0 lane 0 = TMA producer, warps 1..8 =
+//   consumers; consumer warp w owns rows 16 (w - 1) .. + 15 of the 128-row tile, issues mma.m16n8k8 (TF32) on them against every column
+//   of the tile and stores its accumulators itself.  A ring of `stages` operand stages guarded by full/empty mbarriers runs continuously
+//   across tiles, so the producer prefetches the next tile while the consumers finish the current one and write it out.
 //
-//   five Traits supply the per-operation pieces (tile coordinates, TMA boxes, MMA issue list, epilogue):
+//   five Traits supply the per-operation pieces (tile coordinates, TMA boxes, MMA list, epilogue):
 //     AnaTraits   spec[l][m][n]  = sum_k P[m][l][k] X[m][n][k]          A K-major,  B K-major     (RealSHT einsum "...km,mlk->...lm")
 //     SynTraits   Z[m][n][k]     = sum_l P[m][l][k] spec[l][m][n]       A MN-major, B MN-major    (InverseRealSHT "...lm,mlk->...km")
 //     MixFwd      y[row][o]      = sum_i x[row][i] w[i][o]   (complex)  A K-major,  B MN-major    (contractions.py:23 "bgixy,giox->bgoxy")
 //     MixDgrad    gx[row][i]     = sum_o gy[row][o] conj(w[i][o])       A K-major,  B K-major
 //     MixWgrad    gw[i][o]       = sum_row conj(x[row][i]) gy[row][o]   A MN-major, B MN-major
-//   complex products use planar operands: 4 real MMAs into two accumulators (real, imaginary), one of them with the
-//   instruction descriptor's negate-A bit.
+//   complex products use planar operands: 4 real MMAs into two accumulators (real, imaginary), negated terms through a sign flip of
+//   the A fragment.
 //
-// All shared-memory operand tiles use the 128-byte swizzle; every TMA box is [rows][32 floats] so it lands as rows of 128 B.
+// All shared-memory operand tiles use the 128-byte swizzle; every TMA box is [rows][32 floats] so it lands as rows of 128 B.  wgmma is
+// not used: it reads TF32 operands from shared memory only K-major, and synthesis (A and B), mix forward (B) and wgrad (A and B) have
+// MN-major operands; B cannot come from registers.  A register-sourced-A wgmma would serve the K-major analysis and dgrad GEMMs; it is
+// not built, and the H100 cost of this engine is recorded in DESIGN.md section 9.
 #include "umma_common.cuh"
 #include <mutex>
 
 namespace b200sht {
 
 // ======================================================================================================= engine
-constexpr int kUmmaThreads = 192;   // warp 0: TMA producer, warp 1: MMA issuer + TMEM owner, warps 2..5: epilogue
+constexpr int kConsumerWarps = 8;                         // 8 x 16 rows = the 128-row tile
+constexpr int kUmmaThreads = 32 * (1 + kConsumerWarps);   // warp 0: TMA producer, warps 1..8: MMA + epilogue
 constexpr int kMaxStages = 8;
-constexpr int kEpiScratch = 256;     // ints of per-tile epilogue scratch (one per accumulator column)
+constexpr int kMaxCols = 256;                             // accumulator columns of a tile (a complex tile: 2 x 128)
 
 struct EngineParams {
   int stages;
-  uint32_t stage_bytes, tx_bytes, tmem_cols;
+  uint32_t stage_bytes, tx_bytes;
   int gx, gy, gz;          // logical tile grid (x fastest); CTAs walk it round-robin
-  int acc_cols, nbuf;      // TMEM columns of one accumulator set, number of sets (2: epilogue of tile i overlaps main loop of i+1)
   int split;               // 3 x TF32 (strict fp32 on the tensor cores): every stage also holds the residual tiles of both operands, `lo_off`
   uint32_t lo_off;         // bytes after the main tiles, and each MMA becomes hi.hi + hi.lo + lo.hi into the same accumulator
 };
 
+// Accumulators of one consumer warp: 16 rows x kMaxCols columns as m16n8 fragments, acc[j] = columns 8 j .. 8 j + 7.  Complex tiles keep the
+// real part in acc[0 .. 15] and the imaginary part in acc[16 .. 31].
+typedef float Acc[kMaxCols / 8][4];
+
+// acc[j] += A(rows row0 .. + 15) B(columns 8 j .. + 7) over the 32 K of one stage, j < nb
+template <bool AMN, bool BMN>
+__device__ __forceinline__ void gemm_real(const uint8_t* a, const uint8_t* b, int row0, int nb, Acc& acc) {
+#pragma unroll
+  for (int kk = 0; kk < 32; kk += 8) {
+    uint32_t fa[4];
+    frag_a<AMN>(a, row0, kk, fa);
+#pragma unroll
+    for (int j = 0; j < kMaxCols / 8; ++j) {
+      if (j < nb) {
+        uint32_t fb[2];
+        frag_b<BMN>(b, 8 * j, kk, fb);
+        mma_tf32(acc[j], fa, fb);
+      }
+    }
+  }
+}
+// complex product of planar operands, S1..S3 = +-1:  re += ar br + S1 ai bi,  im += S2 ar bi + S3 ai br  (j < nb <= 16)
+template <bool AMN, bool BMN, int S1, int S2, int S3>
+__device__ __forceinline__ void gemm_cplx(const uint8_t* ar, const uint8_t* ai, const uint8_t* br, const uint8_t* bi, int row0, int nb, Acc& acc) {
+#pragma unroll
+  for (int kk = 0; kk < 32; kk += 8) {
+    uint32_t fr[4], fi[4], nr[4], ni[4];
+    frag_a<AMN>(ar, row0, kk, fr);
+    frag_a<AMN>(ai, row0, kk, fi);
+    frag_neg(fr, nr);
+    frag_neg(fi, ni);
+#pragma unroll
+    for (int j = 0; j < kMaxCols / 16; ++j) {
+      if (j < nb) {
+        uint32_t gr[2], gi[2];
+        frag_b<BMN>(br, 8 * j, kk, gr);
+        frag_b<BMN>(bi, 8 * j, kk, gi);
+        mma_tf32(acc[j], fr, gr);
+        mma_tf32(acc[j], S1 > 0 ? fi : ni, gi);
+        mma_tf32(acc[16 + j], S2 > 0 ? fr : nr, gi);
+        mma_tf32(acc[16 + j], S3 > 0 ? fi : ni, gr);
+      }
+    }
+  }
+}
+// f(row, column, value) for every accumulator element of the warp (rows row0 + lane / 4 (+ 8), columns < 8 nb)
+template <class F>
+__device__ __forceinline__ void for_each_acc(const Acc& acc, int row0, int nb, F f) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < kMaxCols / 8; ++j)
+    if (j < nb) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) f(row0 + (lane >> 2) + 8 * (e >> 1), 8 * j + 2 * (lane & 3) + (e & 1), acc[j][e]);
+    }
+}
+// same for a complex accumulator: f(row, column, real, imaginary), nb <= 16
+template <class F>
+__device__ __forceinline__ void for_each_cacc(const Acc& acc, int row0, int nb, F f) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < kMaxCols / 16; ++j)
+    if (j < nb) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) f(row0 + (lane >> 2) + 8 * (e >> 1), 8 * j + 2 * (lane & 3) + (e & 1), acc[j][e], acc[16 + j][e]);
+    }
+}
 
 // Persistent engine: one CTA per SM loops over tiles.  The operand ring (full/empty) runs continuously across tiles, so the
-// TMA producer prefetches the next tile while the tensor core finishes the current one and the four epilogue warps drain the
-// previous accumulator set (acc_full / acc_empty).
+// TMA producer prefetches the next tile while the consumer warps finish the current one.
 template <class T>
 __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_constant__ typename T::Params p) {
   extern __shared__ uint8_t smem_raw[];
@@ -49,27 +118,17 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_cons
   const uint32_t stage_bytes = p.stage_bytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(gbase + (size_t)stages * stage_bytes);
   uint64_t* empty = full + kMaxStages;
-  uint64_t* acc_full = empty + kMaxStages;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  int* epi_scratch = reinterpret_cast<int*>(tmem_slot + 4);   // 2 x kEpiScratch ints, double-buffered by tile parity (epilogue warps only)
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
   pdl_trigger();   // the next kernel of the stream may be scheduled while this one runs (it waits for our completion before touching data)
   if (warp == 0 && lane == 0) {
-    for (int s = 0; s < stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 4); }
+    for (int s = 0; s < stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumerWarps); }
     fence_barrier_init();
     T::prefetch(p);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   const int ntiles = p.gx * p.gy * p.gz;
-  const int nbuf = p.nbuf;
-  pdl_wait();      // prologue done (barriers, TMEM, tensor-map prefetch): from here on this kernel reads what its predecessors wrote
+  pdl_wait();      // prologue done (barriers, tensor-map prefetch): from here on this kernel reads what its predecessors wrote
 
   if (warp == 0) {
     if (lane == 0) {
@@ -87,50 +146,26 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_cons
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    {   // all 32 lanes run the loop (converged); MMAs and commits are issued by an elected lane (umma_*_ws)
-      int kbg = 0, i = 0;
-      for (int ti = blockIdx.x; ti < ntiles; ti += gridDim.x) {
-        typename T::Tile tile;
-        if (!T::make_tile(p, tile, ti % p.gx, (ti / p.gx) % p.gy, ti / (p.gx * p.gy))) continue;
-        const int nk = T::num_kblocks(p, tile);
-        const int buf = i % nbuf, use = i / nbuf;
-        if (use > 0) {  // the epilogue must have drained this accumulator set
-          mbar_wait(&acc_empty[buf], (use - 1) & 1);
-          tc_fence_after();
-        }
-        for (int kb = 0; kb < nk; ++kb, ++kbg) {
-          const int s = kbg % stages, it = kbg / stages;
-          mbar_wait(&full[s], it & 1);
-          tc_fence_after();
-          T::mma(p, tile, base + s * stage_bytes, tmem + buf * p.acc_cols, kb > 0);
-          umma_commit_ws(&empty[s]);
-        }
-        umma_commit_ws(&acc_full[buf]);
-        ++i;
-      }
-    }
-    __syncwarp();
   } else {
-    const int quad = warp & 3;   // a warp may only touch TMEM lanes 32 * (warp % 4) .. + 31
-    int i = 0;
+    const int row0 = 16 * (warp - 1);
+    int kbg = 0;
     for (int ti = blockIdx.x; ti < ntiles; ti += gridDim.x) {
       typename T::Tile tile;
       if (!T::make_tile(p, tile, ti % p.gx, (ti / p.gx) % p.gy, ti / (p.gx * p.gy))) continue;
       const int nk = T::num_kblocks(p, tile);
-      const int buf = i % nbuf, use = i / nbuf;
-      mbar_wait(&acc_full[buf], use & 1);
-      tc_fence_after();
-      T::epilogue(p, tile, tmem + buf * p.acc_cols, quad, lane, nk, epi_scratch + (i & 1) * kEpiScratch);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
-      ++i;
+      Acc acc;
+#pragma unroll
+      for (int j = 0; j < kMaxCols / 8; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+      for (int kb = 0; kb < nk; ++kb, ++kbg) {
+        const int s = kbg % stages, it = kbg / stages;
+        mbar_wait(&full[s], it & 1);
+        T::mma(p, gbase + (size_t)s * stage_bytes, row0, acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);   // this warp's reads of the stage are done
+      }
+      T::epilogue(p, tile, row0, acc);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, p.tmem_cols);
 }
 
 // ================================================================================================ AnaTraits
@@ -143,7 +178,6 @@ struct AnaTraits {
     int L, M, nlat, C, cp, PB, Cc, PBc, n_ct, N, m0;
     int kb0, nkb;        // latitude range of this launch in 32-row K-blocks (latitude-chunked analysis: partial sums over a chunk of rows)
     int acc_in, round_out;   // add to the spec values already stored (chunks after the first) / round the result to TF32 (last chunk)
-    uint32_t idesc;
   };
   struct Tile { int m, l0, c0, pb0; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
@@ -164,61 +198,31 @@ struct AnaTraits {
       tma_load_4d(st + p.lo_off + 16384, &p.tmB_lo, bar, kb * 32, t.c0, t.pb0, t.m);
     }
   }
-  __device__ static void mma(const Params& p, const Tile&, uint32_t st, uint32_t tmem, bool acc) {
-    const uint64_t a = desc_kmajor(st, 0), b = desc_kmajor(st + 16384, 0);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) umma_tf32_ws(tmem, desc_advance(a, 32 * j), desc_advance(b, 32 * j), p.idesc, (acc || j > 0) ? 1u : 0u);
+  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, Acc& acc) {
+    const int nb = p.N / 8;
+    gemm_real<false, false>(st, st + 16384, row0, nb, acc);
     if (p.split) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        umma_tf32_ws(tmem, desc_advance(a, 32 * j), desc_advance(b, p.lo_off + 32 * j), p.idesc, 1u);   // hi . lo
-        umma_tf32_ws(tmem, desc_advance(a, p.lo_off + 32 * j), desc_advance(b, 32 * j), p.idesc, 1u);   // lo . hi
-      }
+      gemm_real<false, false>(st, st + p.lo_off + 16384, row0, nb, acc);   // hi . lo
+      gemm_real<false, false>(st + p.lo_off, st + 16384, row0, nb, acc);   // lo . hi
     }
   }
-  __device__ static void epilogue(const Params& p, const Tile& t, uint32_t tmem, int warp, int lane, int nk, int* scratch) {
-    const int l = t.l0 + warp * 32 + lane;
+  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const Acc& acc) {
     const int ncols = p.Cc * p.PBc;
     const size_t JP = (size_t)p.PB * p.cp;
-    float* orow = p.spec + ((size_t)(l < p.L ? l : 0) * p.M + t.m) * JP;
-    float v[32];
-    for (int n0 = 0; n0 < ncols; n0 += 32) {
-      tmem_ld32(tmem + ((uint32_t)(warp * 32) << 16) + n0, v);
-      if (l >= p.L) continue;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const int n = n0 + q * 4;
-        if (n >= ncols) break;
-        const int pbi = n / p.Cc, ci = n - pbi * p.Cc;
-        const int pb = t.pb0 + pbi, c = t.c0 + ci;
-        if (pb < p.PB && c < p.cp) {
-          float4* dst = reinterpret_cast<float4*>(orow + (size_t)pb * p.cp + c);
-          float4 o = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
-          if (p.acc_in) {   // partial sums of the earlier latitude chunks (unrounded fp32)
-            const float4 old = *dst;
-            o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
-          }
-          // strict fp32 (split) and the partial sums of a chunked analysis stay as accumulated; otherwise the consumers are kind::tf32
-          // MMAs: round to nearest here
-          if (p.round_out) o = make_float4(tf32_rn(o.x), tf32_rn(o.y), tf32_rn(o.z), tf32_rn(o.w));
-          *dst = o;
-        }
-      }
-    }
+    for_each_acc(acc, row0, p.N / 8, [&](int r, int n, float v) {
+      const int l = t.l0 + r;
+      if (l >= p.L || n >= ncols) return;
+      const int pbi = n / p.Cc, ci = n - pbi * p.Cc;
+      const int pb = t.pb0 + pbi, c = t.c0 + ci;
+      if (pb >= p.PB || c >= p.cp) return;
+      float* dst = p.spec + ((size_t)l * p.M + t.m) * JP + (size_t)pb * p.cp + c;
+      if (p.acc_in) v += *dst;   // partial sums of the earlier latitude chunks (unrounded fp32)
+      // strict fp32 (split) and the partial sums of a chunked analysis stay as accumulated; otherwise the consumers are TF32 MMAs: round
+      // to nearest here
+      *dst = p.round_out ? tf32_rn(v) : v;
+    });
   }
 };
-
-// base[o] = v when o >= 0: compare + one wide multiply-add + predicated store, no branch
-__device__ __forceinline__ void st_if_nonneg(float* base, int o, float v) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      ".reg .s64 a;\n"
-      "setp.ge.s32 p, %1, 0;\n"
-      "mad.wide.s32 a, %1, 4, %0;\n"
-      "@p st.global.f32 [a], %2;\n"
-      "}\n" ::"l"(base), "r"(o), "f"(v) : "memory");
-}
 
 // ================================================================================================ SynTraits
 struct SynTraits {
@@ -230,7 +234,6 @@ struct SynTraits {
     int L, M, nlat, kp, C, cp, PB, nblk, N, m0;
     int kc0, kc1;           // latitude range [kc0, kc1) of this launch (kc0 a multiple of 128): the tiles cover these rows only
     int tiled, M2, KT, B;   // tiled output for the tensor-core DFT (dft.cu): Z[r][k / 8][p][m / 8][m % 8][k % 8], orders padded to 8 * M2
-    uint32_t idesc;
   };
   struct Tile { int m, k0, n0, lbeg; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
@@ -254,63 +257,30 @@ struct SynTraits {
       for (int b = 0; b < p.nblk; ++b) tma_load_3d(st + p.lo_off + 16384 + b * 4096, &p.tmB_lo, bar, t.n0 + 32 * b, t.m, l);
     }
   }
-  __device__ static void mma(const Params& p, const Tile&, uint32_t st, uint32_t tmem, bool acc) {
-    const uint64_t a = desc_mnmajor(st, 0, 4096), b = desc_mnmajor(st + 16384, 0, 4096);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) umma_tf32_ws(tmem, desc_advance(a, 1024 * j), desc_advance(b, 1024 * j), p.idesc, (acc || j > 0) ? 1u : 0u);
+  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, Acc& acc) {
+    const int nb = p.N / 8;
+    gemm_real<true, true>(st, st + 16384, row0, nb, acc);
     if (p.split) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        umma_tf32_ws(tmem, desc_advance(a, 1024 * j), desc_advance(b, p.lo_off + 1024 * j), p.idesc, 1u);   // hi . lo
-        umma_tf32_ws(tmem, desc_advance(a, p.lo_off + 1024 * j), desc_advance(b, 1024 * j), p.idesc, 1u);   // lo . hi
-      }
+      gemm_real<true, true>(st, st + p.lo_off + 16384, row0, nb, acc);   // hi . lo
+      gemm_real<true, true>(st + p.lo_off, st + 16384, row0, nb, acc);   // lo . hi
     }
   }
-  __device__ static void epilogue(const Params& p, const Tile& t, uint32_t tmem, int warp, int lane, int nk, int* scratch) {
-    const int k = t.k0 + warp * 32 + lane;
+  // column jp = pb * cp + c of the tile -> row (pb, c) of this order's slab of Z; orders without a contributing degree hold zero accumulators
+  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const Acc& acc) {
     const int JP = p.PB * p.cp;
-    // column jp = pb * cp + c -> element offset of row (pb, c) of this order's slab of Z, -1 for the channel padding: one division per
-    // column per tile, shared by the four epilogue warps through `scratch` (the per-element bookkeeping of an incremental row
-    // pointer made this kernel epilogue-bound: 60 % of its stall samples)
-    for (int n = warp * 32 + lane; n < p.N; n += 128) {
-      const int jp = t.n0 + n;
-      int o = -1;
-      if (jp < JP) {
-        const int pb = jp / p.cp, c = jp - pb * p.cp;
-        if (c < p.C) {
-          if (!p.tiled) o = (pb * p.C + c) * p.kp;
-          else {   // pb = plane * B + b, image r = b * C + c:  Z[r][kt][plane][m2][c8][k8]
-            const int pl = pb / p.B, b = pb - pl * p.B;
-            o = (((b * p.C + c) * p.KT) * 2 + pl) * p.M2 * 64;
-          }
-        }
+    for_each_acc(acc, row0, p.N / 8, [&](int r, int n, float v) {
+      const int k = t.k0 + r, jp = t.n0 + n;
+      if (k >= p.kc1 || jp >= JP) return;
+      const int pb = jp / p.cp, c = jp - pb * p.cp;
+      if (c >= p.C) return;
+      if (!p.tiled) {
+        p.Z[(size_t)t.m * p.PB * p.C * p.kp + (size_t)(pb * p.C + c) * p.kp + k] = v;
+      } else {   // pb = plane * B + b, image r = b * C + c:  Z[r][kt][plane][m2][c8][k8]
+        const int pl = pb / p.B, b = pb - pl * p.B;
+        const int o = (((b * p.C + c) * p.KT) * 2 + pl) * p.M2 * 64;
+        p.Z[(size_t)(k >> 3) * 2 * p.M2 * 64 + (t.m >> 3) * 64 + (t.m & 7) * 8 + (k & 7) + o] = v;
       }
-      scratch[n] = o;
-    }
-    asm volatile("bar.sync 1, 128;" ::: "memory");   // epilogue warps only
-    const bool kok = k < p.kc1;
-    const int kk = kok ? k : 0;
-    float* zb = p.tiled ? p.Z + (size_t)(kk >> 3) * 2 * p.M2 * 64 + (t.m >> 3) * 64 + (t.m & 7) * 8 + (kk & 7)
-                        : p.Z + (size_t)t.m * p.PB * p.C * p.kp + kk;
-    float v[32];
-    for (int n0 = 0; n0 < p.N; n0 += 32) {
-      if (t.n0 + n0 >= JP) break;
-      tmem_ld32(tmem + ((uint32_t)(warp * 32) << 16) + n0, v);
-      if (nk == 0) {   // no degree contributes to this order (cannot happen for m < lmax; kept for safety)
-#pragma unroll
-        for (int q = 0; q < 32; ++q) v[q] = 0.f;
-      }
-      if (kok) {
-#pragma unroll
-        for (int q4 = 0; q4 < 8; ++q4) {
-          const int4 o = *reinterpret_cast<const int4*>(scratch + n0 + 4 * q4);
-          st_if_nonneg(zb, o.x, v[4 * q4 + 0]);
-          st_if_nonneg(zb, o.y, v[4 * q4 + 1]);
-          st_if_nonneg(zb, o.z, v[4 * q4 + 2]);
-          st_if_nonneg(zb, o.w, v[4 * q4 + 3]);
-        }
-      }
-    }
+    });
   }
 };
 
@@ -325,12 +295,11 @@ struct MixParams : EngineParams {
   const float2* cbias;
   int L, M, B, G, Cig, Cog, cpi, cpo, cop;
   int Mt;                  // m values per row tile (Mt * B <= 128 rows)
-  int nblk, N;             // N = output columns per tile; nblk = N / 32 (MN-major B operands)
+  int nblk, N;             // N = output columns per tile (<= 128); nblk = N / 32 (MN-major B operands)
   int n_nt;                // output tiles per group
   int shared_w;            // weight has no l dimension
   int dense;               // spec tensors store every (l, m) entry
   long long wl_stride;
-  uint32_t idesc, idesc_neg;
   uint32_t offA_i, offB_r, offB_i;  // stage offsets of the imaginary A tile and the two B tiles (A_r at 0)
 };
 
@@ -356,64 +325,28 @@ struct MixFwdTraits {
       tma_load_4d(st + p.offB_i + b * 4096, &p.tmW, bar, t.o0 + 32 * b, 1, kb * 32, t.lg);
     }
   }
-  __device__ static void mma(const Params& p, const Tile&, uint32_t st, uint32_t tmem, bool acc) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const uint64_t ar = desc_advance(desc_kmajor(st, 0), 32 * j), ai = desc_advance(desc_kmajor(st + p.offA_i, 0), 32 * j);
-      const uint64_t br = desc_advance(desc_mnmajor(st + p.offB_r, 0, 4096), 1024 * j), bi = desc_advance(desc_mnmajor(st + p.offB_i, 0, 4096), 1024 * j);
-      const uint32_t a0 = (acc || j > 0) ? 1u : 0u;
-      umma_tf32_ws(tmem, ar, br, p.idesc, a0);            // yr  = xr wr
-      umma_tf32_ws(tmem, ai, bi, p.idesc_neg, 1u);        // yr -= xi wi
-      umma_tf32_ws(tmem + p.N, ar, bi, p.idesc, a0);      // yi  = xr wi
-      umma_tf32_ws(tmem + p.N, ai, br, p.idesc, 1u);      // yi += xi wr
-    }
+  // yr = xr wr - xi wi,  yi = xr wi + xi wr
+  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, Acc& acc) {
+    gemm_cplx<false, true, -1, 1, 1>(st, st + p.offA_i, st + p.offB_r, st + p.offB_i, row0, p.N / 8, acc);
   }
   // rows (mi, b) -> spec rows; columns -> output channels of group g; handles cbias and the zero channel padding
-  __device__ static void store_rows(const Params& p, int l, int m0, int g, int o0, int NOg, int cp_out, uint32_t tmem, int warp, int lane,
-                                    bool with_bias) {
-    const int r = warp * 32 + lane;
-    const int m = m0 + r / p.B, b = r % p.B;
-    const bool row_ok = (r < p.Mt * p.B) && (m < mend_d(l, p.M, p.dense));
+  __device__ __forceinline__ static void store_rows(const Params& p, int l, int m0, int g, int o0, int NOg, int cp_out, int row0, const Acc& acc,
+                                                    bool with_bias) {
     const int pad = cp_out - NOg * p.G;
     const int limit = NOg + ((g == p.G - 1) ? pad : 0);  // columns of this group incl. trailing zero padding
-    float* yr = p.out + ((size_t)(row_ok ? l : 0) * p.M + (row_ok ? m : 0)) * 2 * p.B * cp_out + (size_t)b * cp_out + g * NOg;
-    float* yi = yr + (size_t)p.B * cp_out;
-    float vr[32], vi[32];
-    for (int n0 = 0; n0 < p.N; n0 += 32) {
-      if (o0 + n0 >= limit) break;
-      tmem_ld32(tmem + ((uint32_t)(warp * 32) << 16) + n0, vr);
-      tmem_ld32(tmem + ((uint32_t)(warp * 32) << 16) + p.N + n0, vi);
-      if (!row_ok) continue;
-      // 16-byte stores (one row per thread: a warp store touches 32 rows, so wide stores cut the L2 write transactions 4x)
-      const bool vec_ok = (((g * NOg) & 3) == 0);   // cp_out and o0 + n0 are multiples of 4
-#pragma unroll
-      for (int q4 = 0; q4 < 8; ++q4) {
-        const int ob = o0 + n0 + q4 * 4;
-        if (ob >= limit) break;
-        float a[4], c[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int o = ob + u;
-          a[u] = vr[q4 * 4 + u];
-          c[u] = vi[q4 * 4 + u];
-          if (o >= NOg) { a[u] = 0.f; c[u] = 0.f; }
-          else if (with_bias) { const float2 cb = p.cbias[g * NOg + o]; a[u] += cb.x; c[u] += cb.y; }
-          a[u] = tf32_rn(a[u]);
-          c[u] = tf32_rn(c[u]);
-        }
-        if (vec_ok && ob + 3 < limit) {
-          *reinterpret_cast<float4*>(yr + ob) = make_float4(a[0], a[1], a[2], a[3]);
-          *reinterpret_cast<float4*>(yi + ob) = make_float4(c[0], c[1], c[2], c[3]);
-        } else {
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (ob + u < limit) { yr[ob + u] = a[u]; yi[ob + u] = c[u]; }
-        }
-      }
-    }
+    const int mend = mend_d(l, p.M, p.dense);
+    for_each_cacc(acc, row0, p.N / 8, [&](int r, int n, float a, float c) {
+      const int m = m0 + r / p.B, b = r % p.B, o = o0 + n;
+      if (r >= p.Mt * p.B || m >= mend || o >= limit) return;
+      if (o >= NOg) { a = 0.f; c = 0.f; }
+      else if (with_bias) { const float2 cb = p.cbias[g * NOg + o]; a += cb.x; c += cb.y; }
+      float* yr = p.out + ((size_t)l * p.M + m) * 2 * p.B * cp_out + (size_t)b * cp_out + g * NOg + o;
+      yr[0] = tf32_rn(a);
+      yr[(size_t)p.B * cp_out] = tf32_rn(c);
+    });
   }
-  __device__ static void epilogue(const Params& p, const Tile& t, uint32_t tmem, int warp, int lane, int nk, int* scratch) {
-    store_rows(p, t.l, t.m0, t.g, t.o0, p.Cog, p.cpo, tmem, warp, lane, p.cbias != nullptr);
+  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const Acc& acc) {
+    store_rows(p, t.l, t.m0, t.g, t.o0, p.Cog, p.cpo, row0, acc, p.cbias != nullptr);
   }
 };
 
@@ -430,20 +363,12 @@ struct MixDgradTraits {
     tma_load_4d(st + p.offB_r, &p.tmW, bar, kb * 32, 0, t.o0, t.lg);   // box (32 o, 1, N i, 1): K-major rows i
     tma_load_4d(st + p.offB_i, &p.tmW, bar, kb * 32, 1, t.o0, t.lg);
   }
-  __device__ static void mma(const Params& p, const Tile&, uint32_t st, uint32_t tmem, bool acc) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const uint64_t ar = desc_advance(desc_kmajor(st, 0), 32 * j), ai = desc_advance(desc_kmajor(st + p.offA_i, 0), 32 * j);
-      const uint64_t br = desc_advance(desc_kmajor(st + p.offB_r, 0), 32 * j), bi = desc_advance(desc_kmajor(st + p.offB_i, 0), 32 * j);
-      const uint32_t a0 = (acc || j > 0) ? 1u : 0u;
-      umma_tf32_ws(tmem, ar, br, p.idesc, a0);            // gxr  = gr wr
-      umma_tf32_ws(tmem, ai, bi, p.idesc, 1u);            // gxr += gi wi
-      umma_tf32_ws(tmem + p.N, ai, br, p.idesc, a0);      // gxi  = gi wr
-      umma_tf32_ws(tmem + p.N, ar, bi, p.idesc_neg, 1u);  // gxi -= gr wi
-    }
+  // gxr = gr wr + gi wi,  gxi = gi wr - gr wi
+  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, Acc& acc) {
+    gemm_cplx<false, false, 1, -1, 1>(st, st + p.offA_i, st + p.offB_r, st + p.offB_i, row0, p.N / 8, acc);
   }
-  __device__ static void epilogue(const Params& p, const Tile& t, uint32_t tmem, int warp, int lane, int nk, int* scratch) {
-    MixFwdTraits::store_rows(p, t.l, t.m0, t.g, t.o0, p.Cig, p.cpi, tmem, warp, lane, false);
+  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const Acc& acc) {
+    MixFwdTraits::store_rows(p, t.l, t.m0, t.g, t.o0, p.Cig, p.cpi, row0, acc, false);
   }
 };
 
@@ -483,42 +408,19 @@ struct MixWgradTraits {
       tma_load_5d(st + p.offB_i + b * 4096, &p.tmX2, bar, t.g * p.Cog + t.o0 + 32 * b, 0, 1, m, l);
     }
   }
-  __device__ static void mma(const Params& p, const Tile&, uint32_t st, uint32_t tmem, bool acc) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const uint64_t ar = desc_advance(desc_mnmajor(st, 0, 4096), 1024 * j), ai = desc_advance(desc_mnmajor(st + p.offA_i, 0, 4096), 1024 * j);
-      const uint64_t br = desc_advance(desc_mnmajor(st + p.offB_r, 0, 4096), 1024 * j), bi = desc_advance(desc_mnmajor(st + p.offB_i, 0, 4096), 1024 * j);
-      const uint32_t a0 = (acc || j > 0) ? 1u : 0u;
-      umma_tf32_ws(tmem, ar, br, p.idesc, a0);            // gwr  = xr gr
-      umma_tf32_ws(tmem, ai, bi, p.idesc, 1u);            // gwr += xi gi
-      umma_tf32_ws(tmem + p.N, ar, bi, p.idesc, a0);      // gwi  = xr gi
-      umma_tf32_ws(tmem + p.N, ai, br, p.idesc_neg, 1u);  // gwi -= xi gr
-    }
+  // gwr = xr gr + xi gi,  gwi = xr gi - xi gr
+  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, Acc& acc) {
+    gemm_cplx<true, true, 1, 1, -1>(st, st + p.offA_i, st + p.offB_r, st + p.offB_i, row0, p.N / 8, acc);
   }
-  __device__ static void epilogue(const Params& p, const Tile& t, uint32_t tmem, int warp, int lane, int nk, int* scratch) {
-    const int i = t.i0 + warp * 32 + lane;
-    const bool ok = i < p.Cig;
-    float* row = p.out + (size_t)(p.shared_w ? 0 : t.lz) * p.wl_stride + (size_t)(t.g * p.Cig + (ok ? i : 0)) * 2 * p.cop;
-    float vr[32], vi[32];
-    for (int n0 = 0; n0 < p.N; n0 += 32) {
-      if (t.o0 + n0 >= p.cop) break;
-      tmem_ld32(tmem + ((uint32_t)(warp * 32) << 16) + n0, vr);
-      tmem_ld32(tmem + ((uint32_t)(warp * 32) << 16) + p.N + n0, vi);
-      if (!ok) continue;
-#pragma unroll
-      for (int q4 = 0; q4 < 8; ++q4) {   // cop is a multiple of 4: whole float4 groups, 16-byte aligned
-        const int ob = t.o0 + n0 + q4 * 4;
-        if (ob >= p.cop) break;
-        float a[4], c[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          a[u] = (ob + u < p.Cog) ? vr[q4 * 4 + u] : 0.f;
-          c[u] = (ob + u < p.Cog) ? vi[q4 * 4 + u] : 0.f;
-        }
-        *reinterpret_cast<float4*>(row + ob) = make_float4(a[0], a[1], a[2], a[3]);
-        *reinterpret_cast<float4*>(row + p.cop + ob) = make_float4(c[0], c[1], c[2], c[3]);
-      }
-    }
+  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const Acc& acc) {
+    float* const out = p.out + (size_t)(p.shared_w ? 0 : t.lz) * p.wl_stride + (size_t)t.g * p.Cig * 2 * p.cop;
+    for_each_cacc(acc, row0, p.N / 8, [&](int r, int n, float a, float c) {
+      const int i = t.i0 + r, o = t.o0 + n;
+      if (i >= p.Cig || o >= p.cop) return;
+      float* row = out + (size_t)i * 2 * p.cop;
+      row[o] = (o < p.Cog) ? a : 0.f;
+      row[p.cop + o] = (o < p.Cog) ? c : 0.f;
+    });
   }
 };
 
@@ -535,7 +437,7 @@ int umma_available() {
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   if (dev >= 0 && dev < kMaxDevices && g_umma_ok[dev] >= 0) return g_umma_ok[dev];
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  const int ok = (major == 10 && get_encode() != nullptr) ? 1 : 0;
+  const int ok = (major == 9 && get_encode() != nullptr) ? 1 : 0;   // the library is built for sm_90a only
   if (dev >= 0 && dev < kMaxDevices) g_umma_ok[dev] = ok;
   return ok;
 }
@@ -590,21 +492,14 @@ static void pick_stages(EngineParams* e, uint32_t stage_bytes, int /*k-blocks pe
   if (s < 2) s = 2;
   e->stages = s;
 }
-static size_t smem_bytes(const EngineParams& e) { return (size_t)e.stages * e.stage_bytes + 1024 /*align*/ + (2 * kMaxStages + 4) * 8 + 16 + 2 * kEpiScratch * 4; }
-static uint32_t tmem_cols_pow2(int cols) { uint32_t c = 32; while ((int)c < cols) c <<= 1; return c; }
-// accumulator sets: `cols` TMEM columns per tile; two sets (double buffering) when they fit in the 512 columns
-static void set_accumulators(EngineParams* e, int cols) {
-  e->acc_cols = round_up(cols, 32);
-  e->nbuf = (2 * e->acc_cols <= 512) ? 2 : 1;
-  e->tmem_cols = tmem_cols_pow2(e->acc_cols * e->nbuf);
-}
+static size_t smem_bytes(const EngineParams& e) { return (size_t)e.stages * e.stage_bytes + 1024 /*align*/ + 2 * kMaxStages * 8; }
 
 static int sm_count() {   // of the current device (the launch device: _lib.call makes the tensor's device current)
   std::call_once(g_dev_once, init_dev_caches);
   int dev = 0, n = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (dev >= 0 && dev < kMaxDevices && g_sm_count[dev] > 0) return g_sm_count[dev];
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   if (dev >= 0 && dev < kMaxDevices) g_sm_count[dev] = n;
   return n;
 }
@@ -646,7 +541,6 @@ int legendre_analysis_umma(const Plan* pl, const float* X, float* spec, int B, i
   else { p.n_ct = ceil_div(cp, 128); p.Cc = round_up(ceil_div(cp, p.n_ct), 4); p.PBc = (2 * p.Cc <= 256 && PB >= 2) ? 2 : 1; }
   const int rows = p.Cc * p.PBc;
   p.N = round_up(rows, 16);
-  p.idesc = make_idesc(p.N, 0, 0, 0);
   {
     long long d[3] = {pl->nlat, pl->lmax, pl->mmax}, s[3] = {1, pl->kp, (long long)pl->lmax * pl->kp};
     int bx[3] = {32, 128, 1};
@@ -674,7 +568,6 @@ int legendre_analysis_umma(const Plan* pl, const float* X, float* spec, int B, i
   }
   pick_stages(&p, (16384 + bbytes) * (p.split ? 2 : 1), ceil_div(pl->nlat, 32));
   p.tx_bytes = (16384 + (uint32_t)rows * 128) * (p.split ? 2 : 1);
-  set_accumulators(&p, p.N);
   dim3 grid(ceil_div(pl->lmax, 128), p.n_ct * ceil_div(PB, p.PBc), pl->mmax);
   return launch<AnaTraits>(p, grid, st);
 }
@@ -693,17 +586,16 @@ int legendre_synthesis_umma(const Plan* pl, const float* spec, float* Z, int B, 
   B200_REQUIRE(!tiled || (long long)B * C * p.KT * 2 * p.M2 * 64 < (1ll << 31), "legendre_synthesis: tiled latspec of %d images exceeds 2^31 floats", B * C);
   p.nblk = ceil_div(JP, 32) < 8 ? ceil_div(JP, 32) : 8;
   p.N = 32 * p.nblk;
-  p.idesc = make_idesc(p.N, 1, 1, 0);
   {
     long long d[3] = {pl->nlat, pl->lmax, pl->mmax}, s[3] = {1, pl->kp, (long long)pl->lmax * pl->kp};
     int bx[3] = {32, 32, 1};
-    int rc = make_tmap(&p.tmA, pl->d_table_tf32, 3, d, s, bx, true);
+    int rc = make_tmap(&p.tmA, pl->d_table_tf32, 3, d, s, bx);
     if (rc) return rc;
   }
   {
     long long d[3] = {JP, pl->mmax, pl->lmax}, s[3] = {1, JP, (long long)pl->mmax * JP};
     int bx[3] = {32, 1, 32};
-    int rc = make_tmap(&p.tmB, spec, 3, d, s, bx, true);
+    int rc = make_tmap(&p.tmB, spec, 3, d, s, bx);
     if (rc) return rc;
   }
   p.split = spec_lo != nullptr;
@@ -711,37 +603,36 @@ int legendre_synthesis_umma(const Plan* pl, const float* spec, float* Z, int B, 
     B200_REQUIRE(pl->d_table_lo != nullptr, "legendre_synthesis (3 x TF32): the residual table is missing");
     long long d[3] = {pl->nlat, pl->lmax, pl->mmax}, s[3] = {1, pl->kp, (long long)pl->lmax * pl->kp};
     int bx[3] = {32, 32, 1};
-    int rc = make_tmap(&p.tmA_lo, pl->d_table_lo, 3, d, s, bx, true);
+    int rc = make_tmap(&p.tmA_lo, pl->d_table_lo, 3, d, s, bx);
     long long d2[3] = {JP, pl->mmax, pl->lmax}, s2[3] = {1, JP, (long long)pl->mmax * JP};
     int bx2[3] = {32, 1, 32};
-    if (!rc) rc = make_tmap(&p.tmB_lo, spec_lo, 3, d2, s2, bx2, true);
+    if (!rc) rc = make_tmap(&p.tmB_lo, spec_lo, 3, d2, s2, bx2);
     if (rc) return rc;
     p.lo_off = 16384 + 4096 * p.nblk;
   }
   pick_stages(&p, (16384 + 4096 * p.nblk) * (p.split ? 2 : 1), ceil_div(pl->lmax, 32));
   p.tx_bytes = (16384 + 4096 * p.nblk) * (p.split ? 2 : 1);
-  set_accumulators(&p, p.N);
   dim3 grid(ceil_div(k_end - k_begin, 128), ceil_div(JP, p.N), tiled ? 8 * p.M2 : pl->mmax);
   return launch<SynTraits>(p, grid, st);
 }
 
 // --------------------------------------------------------------------------------------------------- mix
-static int spec_tmap(CUtensorMap* tm, const float* base, int L, int M, int B, int Ctot, int cp, int box_c, int box_b, int box_m, bool mn_major = false) {
+static int spec_tmap(CUtensorMap* tm, const float* base, int L, int M, int B, int Ctot, int cp, int box_c, int box_b, int box_m) {
   long long d[5] = {Ctot, B, 2, M, L};
   long long s[5] = {1, cp, (long long)B * cp, 2ll * B * cp, (long long)M * 2 * B * cp};
   int bx[5] = {box_c, box_b, 1, box_m, 1};
-  return make_tmap(tm, base, 5, d, s, bx, mn_major);
+  return make_tmap(tm, base, 5, d, s, bx);
 }
-static int weight_tmap(CUtensorMap* tm, const float* base, int Lw, int G, int Cig, int Cog, int cop, int box_o, int box_i, bool mn_major = false) {
+static int weight_tmap(CUtensorMap* tm, const float* base, int Lw, int G, int Cig, int Cog, int cop, int box_o, int box_i) {
   long long d[4] = {Cog, 2, Cig, (long long)Lw * G};
   long long s[4] = {1, cop, 2ll * cop, (long long)Cig * 2 * cop};
   int bx[4] = {box_o, 1, box_i, 1};
-  return make_tmap(tm, base, 4, d, s, bx, mn_major);
+  return make_tmap(tm, base, 4, d, s, bx);
 }
 
 static int fill_mix(const Plan* pl, int op, int B, int G, int Ci, int Co, MixParams* p) {
-  B200_REQUIRE(B >= 1 && 32 % B == 0, "tcgen05 mix: batch %d must divide 32 (use precision fp32 otherwise)", B);
-  B200_REQUIRE(G == 1 || ((Ci / G) % 4 == 0 && (Co / G) % 4 == 0), "tcgen05 mix: group slices (%d, %d channels) must be 16-byte aligned", Ci / G, Co / G);
+  B200_REQUIRE(B >= 1 && 32 % B == 0, "tensor-core mix: batch %d must divide 32 (use precision fp32 otherwise)", B);
+  B200_REQUIRE(G == 1 || ((Ci / G) % 4 == 0 && (Co / G) % 4 == 0), "tensor-core mix: group slices (%d, %d channels) must be 16-byte aligned", Ci / G, Co / G);
   memset(p, 0, sizeof(*p));
   p->dense = pl->dense;
   p->L = pl->lmax; p->M = pl->mmax; p->B = B; p->G = G; p->Cig = Ci / G; p->Cog = Co / G;
@@ -752,11 +643,10 @@ static int fill_mix(const Plan* pl, int op, int B, int G, int Ci, int Co, MixPar
   return 0;
 }
 
-// Column tiling of a mix GEMM: one tile of up to 256 columns when that covers everything; otherwise equal tiles of at most 128
-// columns (no half-empty last tile -- at C = 384 a 256 + 128 split wasted a quarter of the MMAs -- and 2 N <= 256 TMEM columns per
-// complex accumulator leaves room for two accumulator sets, so the epilogue overlaps the next tile).
+// Column tiling of a mix GEMM: equal tiles of at most 128 columns (no half-empty last tile: at C = 384 a 256 + 128 split wasted a quarter
+// of the MMAs), so that the complex accumulator of a tile, 2 N columns, fits the kMaxCols registers of the consumer warps.
 static void split_cols(int cols, int gran, int* N, int* n_nt) {
-  if (cols <= 256) { *n_nt = 1; *N = round_up(cols, gran); return; }
+  if (cols <= 128) { *n_nt = 1; *N = round_up(cols, gran); return; }
   *n_nt = ceil_div(cols, 128);
   *N = round_up(ceil_div(cols, *n_nt), 32);   // the epilogues drain 32 columns at a time: a tile must not end inside a chunk
 }
@@ -769,15 +659,12 @@ int mix_forward_umma(const Plan* pl, int op, const float* x, const void* w, cons
   const int cols = p.Cog + ((p.cpo - Co) > 0 ? (p.cpo - Co) : 0);   // last group's tile also writes the zero padding
   split_cols(cols, 32, &p.N, &p.n_nt);
   p.nblk = p.N / 32;
-  p.idesc = make_idesc(p.N, 0, 1, 0);
-  p.idesc_neg = make_idesc(p.N, 0, 1, 1);
   p.offA_i = 16384; p.offB_r = 32768; p.offB_i = 32768 + 4096 * p.nblk;
   rc = spec_tmap(&p.tmX, x, p.L, p.M, B, Ci, p.cpi, 32, B, p.Mt);
-  if (!rc) rc = weight_tmap(&p.tmW, static_cast<const float*>(w), p.shared_w ? 1 : p.L, G, p.Cig, p.Cog, p.cop, 32, 32, true);
+  if (!rc) rc = weight_tmap(&p.tmW, static_cast<const float*>(w), p.shared_w ? 1 : p.L, G, p.Cig, p.Cog, p.cop, 32, 32);
   if (rc) return rc;
   pick_stages(&p, 32768 + 8192 * p.nblk, ceil_div(p.Cig, 32));
   p.tx_bytes = 2u * (uint32_t)(p.Mt * B) * 128 + 8192u * p.nblk;
-  set_accumulators(&p, 2 * p.N);
   dim3 grid(ceil_div(p.M, p.Mt), p.n_nt * G, p.L);
   return launch<MixFwdTraits>(p, grid, st);
 }
@@ -792,8 +679,6 @@ int mix_dgrad_umma(const Plan* pl, int op, const void* w, const float* gy, float
   p.out = gx;
   const int cols = p.Cig + ((p.cpi - Ci) > 0 ? (p.cpi - Ci) : 0);
   split_cols(cols, 16, &p.N, &p.n_nt);
-  p.idesc = make_idesc(p.N, 0, 0, 0);
-  p.idesc_neg = make_idesc(p.N, 0, 0, 1);
   const uint32_t bb = (uint32_t)round_up(p.N * 128, 1024);
   p.offA_i = 16384; p.offB_r = 32768; p.offB_i = 32768 + bb;
   rc = spec_tmap(&p.tmX, gy, p.L, p.M, B, Co, p.cpo, 32, B, p.Mt);
@@ -801,7 +686,6 @@ int mix_dgrad_umma(const Plan* pl, int op, const void* w, const float* gy, float
   if (rc) return rc;
   pick_stages(&p, 32768 + 2 * bb, ceil_div(p.Cog, 32));
   p.tx_bytes = 2u * (uint32_t)(p.Mt * B) * 128 + 2u * (uint32_t)p.N * 128;
-  set_accumulators(&p, 2 * p.N);
   dim3 grid(ceil_div(p.M, p.Mt), p.n_nt * G, p.L);
   return launch<MixDgradTraits>(p, grid, st);
 }
@@ -813,15 +697,12 @@ int mix_wgrad_umma(const Plan* pl, int op, const float* x, const float* gy, floa
   p.out = gw;
   split_cols(p.cop, 32, &p.N, &p.n_nt);
   p.nblk = p.N / 32;
-  p.idesc = make_idesc(p.N, 1, 1, 0);
-  p.idesc_neg = make_idesc(p.N, 1, 1, 1);
   p.offA_i = 16384; p.offB_r = 32768; p.offB_i = 32768 + 4096 * p.nblk;
-  rc = spec_tmap(&p.tmX, x, p.L, p.M, B, Ci, p.cpi, 32, B, 32 / B, true);
-  if (!rc) rc = spec_tmap(&p.tmX2, gy, p.L, p.M, B, Co, p.cpo, 32, B, 32 / B, true);
+  rc = spec_tmap(&p.tmX, x, p.L, p.M, B, Ci, p.cpi, 32, B, 32 / B);
+  if (!rc) rc = spec_tmap(&p.tmX2, gy, p.L, p.M, B, Co, p.cpo, 32, B, 32 / B);
   if (rc) return rc;
   pick_stages(&p, 32768 + 8192 * p.nblk, 8);
   p.tx_bytes = 32768u + 8192u * p.nblk;
-  set_accumulators(&p, 2 * p.N);
   dim3 grid(ceil_div(p.Cig, 128), p.n_nt * G, p.shared_w ? 1 : p.L);
   return launch<MixWgradTraits>(p, grid, st);
 }

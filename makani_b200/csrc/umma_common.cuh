@@ -1,5 +1,5 @@
-// tcgen05 / TMA / mbarrier PTX wrappers, UMMA descriptors and the tensor-map helper shared by umma.cu (Legendre + mix engine)
-// and dft.cu (tensor-core longitude DFT).
+// TMA / mbarrier PTX wrappers, TF32 MMA fragments and the tensor-map helper shared by umma.cu (Legendre + mix engine) and dft.cu
+// (tensor-core longitude DFT).
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -96,94 +96,45 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* tm,
 }
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) { asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ------------------------------------------------------------------------------------------- warp-level TF32 MMA
+// Operand tiles are written by TMA with the 128-byte swizzle (16-byte chunk c of a 128-byte row lands at c ^ (row % 8); stage bases are
+// 1024-byte aligned).  Two layouts, both 32 floats wide:
+//   K-major:  row r (an M or N index) holds 32 consecutive K values
+//   MN-major: blocks of [32 K-rows][32 consecutive M / N values], 4096 bytes apart
+// Hopper's wgmma reads TF32 operands from shared memory only K-major; the m16n8k8 fragments below are loaded element by element, so
+// both layouts feed the same instruction.
+template <bool MN>
+__device__ __forceinline__ uint32_t ld_op(const uint8_t* tile, int r, int k) {
+  const uint32_t off = MN ? (uint32_t)((r >> 5) * 4096 + k * 128 + (r & 31) * 4) : (uint32_t)(r * 128 + k * 4);
+  return *reinterpret_cast<const uint32_t*>(tile + (off ^ ((off >> 3) & 0x70u)));
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// A fragment of mma.m16n8k8 (rows r0 + g, r0 + g + 8; K columns k0 + q, k0 + q + 4; g = lane / 4, q = lane % 4)
+template <bool MN>
+__device__ __forceinline__ void frag_a(const uint8_t* tile, int r0, int k0, uint32_t (&a)[4]) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  a[0] = ld_op<MN>(tile, r0 + g, k0 + q);
+  a[1] = ld_op<MN>(tile, r0 + g + 8, k0 + q);
+  a[2] = ld_op<MN>(tile, r0 + g, k0 + q + 4);
+  a[3] = ld_op<MN>(tile, r0 + g + 8, k0 + q + 4);
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], kind::tf32, issued by one thread
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// B fragment (column n0 + g; K rows k0 + q, k0 + q + 4)
+template <bool MN>
+__device__ __forceinline__ void frag_b(const uint8_t* tile, int n0, int k0, uint32_t (&b)[2]) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  b[0] = ld_op<MN>(tile, n0 + g, k0 + q);
+  b[1] = ld_op<MN>(tile, n0 + g, k0 + q + 4);
 }
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void frag_neg(const uint32_t (&a)[4], uint32_t (&n)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) n[i] = a[i] ^ 0x80000000u;   // exact negation: flip the sign bit
 }
-// Warp-synchronous forms: called by all 32 lanes of a converged warp, one elected lane issues.  Under `if (lane == 0)` the compiler wraps
-// every UTCHMMA / UTCBAR in a five-instruction lane-serialising loop (the instruction is uniform, the predicate is not); with elect.sync it
-// emits the instruction alone.
-__device__ __forceinline__ void umma_tf32_ws(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, e;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// d += a * b; the accumulator element e of the fragment is (row g + 8 (e / 2), column 2 q + e % 2).  The tensor core reads the TF32 part of
+// each operand (the 13 low mantissa bits are ignored), so producers of operands round first.
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
-__device__ __forceinline__ void umma_commit_ws(uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(smem_u32(bar))
-      : "memory");
-}
-// 32 consecutive accumulator columns of this thread's TMEM lane
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, "
-      "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-        "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ------------------------------------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start address, LBO, SBO (all >> 4), version = 1 (bit 46),
-// layout type SWIZZLE_128B = 2 (bits 61..63).
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint64_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 46;
-  d |= layout_type << 61;
-  return d;
-}
-// Descriptor of the same operand `bytes` further on in shared memory: one 32-bit add on the address field.  (Rebuilding a descriptor
-// from an address costs ~5 uniform-datapath instructions; a single thread issuing 16 MMAs per stage was spending most of its time there.)
-__device__ __forceinline__ uint64_t desc_advance(uint64_t d, uint32_t bytes) {
-  return (d & 0xffffffff00000000ull) | (uint64_t)((uint32_t)d + (bytes >> 4));
-}
-// K-major operand tile: rows of 128 B (32 floats of K), 8-row groups 1024 B apart.  kstep selects the K = 8 slice (32 B).
-__device__ __forceinline__ uint64_t desc_kmajor(uint32_t tile, int kstep) { return make_smem_desc(tile + kstep * 32, 16, 1024, 2 /*SWIZZLE_128B*/); }
-// MN-major operand tile: blocks of [32 K-rows][32 floats of M/N]; blocks `blk_bytes` apart; kstep selects 8 K-rows (1024 B).
-// 32-bit MN-major operands use SWIZZLE_128B_BASE32B (cute: Layout_MN_SW128_32B_Atom, Swizzle<2,5,2>): atoms of 4 K-rows x 128 B,
-// so one K = 8 MMA spans two atoms SBO = 512 B apart; LBO = distance between 32-float M/N blocks.
-__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t tile, int kstep, uint32_t blk_bytes) {
-  return make_smem_desc(tile + kstep * 1024, blk_bytes, 512, 1 /*SWIZZLE_128B_BASE32B*/);
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor), kind::tf32, fp32 accumulate, M = 128.
-__host__ __device__ constexpr uint32_t make_idesc(int N, int a_mn_major, int b_mn_major, int negate_a) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)negate_a << 13) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -193,7 +144,7 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm,
                "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
                : "memory");
 }
-// generic-proxy shared-memory writes -> visible to the async proxy (tcgen05.mma / TMA reads)
+// generic-proxy shared-memory writes -> visible to the async proxy (TMA)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ================================================================================================== host side
@@ -218,7 +169,7 @@ struct TmapKey {
   const void* base;
   long long dims[5], strides[5];
   int box[5];
-  int rank, kind;   // kind: 0 fp32 / 128-byte swizzle, 1 same with 32-byte atoms (MN-major), 2 fp32 rows, 3 bf16 rows, 4 fp32 segments, 5 bf16 segments
+  int rank, kind;   // kind: 0 fp32 / 128-byte swizzle, 4 fp32 segments, 5 bf16 segments
 };
 struct TmapCache {
   static constexpr int kSlots = 128;
@@ -250,11 +201,10 @@ inline void tmap_store(const TmapKey& k, const CUtensorMap* tm, int slot) {
 }
 
 // fp32 tensor map, 128-byte swizzle.  dims[0] is the contiguous dimension; strides (in floats) for dims 1..rank-1.
-// mn_major: the operand is read M/N-major by kind::tf32, which needs the 128-byte swizzle with 32-byte atoms
-inline int make_tmap(CUtensorMap* tm, const void* base, int rank, const long long* dims, const long long* strides, const int* box, bool mn_major = false) {
+inline int make_tmap(CUtensorMap* tm, const void* base, int rank, const long long* dims, const long long* strides, const int* box) {
   TmapKey key;
   memset(&key, 0, sizeof(key));
-  key.base = base; key.rank = rank; key.kind = mn_major ? 1 : 0;
+  key.base = base; key.rank = rank; key.kind = 0;
   for (int i = 0; i < rank; ++i) { key.dims[i] = dims[i]; key.strides[i] = i ? strides[i] : 1; key.box[i] = box[i]; }
   int slot = 0;
   if (tmap_lookup(key, tm, &slot)) return 0;
@@ -273,7 +223,7 @@ inline int make_tmap(CUtensorMap* tm, const void* base, int rank, const long lon
   }
   if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) { set_error("tensor map base is not 16-byte aligned"); return B200SHT_ERR_INVALID; }
   CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   mn_major ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d), rank %d", (int)r, rank); return B200SHT_ERR_CUDA; }
   tmap_store(key, tm, slot);

@@ -1,6 +1,6 @@
 """RealSHT / InverseRealSHT -- drop-in for `torch_harmonics.RealSHT` / `InverseRealSHT` as makani uses them
 (/root/reference/makani/models/networks/sfnonet.py:792-805, /root/reference/makani/models/common/spectral_convolution.py:239-253),
-computed by the hand-written sm_100a kernels in `csrc/` through the C ABI in include/b200sht.h.
+computed by the hand-written sm_90a kernels in `csrc/` through the C ABI in include/b200sht.h.
 
 Same constructor signature, attributes (.nlat .nlon .lmax .mmax .grid .norm .csphase) and call convention:
     RealSHT(nlat, nlon, lmax=None, mmax=None, grid="equiangular", norm="ortho", csphase=True)(x: (..., nlat, nlon)) -> complex (..., lmax, mmax)
@@ -40,7 +40,7 @@ def _dtype_code(dt):
 
 
 def resolve_precision(precision="auto"):
-    """'fp32' -> CUDA-core fp32 FMA; 'tf32' -> tcgen05 TF32; 'fp32x3' -> fp32 operands with the Legendre stages as 3 x TF32 on the
+    """'fp32' -> CUDA-core fp32 FMA; 'tf32' -> tensor-core TF32; 'fp32x3' -> fp32 operands with the Legendre stages as 3 x TF32 on the
     tensor cores (rtol 1e-5 element bound, ~1.7 x faster than 'fp32'; see B200SHT_PREC_FP32X3 in include/b200sht.h); 'auto' follows
     torch.backends.cuda.matmul.allow_tf32, which is how the reference picks its arithmetic (train.py:87 sets allow_tf32=True,
     tests/testutils.py:55-66 disable it)."""
@@ -82,7 +82,7 @@ class Plan:
         self.dft_ok = bool(lib.b200sht_plan_query(handle, 8))
 
     def query(self, what):
-        """b200sht_plan_query: 0 nlat, 1 nlon, 2 lmax, 3 mmax, 4 kp, 5 table bytes, 6 tcgen05 available, 7 m_offset, 8 tensor-core DFT available."""
+        """b200sht_plan_query: 0 nlat, 1 nlon, 2 lmax, 3 mmax, 4 kp, 5 table bytes, 6 tensor-core path available, 7 m_offset, 8 tensor-core DFT available."""
         return int(_lib.load().b200sht_plan_query(self.handle, what))
 
     @classmethod

@@ -38,7 +38,7 @@ _warned_mix_fallback = set()
 
 
 def mix_pack_precision(op, B, G, Ci, Co, precision):
-    """Precision the packed weight must be prepared for.  The tcgen05 channel mix (precision tf32) needs a batch that divides 32 and
+    """Precision the packed weight must be prepared for.  The tensor-core channel mix (precision tf32) needs a batch that divides 32 and
     16-byte aligned group slices; other shapes are served by the fp32 CUDA-core kernels (correct, slower).  In that case the weight is NOT
     rounded to TF32 (the result is then plain fp32, not a mixture) and the user is told once per shape."""
     if precision != _lib.PREC_TF32:

@@ -31,11 +31,11 @@ def timed(fn, n=20):
     return e0.elapsed_time(e1) / n * 1e3
 print("analysis us/launch (profile on):", round(timed(lambda: _lib.call("b200sht_fft_analysis", plan.handle, _ptr(x), 1, B, C, _ptr(lat), 0 | 2, st)), 1))
 print("synthesis us/launch (profile on):", round(timed(lambda: _lib.call("b200sht_fft_synthesis", plan.handle, _ptr(lat), _ptr(y), 1, B, C, _VP(0), 0 | 2, st)), 1))
-ctas = 148
+ctas = torch.cuda.get_device_properties(0).multi_processor_count   # one persistent CTA per SM
 life = a[6] / ctas
 print(f"analysis: CTA lifetime {life:.0f} clk; items {a[7]:.0f}")
-names = ["producers wait samples (per warp)", "producers wait operand stage (per warp)", "loader waits raw stage", "MMA waits operand", "MMA waits accumulator", "epilogue waits accumulator (per warp)"]
-div = [12, 12, 1, 1, 1, 4]
+names = ["producers wait samples (per warp)", "producers wait operand stage (per warp)", "loader waits raw stage", "MMA warps wait operand (per warp)"]
+div = [12, 12, 1, 4]
 for i, nme in enumerate(names):
     print(f"  {nme:45s} {a[i] / ctas / div[i]:10.0f} clk  = {100 * a[i] / ctas / div[i] / life:5.1f}% of the CTA lifetime")
 for _ in range(2):

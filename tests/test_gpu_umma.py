@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 (TF32) path: same checks as test_gpu_parity.py at the tolerance BASELINE.json states for the
+"""GPU parity of the tensor-core (TF32) path: same checks as test_gpu_parity.py at the tolerance BASELINE.json states for the
 reduced-precision path (rtol 1e-3), plus kernel-by-kernel agreement with the fp32 CUDA-core kernels."""
 import os
 import subprocess
@@ -17,12 +17,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def test_tcgen05_path_is_available():
     plan = mb.get_plan(33, 64, 16, 17, "equiangular", True, torch.device(DEV))
-    assert plan.umma_ok, "tcgen05 path unavailable on this device"
+    assert plan.umma_ok, "tensor-core path unavailable on this device"
 
 
 @pytest.mark.parametrize("case", ["small", "odd", "tiles", "wide", "cfg2c"])
 def test_umma_kernels_agree_with_fp32_kernels(case):
-    """each tcgen05 kernel against the fp32 CUDA-core kernel on identical inputs (own process: a trap cannot poison the suite)"""
+    """each tensor-core kernel against the fp32 CUDA-core kernel on identical inputs (own process: a trap cannot poison the suite)"""
     r = subprocess.run([sys.executable, os.path.join(ROOT, "scripts", "umma_diag.py"), "all", case], capture_output=True, text=True, timeout=900)
     print(r.stdout[-3000:])
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-1000:]
