@@ -290,9 +290,9 @@ static int& lat_chunks_forced() {
   return forced;
 }
 // the synthesis pair (Legendre synthesis -> longitude synthesis) can be chunked the same way (B200SHT_LAT_CHUNKS_SYN = n; off by default):
-// its consumer, the DFT kernel, is not HBM-bound, so the gain is the latency of L2 hits only
-static int lat_chunks_syn() {
-  static const int n = [] { const char* e = getenv("B200SHT_LAT_CHUNKS_SYN"); return e ? atoi(e) : 0; }();
+// its consumer, the DFT kernel, is not HBM-bound, so the gain is the latency of L2 hits only.  b200sht_debug_set_lat_chunks_syn changes it.
+static int& lat_chunks_syn() {
+  static int n = [] { const char* e = getenv("B200SHT_LAT_CHUNKS_SYN"); return e ? atoi(e) : 0; }();
   return n;
 }
 static int lat_chunks(const b200sht_plan* pl, int B, int C) {
@@ -704,6 +704,12 @@ int b200sht_debug_set_pdl(int on) {
 int b200sht_debug_set_lat_chunks(int n) {
   const int old = lat_chunks_forced();
   lat_chunks_forced() = n;
+  return old;
+}
+
+int b200sht_debug_set_lat_chunks_syn(int n) {
+  const int old = lat_chunks_syn();
+  lat_chunks_syn() = n;
   return old;
 }
 

@@ -10,6 +10,7 @@ import torch
 import makani_b200 as mb
 from makani_b200 import _lib
 from oracle import makani_oracle as O
+from engine_ref import to_tiled
 from test_gpu_parity import close
 
 pytestmark = pytest.mark.gpu
@@ -32,17 +33,6 @@ CASES = [
 
 def _latview(lat, plan, B, C, mmax):
     return lat[: mmax * 2 * B * C * plan.kp].view(mmax, 2, B * C, plan.kp)
-
-
-def to_tiled(Z, plan):
-    """standard latspec [mmax][2][R][kp] -> the tiled layout [R][kp/8][2][M2][8][8] (orders zero-padded to 8 * M2) that
-    b200sht_legendre_synthesis_tiled writes and b200sht_fft_synthesis(scale_mode | 2) reads (include/b200sht.h)"""
-    mmax, _, R, kp = Z.shape
-    M2 = (mmax + 7) // 8
-    Zp = torch.zeros(8 * M2, 2, R, kp, device=Z.device, dtype=Z.dtype)
-    Zp[:mmax] = Z
-    # (m2, c, p, r, kt, k8) -> (r, kt, p, m2, c, k8)
-    return Zp.view(M2, 8, 2, R, kp // 8, 8).permute(3, 4, 2, 0, 1, 5).contiguous().reshape(-1)
 
 
 @pytest.mark.parametrize("nlat,nlon,mmax,C,dtype", CASES)
@@ -83,7 +73,7 @@ def test_dft_synthesis_gpu(nlat, nlon, mmax, C, dtype):
     Z = torch.randn(mmax, 2, B * C, plan.kp, device=DEV)
     # operands of the kind::tf32 GEMM are TF32 values in the product path (the Legendre epilogue rounds): do the same here
     Z = (Z.view(torch.int32) + 0x1000).bitwise_and(~0x1FFF).view(torch.float32)
-    lat = to_tiled(Z, plan)
+    lat = to_tiled(Z)
     assert lat.numel() == plan.latspec_elems(B, C)
     bias = torch.randn(C, device=DEV)
     Zc = torch.complex(Z[:, 0, :, :nlat], Z[:, 1, :, :nlat]).permute(1, 2, 0).reshape(B, C, nlat, mmax).to(torch.complex128).cpu()
@@ -116,7 +106,7 @@ def test_dft_adjoint_pair_full_size():
     _lib.call("b200sht_fft_analysis", plan.handle, mb.sht._ptr(x), 0, B, C, mb.sht._ptr(lat), 0 | 2, st)
     Ax = _latview(lat, plan, B, C, mmax).clone()
     Z = torch.randn(mmax, 2, B * C, plan.kp, device=DEV)
-    lat2 = to_tiled(Z, plan)
+    lat2 = to_tiled(Z)
     y = torch.empty(B, C, nlat, nlon, device=DEV)
     _lib.call("b200sht_fft_synthesis", plan.handle, mb.sht._ptr(lat2), mb.sht._ptr(y), 0, B, C, mb.sht._VP(0), 1 | 2, st)
     lhs = (Ax[..., :nlat].double() * Z[..., :nlat].double()).sum().item()
@@ -137,6 +127,6 @@ def test_legendre_synthesis_tiled_is_a_relayout(grid, nlat, nlon, lmax, mmax, B,
     til = torch.full((plan.latspec_elems(B, C),), float("nan"), device=DEV)
     _lib.call("b200sht_legendre_synthesis", plan.handle, mb.sht._ptr(sp), mb.sht._ptr(std), B, C, _lib.PREC_TF32, st)
     _lib.call("b200sht_legendre_synthesis_tiled", plan.handle, mb.sht._ptr(sp), mb.sht._ptr(til), B, C, st)
-    ref = to_tiled(_latview(std, plan, B, C, mmax), plan)
+    ref = to_tiled(_latview(std, plan, B, C, mmax))
     assert torch.isfinite(til).all()
     assert torch.equal(til, ref)

@@ -1,0 +1,298 @@
+"""The tensor-core engine (csrc/umma.cu) through the C ABI against fp64 references of its exact operands (tests/engine_ref.py).
+
+TF32 mode: inputs are TF32 values, the weight is packed at TF32 (unpacking it must give tf32_rna(w) bit for bit) and the reference uses
+the table rounded as the plan rounds it, so every product is exact and the only error allowed is the fp32 accumulation (+ one TF32
+rounding where the epilogue rounds): |got - ref| <= r |ref| + (1 + r) c K 2^-24 sum |a||b|, far tighter than a relative-L2 check.
+fp32x3 mode: fp32 operands, the fp32 table, plus a derived term for the omitted lo.lo product.
+
+Inputs the kernels must not read hold NaN (unstored spec entries, latitude padding of the analysis input).  Outputs start as a NaN with
+a fixed payload: stored entries must be finite and in the bound, the padding and the l < m entries exact zeros, everything else
+untouched.  Every mix case asserts that it runs on the tensor cores.  Each case id names the tile boundary it exercises.  Every check
+prints its worst bound ratio and the smallest c it would pass with (run with -s)."""
+import pytest
+import torch
+
+import engine_ref as E
+import makani_b200 as mb
+from makani_b200 import _lib
+from makani_b200.quadrature import _grid_np
+from makani_b200.sht import Plan, _ptr, _stream
+
+pytestmark = pytest.mark.gpu
+DEV = torch.device("cuda", 0)
+SENTINEL = 0x7FC05EED   # quiet NaN with a payload no kernel writes
+TF32, X3, FP32 = _lib.PREC_TF32, _lib.PREC_FP32X3, _lib.PREC_FP32
+
+
+def sentinel(n):
+    return torch.full((n,), SENTINEL, dtype=torch.int32, device=DEV).view(torch.float32)
+
+
+def untouched(t):
+    return bool((t.contiguous().view(torch.int32) == SENTINEL).all())
+
+
+def check(case, what, got, ref, mag, K, r=0.0, extra=0.0, floor=0.0):
+    ratio = E.bound_ratio(got, ref, mag, K, r=r, extra=extra, floor=floor)
+    need = E.needed_c(got, ref, mag, K, r=r, extra=extra, floor=floor)
+    print(f"[engine] {case} {what}: worst ratio {ratio:.3e}, needs c >= {need:.3e} (c = {E.C_ACC})")
+    if ratio > 1.0:
+        g, f = (torch.view_as_real(got), torch.view_as_real(ref)) if torch.is_complex(got) else (got, ref)
+        err = (g.double() - f).abs().flatten()
+        err[~torch.isfinite(err)] = float("inf")
+        i = int(err.argmax())
+        m = mag.double().flatten()[i // 2 if torch.is_complex(got) else i]
+        raise AssertionError(f"{case} {what}: |got - ref| exceeds the bound by {ratio:.3g}x; worst at flat index {i}: got {g.flatten()[i].item()!r}, "
+                             f"ref {f.flatten()[i].item()!r}, sum |a||b| {m.item()!r}")
+
+
+def call(name, *args):
+    _lib.call(name, *args)
+    torch.cuda.synchronize()
+
+
+# ------------------------------------------------------------------------------------------------------ Legendre
+# id, grid, nlat, nlon, lmax, mmax, B, C, m_offset (None: ordinary plan)
+LEG_CASES = [
+    ("one-kblock-one-ltile", "legendre-gauss", 32, 64, 32, 17, 1, 4, None),
+    ("ktail1-lstart32-cppad", "equiangular", 33, 64, 33, 33, 2, 5, None),
+    ("ltiles128+1-kp136-PBc3", "legendre-gauss", 129, 256, 129, 129, 2, 73, None),
+    ("B32-two-pbtiles-JP512", "equiangular", 91, 180, 91, 91, 32, 8, None),
+    ("nct2-JP400", "legendre-gauss", 64, 128, 64, 65, 1, 200, None),
+    ("headline-23kblocks-tail17", "equiangular", 721, 1440, 240, 241, 1, 3, None),
+    ("m0=23", "equiangular", 65, 128, 40, 45 - 23, 2, 5, 23),
+    ("m0=32", "equiangular", 65, 128, 40, 45 - 32, 2, 5, 32),
+]
+
+
+def _plan(grid, nlat, nlon, L, M, m0):
+    if m0 is None:
+        return mb.get_plan(nlat, nlon, L, M, grid, True, DEV), 0
+    cost, w = _grid_np(nlat, grid)
+    return Plan.create_ex(nlat, nlon, L, M, m0, 0, cost, w, True, DEV), m0
+
+
+def check_spec(case, what, sv, ref, mag, K, C, m0=0, dense=False, r=0.0, extra=0.0, zeros=True, floor=0.0):
+    """packed spec output [L][M][2][B][cp]: unstored entries untouched, stored ones in the bound (the padding channels and, with
+    `zeros`, the l < m entries exact zeros)"""
+    L, M = sv.shape[:2]
+    st = E.stored_mask(L, M, m0, dense, device=DEV)
+    assert untouched(sv[~st]), f"{case} {what}: an unstored entry was written"
+    assert (sv[st][..., C:] == 0).all(), f"{case} {what}: channel padding must hold exact zeros"
+    if zeros:
+        assert (sv[E.zero_mask(L, M, m0, dense, device=DEV)] == 0).all(), f"{case} {what}: l < m entries must be exact zeros"
+    check(case, what, sv[st], ref[st], mag[st], K, r=r, extra=extra, floor=floor)
+
+
+@pytest.mark.parametrize("prec", [TF32, X3], ids=["tf32", "fp32x3"])
+@pytest.mark.parametrize("case,grid,nlat,nlon,L,M,B,C,m0", LEG_CASES, ids=[c[0] for c in LEG_CASES])
+def test_legendre_engine(case, grid, nlat, nlon, L, M, B, C, m0, prec):
+    plan, m0 = _plan(grid, nlat, nlon, L, M, m0)
+    assert plan.umma_ok, "tensor-core path unavailable"
+    kp, cp = plan.kp, (C + 3) // 4 * 4
+    split = prec == X3
+    st = _stream(DEV)
+    gen = torch.Generator(device=DEV).manual_seed(1234)
+    T = plan.table() if split else E.tf32_rna(plan.table())
+    rnd = (lambda *s: torch.randn(*s, device=DEV, generator=gen)) if split else (lambda *s: E.rand_tf32(*s, device=DEV, generator=gen))
+    tag = f"{case} {'fp32x3' if split else 'tf32'}"
+    extra = E.SPLIT_TERM if split else 0.0
+    kmul = 3 if split else 1   # hi.hi + hi.lo + lo.hi into one accumulator
+
+    # analysis: latspec [M8][2][B][C][kp] with NaN in the latitude padding and the padding orders
+    lat = torch.full((plan.latspec_elems(B, C),), float("nan"), device=DEV)
+    X = lat[: M * 2 * B * C * kp].view(M, 2, B, C, kp)
+    X[..., :nlat] = rnd(M, 2, B, C, nlat)
+    spec = sentinel(plan.spec_elems(B, C))
+    call("b200sht_legendre_analysis", plan.handle, _ptr(lat), _ptr(spec), B, C, prec, st)
+    ref, mag = E.legendre_analysis_ref(T, X, nlat, cp, m0)
+    check_spec(tag, "analysis", spec.view(L, M, 2, B, cp), ref, mag, kmul * nlat, C, m0, r=0.0 if split else E.R_TF32, extra=extra,
+               floor=E.underflow_floor(kmul * nlat, X[..., :nlat]))
+
+    # synthesis: spec with NaN in the unstored region, zeros where l < m and in the channel padding
+    S = rnd(L, M, 2, B, cp)
+    S[..., C:] = 0
+    S[E.zero_mask(L, M, m0, device=DEV)] = 0
+    S[~E.stored_mask(L, M, m0, device=DEV)] = float("nan")
+    ref, mag, K = E.legendre_synthesis_ref(T, S, C, m0)
+    n = M * 2 * B * C * kp
+    Z = sentinel(plan.latspec_elems(B, C))
+    call("b200sht_legendre_synthesis", plan.handle, _ptr(S), _ptr(Z), B, C, prec, st)
+    assert untouched(Z[n:]), f"{tag}: the padding orders of the standard layout must not be written"
+    Zv = Z[:n].view(M, 2, B, C, kp)
+    assert (Zv[..., nlat:] == 0).all(), f"{tag}: latitude padding rows must be exact zeros"
+    floor = E.underflow_floor(kmul * L, S)
+    check(tag, "synthesis", Zv, ref, mag, kmul * K, extra=extra, floor=floor)
+    if not split and plan.dft_ok:
+        Zt = sentinel(plan.latspec_elems(B, C))
+        call("b200sht_legendre_synthesis_tiled", plan.handle, _ptr(S), _ptr(Zt), B, C, st)
+        R = B * C
+        tK = E.to_tiled(K.expand(M, 2, B, C, kp).reshape(M, 2, R, kp))
+        # padding orders [M, 8 M2) have K = 0: exact zeros
+        check(tag, "synthesis-tiled", Zt, E.to_tiled(ref.view(M, 2, R, kp)), E.to_tiled(mag.view(M, 2, R, kp)), tK, floor=floor)
+        assert (Zt.view(R, kp // 8, 2, -1, 8, 8).permute(3, 4, 2, 0, 1, 5).reshape(-1, 2, R, kp)[M:] == 0).all()
+
+
+# ------------------------------------------------------------------------------------------------------------ mix
+# id, L, M, B, G, Ci, Co, dense
+MIX_CASES = [
+    ("M-crosses-32", 33, 33, 1, 1, 8, 8, False),
+    ("raggedK-73-cppad", 65, 65, 2, 1, 73, 73, False),
+    ("G2-B4-Mt32", 64, 65, 4, 2, 16, 24, False),
+    ("G2-B4-Mt32-dense", 64, 65, 4, 2, 16, 24, True),
+    ("G3-B8-crossgroupK-wgradstride4", 40, 41, 8, 3, 36, 12, False),
+    ("B32-Mt4-one-order-per-wgrad-kblock", 32, 33, 32, 1, 8, 12, False),
+    ("B32-Mt4-dense", 32, 33, 32, 1, 8, 12, True),
+    ("wgrad-rowtiles-dgrad-coltiles-200-136", 64, 65, 1, 1, 200, 136, False),
+    ("three-ragged-coltiles-300-330", 64, 65, 1, 1, 300, 330, False),
+    ("headline-240x241-73", 240, 241, 1, 1, 73, 73, False),
+]
+OPS = {"dhconv": _lib.OP_DHCONV, "ldep": _lib.OP_LDEP, "shared": _lib.OP_SHARED}
+MIX_PARAMS = [pytest.param(*c, op, id=f"{c[0]}-{op}") for c in MIX_CASES for op in OPS if c[4] == 1 or op == "dhconv"]
+
+
+def _native_weight(op, L, G, Ci, Co, gen):
+    shape = {"dhconv": (G, Ci // G, Co // G, L), "ldep": (L, Ci, Co), "shared": (Ci, Co)}[op]
+    return torch.randn(*shape, dtype=torch.complex64, device=DEV, generator=gen)
+
+
+def _spec_input(L, M, B, C, dense, rnd):
+    cp = (C + 3) // 4 * 4
+    s = rnd(L, M, 2, B, cp)
+    s[..., C:] = 0
+    s[E.zero_mask(L, M, 0, dense, device=DEV)] = 0
+    s[~E.stored_mask(L, M, 0, dense, device=DEV)] = float("nan")
+    return s
+
+
+def _run_mix(case, L, M, B, G, Ci, Co, dense, op, tensor_cores):
+    """forward (without and with cbias) and backward (gx, gw, gcbias) of one shape through b200sht_mix_* at PREC_TF32, every output
+    against the fp64 reference.  `tensor_cores`: TF32 operands and weight packed at TF32; otherwise the shape is served by the fp32
+    kernels, so fp32 operands and a weight packed at fp32 (as include/b200sht.h advises for such shapes)"""
+    lib = _lib.load()
+    code = OPS[op]
+    opf = code | (_lib.DENSE_FLAG if dense else 0)
+    st = _stream(DEV)
+    gen = torch.Generator(device=DEV).manual_seed(4321)
+    tf32 = tensor_cores
+    rnd =(lambda *s: E.rand_tf32(*s, device=DEV, generator=gen)) if tf32 else (lambda *s: torch.randn(*s, device=DEV, generator=gen))
+    Cig, Cog = Ci // G, Co // G
+    cpi, cpo, cop = (Ci + 3) // 4 * 4, (Co + 3) // 4 * 4, (Cog + 3) // 4 * 4
+    r = E.R_TF32 if tf32 else 0.0   # the tensor-core forward / dgrad epilogues round to TF32
+
+    wn = _native_weight(op, L, G, Ci, Co, gen)
+    wp = sentinel(int(lib.b200sht_mix_weight_elems(code, L, M, G, Ci, Co)))
+    call("b200sht_mix_weight_pack", code, _ptr(wn), _ptr(wp), L, G, Ci, Co, TF32 if tf32 else FP32, st)
+    wu = torch.empty_like(wn)
+    call("b200sht_mix_weight_unpack", code, _ptr(wp), _ptr(wu), L, G, Ci, Co, st)
+    want = E.tf32_rna(torch.view_as_real(wn)) if tf32 else torch.view_as_real(wn)
+    assert torch.equal(torch.view_as_real(wu).view(torch.int32), want.view(torch.int32)), f"{case}: packed weight != tf32_rna(w)"
+    assert (wp.view(-1, G, Cig, 2, cop)[..., Cog:] == 0).all(), f"{case}: packed-weight padding must be exact zeros"
+
+    x = _spec_input(L, M, B, Ci, dense, rnd)
+    gy = _spec_input(L, M, B, Co, dense, rnd)
+    cb = torch.randn(Co, dtype=torch.complex64, device=DEV, generator=gen)
+    for bias in (None, cb):
+        y = sentinel(L * M * 2 * B * cpo)
+        call("b200sht_mix_forward", L, M, opf, _ptr(x), _ptr(wp), _ptr(bias), _ptr(y), B, G, Ci, Co, TF32, st)
+        ref, mag, K = E.mix_forward_ref(x, wp, G, Ci, Co, cbias=bias, dense=dense)
+        check_spec(case, "forward" + ("+cbias" if bias is not None else ""), y.view(L, M, 2, B, cpo), ref, mag, K, Co, dense=dense, r=r,
+                   zeros=bias is None)
+
+    gx = sentinel(L * M * 2 * B * cpi)
+    gw = sentinel(wp.numel())
+    gcb = sentinel(2 * Co)
+    call("b200sht_mix_backward", L, M, opf, _ptr(x), _ptr(wp), _ptr(gy), _ptr(gx), _ptr(gw), _ptr(gcb), B, G, Ci, Co, TF32, st)
+    ref, mag, K = E.mix_dgrad_ref(gy, wp, G, Ci, Co, dense=dense)
+    check_spec(case, "dgrad", gx.view(L, M, 2, B, cpi), ref, mag, K, Ci, dense=dense, r=r)
+    ref, mag, K = E.mix_wgrad_ref(x, gy, G, Ci, Co, shared=(op == "shared"), dense=dense)
+    check(case, "wgrad", gw.view(ref.shape), ref, mag, K)   # channel padding [Cog, cop): reference and bound 0 -> exact zeros
+    ref, mag, K = E.mix_cbias_grad_ref(gy, Co, dense=dense)
+    check(case, "cbias-grad", torch.view_as_complex(gcb.view(Co, 2)), ref, mag, K)
+
+
+@pytest.mark.parametrize("case,L,M,B,G,Ci,Co,dense,op", MIX_PARAMS)
+def test_mix_engine(case, L, M, B, G, Ci, Co, dense, op):
+    assert _lib.load().b200sht_mix_uses_tensor_cores(OPS[op], B, G, Ci, Co, TF32) == 1, f"{case}: not on the tensor cores"
+    _run_mix(f"{case}-{op}", L, M, B, G, Ci, Co, dense, op, True)
+
+
+@pytest.mark.parametrize("case,L,M,B,G,Ci,Co", [("B3", 33, 33, 3, 1, 8, 8), ("G2-slices5to6", 33, 33, 1, 2, 10, 12)], ids=["B3", "G2-slices5to6"])
+def test_mix_shapes_outside_the_tensor_cores(case, L, M, B, G, Ci, Co):
+    """shapes the tensor-core mix cannot address are served by the fp32 CUDA-core kernels (the route query says so): unrounded fp32
+    weight and operands, no TF32 rounding of the output, same reference and bound"""
+    assert _lib.load().b200sht_mix_uses_tensor_cores(_lib.OP_DHCONV, B, G, Ci, Co, TF32) == 0
+    _run_mix(f"fallback-{case}", L, M, B, G, Ci, Co, False, "dhconv", False)
+
+
+# ------------------------------------------------------------------------------------------------ latitude ranges
+def _workspace(plan, B, C):
+    nbytes = int(_lib.load().b200sht_sht_workspace_bytes(plan.handle, B, C))
+    return sentinel(nbytes // 4)
+
+
+CHUNK_GRIDS = [  # id, grid, nlat, nlon, lmax, mmax, B, C, dtype (the tensor-core DFT takes fp32 rows when nlon % 32 == 0, bf16 otherwise)
+    ("181x360-bf16", "legendre-gauss", 181, 360, 181, 181, 1, 4, torch.bfloat16),
+    ("721x1440", "equiangular", 721, 1440, 240, 241, 1, 3, torch.float32),
+]
+
+
+@pytest.mark.parametrize("n", [2, 3, 5])
+@pytest.mark.parametrize("case,grid,nlat,nlon,L,M,B,C,dtype", CHUNK_GRIDS, ids=[c[0] for c in CHUNK_GRIDS])
+def test_chunked_analysis(case, grid, nlat, nlon, L, M, B, C, dtype, n):
+    """b200sht_sht_forward with the (longitude analysis -> Legendre analysis) pair in n latitude chunks (at most nlat / 64): partial sums
+    per chunk, TF32 rounding on the last.  Operands: the latspec the longitude stage left in the workspace (the same rows as one plain
+    b200sht_fft_analysis) and the TF32 table."""
+    lib = _lib.load()
+    plan = mb.get_plan(nlat, nlon, L, M, grid, True, DEV)
+    assert plan.umma_ok and plan.dft_ok
+    kp, cp = plan.kp, (C + 3) // 4 * 4
+    st = _stream(DEV)
+    torch.manual_seed(99)
+    x = torch.randn(B, C, nlat, nlon, device=DEV).to(dtype)
+    code = mb.sht._dtype_code(dtype)
+    nl = M * 2 * B * C * kp
+    lat0 = torch.full((plan.latspec_elems(B, C),), float("nan"), device=DEV)
+    call("b200sht_fft_analysis", plan.handle, _ptr(x), code, B, C, _ptr(lat0), 0 | 2, st)
+    ws = _workspace(plan, B, C)
+    coeffs = torch.empty(B, C, L, M, dtype=torch.complex64, device=DEV)
+    old = lib.b200sht_debug_set_lat_chunks(n)
+    try:
+        call("b200sht_sht_forward", plan.handle, _ptr(x), code, B, C, _ptr(coeffs), _ptr(ws), TF32, st)
+    finally:
+        lib.b200sht_debug_set_lat_chunks(old)
+    X = ws[:nl].view(M, 2, B, C, kp)
+    X0 = lat0[:nl].view(M, 2, B, C, kp)
+    assert torch.equal(X[..., :nlat].view(torch.int32), X0[..., :nlat].view(torch.int32)), "chunked latspec rows != plain fft_analysis"
+    spec_off = (4 * plan.latspec_elems(B, C) + 255) // 256 * 256 // 4
+    sv = ws[spec_off : spec_off + plan.spec_elems(B, C)].view(L, M, 2, B, cp)
+    ref, mag = E.legendre_analysis_ref(E.tf32_rna(plan.table()), E.tf32_trunc(X), nlat, cp)
+    check_spec(f"{case} chunks={n}", "analysis", sv, ref, mag, nlat, C, r=E.R_TF32, floor=E.underflow_floor(nlat, X[..., :nlat]))
+    tri = torch.tril(torch.ones(L, M, dtype=torch.bool, device=DEV))
+    want = torch.where(tri, torch.complex(sv[:, :, 0, :, :C], sv[:, :, 1, :, :C]).permute(2, 3, 0, 1), 0)
+    assert torch.equal(coeffs, want), "coefficients != the packed spectrum in the workspace"
+
+
+@pytest.mark.parametrize("case,grid,nlat,nlon,L,M,B,C,dtype", CHUNK_GRIDS, ids=[c[0] for c in CHUNK_GRIDS])
+def test_chunked_synthesis_is_bit_identical(case, grid, nlat, nlon, L, M, B, C, dtype):
+    """b200sht_sht_inverse / _forward_adjoint with the (Legendre synthesis -> longitude synthesis) pair in 2 or 3 chunks of whole
+    128-row tiles compute every output row exactly as the unchunked call"""
+    lib = _lib.load()
+    plan = mb.get_plan(nlat, nlon, L, M, grid, True, DEV)
+    assert plan.dft_ok and plan.kp > 128
+    st = _stream(DEV)
+    torch.manual_seed(98)
+    c = torch.randn(B, C, L, M, dtype=torch.complex64, device=DEV)
+    for fn in ("b200sht_sht_inverse", "b200sht_sht_forward_adjoint"):
+        ys = []
+        for n in (1, 2, 3):
+            y = torch.full((B, C, nlat, nlon), float("nan"), device=DEV)
+            old = lib.b200sht_debug_set_lat_chunks_syn(n)
+            try:
+                call(fn, plan.handle, _ptr(c), _ptr(y), _lib.F32, B, C, _ptr(_workspace(plan, B, C)), TF32, st)
+            finally:
+                lib.b200sht_debug_set_lat_chunks_syn(old)
+            assert torch.isfinite(y).all()
+            ys.append(y)
+        for n, y in zip((2, 3), ys[1:]):
+            assert torch.equal(y, ys[0]), f"{fn}: {n} latitude chunks changed the result"

@@ -1,31 +1,20 @@
 """GPU parity of the tensor-core (TF32) path: same checks as test_gpu_parity.py at the tolerance BASELINE.json states for the
-reduced-precision path (rtol 1e-3), plus kernel-by-kernel agreement with the fp32 CUDA-core kernels."""
-import os
-import subprocess
-import sys
-
+reduced-precision path (rtol 1e-3).  The tensor-core kernels one by one, against fp64 references of their exact operands, are in
+test_gpu_engine.py."""
 import pytest
 import torch
 
 import makani_b200 as mb
+from makani_b200 import _lib
 from test_gpu_parity import CONV_CASES, SHT_CASES, _run_conv_case, close, oracle_pair
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_tcgen05_path_is_available():
     plan = mb.get_plan(33, 64, 16, 17, "equiangular", True, torch.device(DEV))
     assert plan.umma_ok, "tensor-core path unavailable on this device"
-
-
-@pytest.mark.parametrize("case", ["small", "odd", "tiles", "wide", "cfg2c"])
-def test_umma_kernels_agree_with_fp32_kernels(case):
-    """each tensor-core kernel against the fp32 CUDA-core kernel on identical inputs (own process: a trap cannot poison the suite)"""
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "scripts", "umma_diag.py"), "all", case], capture_output=True, text=True, timeout=900)
-    print(r.stdout[-3000:])
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-1000:]
 
 
 @pytest.mark.parametrize("grid,nlat,nlon,lmax,mmax,B,C", SHT_CASES)
@@ -40,8 +29,15 @@ def test_real_sht_tf32(grid, nlat, nlon, lmax, mmax, B, C):
     close(isht(cin.to(DEV)), oisht(cin.to(torch.complex128)), 1e-3, f"InverseRealSHT tf32 {grid} {nlat}x{nlon}")
 
 
-@pytest.mark.parametrize("case", CONV_CASES[:3])
+# grouped dhconv whose group slices and batch the tensor-core mix addresses (G = 2, 16 -> 24 channels, B = 4)
+GROUPED_TC_CASE = (48, 96, "legendre-gauss", 48, 96, "legendre-gauss", 32, 33, 4, 16, 24, 2, "dhconv", False, True)
+
+
+@pytest.mark.parametrize("case", CONV_CASES[:3] + [GROUPED_TC_CASE])
 def test_spectral_conv_fwd_bwd_tf32(case):
+    if case == GROUPED_TC_CASE:
+        B, Cin, Cout, G = case[8:12]
+        assert _lib.load().b200sht_mix_uses_tensor_cores(_lib.OP_DHCONV, B, G, Cin, Cout, _lib.PREC_TF32) == 1
     _run_conv_case(case, "tf32", 1e-3)
 
 
