@@ -1,9 +1,10 @@
 // Tensor-core path (B200SHT_PREC_TF32): the Legendre contractions and the dense channel mix as TMA-fed TF32 GEMMs with fp32
 // accumulation.
 //
-//   one persistent engine (umma_kernel<Traits>, one CTA per SM walking the tile list): warp 0 lane 0 = TMA producer, warps 1..8 =
-//   consumers; consumer warp w owns rows 16 (w - 1) .. + 15 of the 128-row tile, issues mma.m16n8k8 (TF32) on them against every column
-//   of the tile and stores its accumulators itself.  A ring of `stages` operand stages guarded by full/empty mbarriers runs continuously
+//   one persistent engine (umma_kernel<Traits, NB, SPLIT>, one CTA per SM walking the tile list): warp 0 lane 0 = TMA producer, warps
+//   1..8 = consumers; consumer warp w owns rows 16 (w - 1) .. + 15 of the 128-row tile, issues mma.m16n8k8 (TF32) on them against every
+//   column of the tile and stores its accumulators itself.  The tile width (NB fragments of 8 columns) and the 3 x TF32 mode are template
+//   parameters: the MMA loop is straight-line code without per-fragment predicates, and no instantiation spills registers.  A ring of `stages` operand stages guarded by full/empty mbarriers runs continuously
 //   across tiles, so the producer prefetches the next tile while the consumers finish the current one and write it out.
 //
 //   five Traits supply the per-operation pieces (tile coordinates, TMA boxes, MMA list, epilogue):
@@ -13,9 +14,12 @@
 //     MixDgrad    gx[row][i]     = sum_o gy[row][o] conj(w[i][o])       A K-major,  B K-major
 //     MixWgrad    gw[i][o]       = sum_row conj(x[row][i]) gy[row][o]   A MN-major, B MN-major
 //   complex products use planar operands: 4 real MMAs into two accumulators (real, imaginary), negated terms through a sign flip of
-//   the A fragment.
+//   a fragment.
 //
-// All shared-memory operand tiles use the 128-byte swizzle; every TMA box is [rows][32 floats] so it lands as rows of 128 B.  wgmma is
+// All shared-memory operand tiles use the 128-byte swizzle; every TMA box is [rows][32 floats] so it lands as rows of 128 B.  Fragments
+// are read with 8- and 16-byte shared loads, conflict-free: within each 32-wide stage the K order, and for MN-major operands the row /
+// column order, is permuted so that each thread's operands are contiguous (layouts KK / MM / KM below); the epilogues undo the
+// permutation and store 8- or 16-byte vectors where the output is contiguous along the permuted index.  wgmma is
 // not used: it reads TF32 operands from shared memory only K-major, and synthesis (A and B), mix forward (B) and wgrad (A and B) have
 // MN-major operands; B cannot come from registers.  A register-sourced-A wgmma would serve the K-major analysis and dgrad GEMMs; it is
 // not built, and the H100 cost of this engine is recorded in DESIGN.md section 9.
@@ -28,7 +32,6 @@ namespace b200sht {
 constexpr int kConsumerWarps = 8;                         // 8 x 16 rows = the 128-row tile
 constexpr int kUmmaThreads = 32 * (1 + kConsumerWarps);   // warp 0: TMA producer, warps 1..8: MMA + epilogue
 constexpr int kMaxStages = 8;
-constexpr int kMaxCols = 256;                             // accumulator columns of a tile (a complex tile: 2 x 128)
 
 struct EngineParams {
   int stages;
@@ -38,77 +41,221 @@ struct EngineParams {
   uint32_t lo_off;         // bytes after the main tiles, and each MMA becomes hi.hi + hi.lo + lo.hi into the same accumulator
 };
 
-// Accumulators of one consumer warp: 16 rows x kMaxCols columns as m16n8 fragments, acc[j] = columns 8 j .. 8 j + 7.  Complex tiles keep the
-// real part in acc[0 .. 15] and the imaginary part in acc[16 .. 31].
-typedef float Acc[kMaxCols / 8][4];
+// ------------------------------------------------------------------------------------------- fragment layouts
+// The engine is instantiated for a compile-time number NB of 8-column fragments per warp (the host pads N up to a built width; padded
+// columns read zeros or stale shared memory and are never stored).  A warp's accumulator is float acc[NB][4] (real) or acc[2 NB][4]
+// (complex: real part in 0 .. NB-1, imaginary part in NB .. 2 NB-1).  K is summed over, so the 32 K of a stage may be visited in any order
+// that is the same for both operands, and the rows / columns of a fragment may be any rows / columns of the tile as long as the epilogue
+// maps them back.  Three layouts, chosen per GEMM so that every fragment load is 8 or 16 bytes and bank-conflict-free under the 128-byte
+// swizzle (g = lane / 4, q = lane % 4; the MMA's K positions q, q + 4 of k8 step s are called (s, q, h = 0 / 1)):
+//   KK (both operands K-major: analysis, dgrad)   (s, q, h) -> K 8 q + 2 s + h: thread q owns K 8q .. 8q+7 of every row, two 16-byte loads
+//        per row and stage (one per pair of k8 steps); rows / columns are the plain m16n8 ones.
+//   MM (both operands MN-major: synthesis, wgrad) (s, q, h) -> K 8 s + 2 q + h.  A: the warp's rows g, g + 8 are adjacent physical rows
+//        2g, 2g + 1 (one 8-byte load per K row); B: column g of fragments 4J .. 4J + 3 is physical column 32 J + 4 g .. + 3 (one 16-byte
+//        load serves four fragments).
+//   KM (A K-major, B MN-major: mix forward)        K as MM, B as MM; A: one 8-byte load per row and k8 step, rows g, g + 8 at physical
+//        2 (g % 4) + g / 4 and that + 8, so that the eight rows of a load phase fall on distinct chunks after the swizzle.
+enum class Lay { KK, MM, KM };
 
-// acc[j] += A(rows row0 .. + 15) B(columns 8 j .. + 7) over the 32 K of one stage, j < nb
-template <bool AMN, bool BMN>
-__device__ __forceinline__ void gemm_real(const uint8_t* a, const uint8_t* b, int row0, int nb, Acc& acc) {
+// tile row of accumulator element e (0..3) of this lane: rows of a fragment are g (e < 2) and g + 8 (e >= 2)
+template <Lay L>
+__device__ __forceinline__ int frag_row(int row0, int h) {
+  const int g = (threadIdx.x & 31) >> 2;
+  if (L == Lay::KK) return row0 + g + 8 * h;
+  if (L == Lay::MM) return row0 + 2 * g + h;
+  return row0 + 2 * (g & 3) + (g >> 2) + 8 * h;
+}
+
+// A fragments of one stage, KK: f[t] = k8 step 2 hh + t
+__device__ __forceinline__ void lda_kk(const uint8_t* a, int row0, int hh, uint32_t (&f)[2][4]) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  const uint32_t ko = (8 * q + 4 * hh) * 4;
+  const uint4 x = lds128(a, (row0 + g) * 128 + ko), y = lds128(a, (row0 + g + 8) * 128 + ko);
+  f[0][0] = x.x; f[0][1] = y.x; f[0][2] = x.y; f[0][3] = y.y;
+  f[1][0] = x.z; f[1][1] = y.z; f[1][2] = x.w; f[1][3] = y.w;
+}
+// B fragment j, KK: f[t] = k8 step 2 hh + t
+__device__ __forceinline__ void ldb_kk(const uint8_t* b, int j, int hh, uint32_t (&f)[2][2]) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  const uint4 x = lds128(b, (8 * j + g) * 128 + (8 * q + 4 * hh) * 4);
+  f[0][0] = x.x; f[0][1] = x.y; f[1][0] = x.z; f[1][1] = x.w;
+}
+// A fragment of k8 step s, MM (MN-major, [32 K][32 M] blocks of 4096 bytes)
+__device__ __forceinline__ void lda_mm(const uint8_t* a, int row0, int s, uint32_t (&f)[4]) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  const uint32_t o = (row0 >> 5) * 4096 + (8 * s + 2 * q) * 128 + ((row0 & 31) + 2 * g) * 4;
+  const uint2 x = lds64(a, o), y = lds64(a, o + 128);
+  f[0] = x.x; f[1] = x.y; f[2] = y.x; f[3] = y.y;
+}
+// A fragment of k8 step s, KM (K-major rows)
+__device__ __forceinline__ void lda_km(const uint8_t* a, int row0, int s, uint32_t (&f)[4]) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  const uint32_t o = (row0 + 2 * (g & 3) + (g >> 2)) * 128 + (8 * s + 2 * q) * 4;
+  const uint2 x = lds64(a, o), y = lds64(a, o + 8 * 128);
+  f[0] = x.x; f[1] = y.x; f[2] = x.y; f[3] = y.y;
+}
+// B fragments 4 J .. 4 J + 3 of k8 step s, MM / KM (MN-major)
+__device__ __forceinline__ void ldb_mn(const uint8_t* b, int J, int s, uint32_t (&f)[4][2]) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  const uint32_t o = J * 4096 + (8 * s + 2 * q) * 128 + g * 16;
+  const uint4 x = lds128(b, o), y = lds128(b, o + 128);
+  f[0][0] = x.x; f[0][1] = y.x; f[1][0] = x.y; f[1][1] = y.y;
+  f[2][0] = x.z; f[2][1] = y.z; f[3][0] = x.w; f[3][1] = y.w;
+}
+template <int S>
+__device__ __forceinline__ void sgn(const uint32_t (&a)[4], uint32_t (&o)[4]) {   // exact negation for S < 0: flip the sign bits
 #pragma unroll
-  for (int kk = 0; kk < 32; kk += 8) {
-    uint32_t fa[4];
-    frag_a<AMN>(a, row0, kk, fa);
+  for (int i = 0; i < 4; ++i) o[i] = S > 0 ? a[i] : a[i] ^ 0x80000000u;
+}
+
+template <int S>
+__device__ __forceinline__ void sgn2(const uint32_t (&b)[2], uint32_t (&o)[2]) {
+  o[0] = S > 0 ? b[0] : b[0] ^ 0x80000000u;
+  o[1] = S > 0 ? b[1] : b[1] ^ 0x80000000u;
+}
+
+// acc[j] += A(the warp's 16 rows) B(fragment j) over the 32 K of one stage.  SPLIT (3 x TF32): the residual tiles lie `lo` bytes after A and
+// B, and every product becomes hi.hi + hi.lo + lo.hi, issued per fragment so that no operand is loaded twice.
+template <Lay L, int NB, bool SPLIT>
+__device__ __forceinline__ void gemm_real(const uint8_t* a, const uint8_t* b, uint32_t lo, int row0, float (&acc)[NB][4]) {
+  if constexpr (L == Lay::KK) {
+    // fragments per batch of B loads, so that consecutive MMAs go to different accumulators (fewer when the accumulators leave few registers)
+    constexpr int CH = (SPLIT || NB > 24) ? 1 : (NB % 4 == 0 && NB <= 20) ? 4 : 2;
+    static_assert(NB % CH == 0, "KK: NB must be even");
+#pragma unroll(NB > 24 ? 1 : 2)
+    for (int hh = 0; hh < 2; ++hh) {
+      uint32_t fa[2][4], la[2][4];
+      lda_kk(a, row0, hh, fa);
+      if (SPLIT) lda_kk(a + lo, row0, hh, la);
 #pragma unroll
-    for (int j = 0; j < kMaxCols / 8; ++j) {
-      if (j < nb) {
-        uint32_t fb[2];
-        frag_b<BMN>(b, 8 * j, kk, fb);
-        mma_tf32(acc[j], fa, fb);
+      for (int j0 = 0; j0 < NB; j0 += CH) {
+        uint32_t fb[CH][2][2], lb[CH][2][2];
+#pragma unroll
+        for (int c = 0; c < CH; ++c) {
+          ldb_kk(b, j0 + c, hh, fb[c]);
+          if (SPLIT) ldb_kk(b + lo, j0 + c, hh, lb[c]);
+        }
+#pragma unroll
+        for (int t = 0; t < 2; ++t)
+#pragma unroll
+          for (int c = 0; c < CH; ++c) {
+            mma_tf32(acc[j0 + c], fa[t], fb[c][t]);
+            if (SPLIT) { mma_tf32(acc[j0 + c], fa[t], lb[c][t]); mma_tf32(acc[j0 + c], la[t], fb[c][t]); }
+          }
+      }
+    }
+  } else {
+    static_assert(NB % 4 == 0, "MN-major B: NB must be a multiple of 4");
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      uint32_t fa[4], la[4];
+      if (L == Lay::MM) { lda_mm(a, row0, s, fa); if (SPLIT) lda_mm(a + lo, row0, s, la); }
+      else { lda_km(a, row0, s, fa); if (SPLIT) lda_km(a + lo, row0, s, la); }
+#pragma unroll
+      for (int J = 0; J < NB / 4; ++J) {
+        uint32_t fb[4][2], lb[4][2];
+        ldb_mn(b, J, s, fb);
+        if (SPLIT) ldb_mn(b + lo, J, s, lb);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          mma_tf32(acc[4 * J + c], fa, fb[c]);
+          if (SPLIT) { mma_tf32(acc[4 * J + c], fa, lb[c]); mma_tf32(acc[4 * J + c], la, fb[c]); }
+        }
       }
     }
   }
 }
-// complex product of planar operands, S1..S3 = +-1:  re += ar br + S1 ai bi,  im += S2 ar bi + S3 ai br  (j < nb <= 16)
-template <bool AMN, bool BMN, int S1, int S2, int S3>
-__device__ __forceinline__ void gemm_cplx(const uint8_t* ar, const uint8_t* ai, const uint8_t* br, const uint8_t* bi, int row0, int nb, Acc& acc) {
+// complex product of planar operands over one stage (S1..S3 = +-1):  re += ar br + S1 ai bi,  im += S2 ar bi + S3 ai br.  The signs go on
+// the A fragments (MN-major B: a B load holds four fragments) or on the B fragment (KK); the two B planes are consumed one after the
+// other, so only one is held at a time.
+template <Lay L, int NB, int S1, int S2, int S3>
+__device__ __forceinline__ void gemm_cplx(const uint8_t* ar, const uint8_t* ai, const uint8_t* br, const uint8_t* bi, int row0, float (&acc)[2 * NB][4]) {
+  if constexpr (L == Lay::KK) {
 #pragma unroll
-  for (int kk = 0; kk < 32; kk += 8) {
-    uint32_t fr[4], fi[4], nr[4], ni[4];
-    frag_a<AMN>(ar, row0, kk, fr);
-    frag_a<AMN>(ai, row0, kk, fi);
-    frag_neg(fr, nr);
-    frag_neg(fi, ni);
+    for (int hh = 0; hh < 2; ++hh) {
+      uint32_t fr[2][4], fi[2][4];
+      lda_kk(ar, row0, hh, fr);
+      lda_kk(ai, row0, hh, fi);
 #pragma unroll
-    for (int j = 0; j < kMaxCols / 16; ++j) {
-      if (j < nb) {
-        uint32_t gr[2], gi[2];
-        frag_b<BMN>(br, 8 * j, kk, gr);
-        frag_b<BMN>(bi, 8 * j, kk, gi);
-        mma_tf32(acc[j], fr, gr);
-        mma_tf32(acc[j], S1 > 0 ? fi : ni, gi);
-        mma_tf32(acc[16 + j], S2 > 0 ? fr : nr, gi);
-        mma_tf32(acc[16 + j], S3 > 0 ? fi : ni, gr);
+      for (int j = 0; j < NB; ++j) {   // here the signs go on the B fragment (two registers per k8 step)
+        uint32_t g[2][2];
+        ldb_kk(br, j, hh, g);
+#pragma unroll
+        for (int t = 0; t < 2; ++t) {
+          uint32_t x[2];
+          sgn2<S3>(g[t], x);
+          mma_tf32(acc[j], fr[t], g[t]);
+          mma_tf32(acc[NB + j], fi[t], x);
+        }
+        ldb_kk(bi, j, hh, g);
+#pragma unroll
+        for (int t = 0; t < 2; ++t) {
+          uint32_t x[2], y[2];
+          sgn2<S1>(g[t], x);
+          sgn2<S2>(g[t], y);
+          mma_tf32(acc[j], fi[t], x);
+          mma_tf32(acc[NB + j], fr[t], y);
+        }
+      }
+    }
+  } else {
+    static_assert(NB % 4 == 0, "MN-major B: NB must be a multiple of 4");
+#pragma unroll 1   // one k8 step at a time: unrolled, the loads of the next steps are hoisted and the accumulators spill
+    for (int s = 0; s < 4; ++s) {
+      uint32_t fr[4], fi[4], x[4];
+      if (L == Lay::MM) { lda_mm(ar, row0, s, fr); lda_mm(ai, row0, s, fi); }
+      else { lda_km(ar, row0, s, fr); lda_km(ai, row0, s, fi); }
+#pragma unroll
+      for (int J = 0; J < NB / 4; ++J) {
+        uint32_t g[4][2];
+        ldb_mn(br, J, s, g);
+        sgn<S3>(fi, x);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) { mma_tf32(acc[4 * J + c], fr, g[c]); mma_tf32(acc[NB + 4 * J + c], x, g[c]); }
+        ldb_mn(bi, J, s, g);
+        uint32_t y[4];
+        sgn<S1>(fi, x);
+        sgn<S2>(fr, y);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) { mma_tf32(acc[4 * J + c], x, g[c]); mma_tf32(acc[NB + 4 * J + c], y, g[c]); }
       }
     }
   }
 }
-// f(row, column, value) for every accumulator element of the warp (rows row0 + lane / 4 (+ 8), columns < 8 nb)
-template <class F>
-__device__ __forceinline__ void for_each_acc(const Acc& acc, int row0, int nb, F f) {
-  const int lane = threadIdx.x & 31;
+
+// f(h, col, re[V], im[V]) for every run of V contiguous tile columns this lane holds in tile row frag_row<L>(row0, h): V = 2 in KK (columns
+// 8 j + 2 q, + 1), V = 4 in MM / KM (columns 32 J + 8 q + 4 e .. + 3 from fragments 4 J .. 4 J + 3).  im is the imaginary part of a
+// complex accumulator (NA = 2 NB) and unused otherwise.
+template <Lay L, int NB, int NA, class F>
+__device__ __forceinline__ void for_each_run(const float (&acc)[NA][4], F f) {
+  const int q = threadIdx.x & 3;
+  constexpr int IM = NA == 2 * NB ? NB : 0;
+  if constexpr (L == Lay::KK) {
 #pragma unroll
-  for (int j = 0; j < kMaxCols / 8; ++j)
-    if (j < nb) {
+    for (int j = 0; j < NB; ++j)
 #pragma unroll
-      for (int e = 0; e < 4; ++e) f(row0 + (lane >> 2) + 8 * (e >> 1), 8 * j + 2 * (lane & 3) + (e & 1), acc[j][e]);
-    }
-}
-// same for a complex accumulator: f(row, column, real, imaginary), nb <= 16
-template <class F>
-__device__ __forceinline__ void for_each_cacc(const Acc& acc, int row0, int nb, F f) {
-  const int lane = threadIdx.x & 31;
+      for (int h = 0; h < 2; ++h) {
+        const float re[2] = {acc[j][2 * h], acc[j][2 * h + 1]}, im[2] = {acc[IM + j][2 * h], acc[IM + j][2 * h + 1]};
+        f(h, 8 * j + 2 * q, re, im);
+      }
+  } else {
 #pragma unroll
-  for (int j = 0; j < kMaxCols / 16; ++j)
-    if (j < nb) {
+    for (int J = 0; J < NB / 4; ++J)
 #pragma unroll
-      for (int e = 0; e < 4; ++e) f(row0 + (lane >> 2) + 8 * (e >> 1), 8 * j + 2 * (lane & 3) + (e & 1), acc[j][e], acc[16 + j][e]);
-    }
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 2 * h + e;
+          const float re[4] = {acc[4 * J][x], acc[4 * J + 1][x], acc[4 * J + 2][x], acc[4 * J + 3][x]};
+          const float im[4] = {acc[IM + 4 * J][x], acc[IM + 4 * J + 1][x], acc[IM + 4 * J + 2][x], acc[IM + 4 * J + 3][x]};
+          f(h, 32 * J + 8 * q + 4 * e, re, im);
+        }
+  }
 }
 
 // Persistent engine: one CTA per SM loops over tiles.  The operand ring (full/empty) runs continuously across tiles, so the
-// TMA producer prefetches the next tile while the consumer warps finish the current one.
-template <class T>
+// TMA producer prefetches the next tile while the consumer warps finish the current one.  NB: 8-column fragments per warp; SPLIT: 3 x TF32.
+template <class T, int NB, bool SPLIT>
 __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_constant__ typename T::Params p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -153,17 +300,17 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_cons
       typename T::Tile tile;
       if (!T::make_tile(p, tile, ti % p.gx, (ti / p.gx) % p.gy, ti / (p.gx * p.gy))) continue;
       const int nk = T::num_kblocks(p, tile);
-      Acc acc;
+      float acc[NB * T::kPlanes][4];
 #pragma unroll
-      for (int j = 0; j < kMaxCols / 8; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+      for (int j = 0; j < NB * T::kPlanes; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
       for (int kb = 0; kb < nk; ++kb, ++kbg) {
         const int s = kbg % stages, it = kbg / stages;
         mbar_wait(&full[s], it & 1);
-        T::mma(p, gbase + (size_t)s * stage_bytes, row0, acc);
+        T::template mma<NB, SPLIT>(p, gbase + (size_t)s * stage_bytes, row0, acc);
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[s]);   // this warp's reads of the stage are done
       }
-      T::epilogue(p, tile, row0, acc);
+      T::template epilogue<NB>(p, tile, row0, acc);
     }
   }
 }
@@ -179,6 +326,7 @@ struct AnaTraits {
     int kb0, nkb;        // latitude range of this launch in 32-row K-blocks (latitude-chunked analysis: partial sums over a chunk of rows)
     int acc_in, round_out;   // add to the spec values already stored (chunks after the first) / round the result to TF32 (last chunk)
   };
+  static constexpr int kPlanes = 1;
   struct Tile { int m, l0, c0, pb0; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.m = bz;
@@ -198,28 +346,29 @@ struct AnaTraits {
       tma_load_4d(st + p.lo_off + 16384, &p.tmB_lo, bar, kb * 32, t.c0, t.pb0, t.m);
     }
   }
-  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, Acc& acc) {
-    const int nb = p.N / 8;
-    gemm_real<false, false>(st, st + 16384, row0, nb, acc);
-    if (p.split) {
-      gemm_real<false, false>(st, st + p.lo_off + 16384, row0, nb, acc);   // hi . lo
-      gemm_real<false, false>(st + p.lo_off, st + 16384, row0, nb, acc);   // lo . hi
-    }
+  template <int NB, bool SPLIT>
+  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, float (&acc)[NB][4]) {
+    gemm_real<Lay::KK, NB, SPLIT>(st, st + 16384, p.lo_off, row0, acc);
   }
-  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const Acc& acc) {
+  // column n = pbi * Cc + ci of the tile; Cc and cp are multiples of 4, so the column pair (n, n + 1) of a run is one float2 of spec
+  template <int NB>
+  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const float (&acc)[NB][4]) {
     const int ncols = p.Cc * p.PBc;
     const size_t JP = (size_t)p.PB * p.cp;
-    for_each_acc(acc, row0, p.N / 8, [&](int r, int n, float v) {
-      const int l = t.l0 + r;
+    const int l0 = t.l0 + frag_row<Lay::KK>(row0, 0);
+    for_each_run<Lay::KK, NB>(acc, [&](int h, int n, const float (&v)[2], const float (&)[2]) {
+      const int l = l0 + 8 * h;
       if (l >= p.L || n >= ncols) return;
       const int pbi = n / p.Cc, ci = n - pbi * p.Cc;
       const int pb = t.pb0 + pbi, c = t.c0 + ci;
       if (pb >= p.PB || c >= p.cp) return;
-      float* dst = p.spec + ((size_t)l * p.M + t.m) * JP + (size_t)pb * p.cp + c;
-      if (p.acc_in) v += *dst;   // partial sums of the earlier latitude chunks (unrounded fp32)
+      float2* dst = reinterpret_cast<float2*>(p.spec + ((size_t)l * p.M + t.m) * JP + (size_t)pb * p.cp + c);
+      float2 o = make_float2(v[0], v[1]);
+      if (p.acc_in) { const float2 d = *dst; o.x += d.x; o.y += d.y; }   // partial sums of the earlier latitude chunks (unrounded fp32)
       // strict fp32 (split) and the partial sums of a chunked analysis stay as accumulated; otherwise the consumers are TF32 MMAs: round
       // to nearest here
-      *dst = p.round_out ? tf32_rn(v) : v;
+      if (p.round_out) { o.x = tf32_rn(o.x); o.y = tf32_rn(o.y); }
+      *dst = o;
     });
   }
 };
@@ -235,6 +384,7 @@ struct SynTraits {
     int kc0, kc1;           // latitude range [kc0, kc1) of this launch (kc0 a multiple of 128): the tiles cover these rows only
     int tiled, M2, KT, B;   // tiled output for the tensor-core DFT (dft.cu): Z[r][k / 8][p][m / 8][m % 8][k % 8], orders padded to 8 * M2
   };
+  static constexpr int kPlanes = 1;
   struct Tile { int m, k0, n0, lbeg; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.m = bz;
@@ -257,30 +407,44 @@ struct SynTraits {
       for (int b = 0; b < p.nblk; ++b) tma_load_3d(st + p.lo_off + 16384 + b * 4096, &p.tmB_lo, bar, t.n0 + 32 * b, t.m, l);
     }
   }
-  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, Acc& acc) {
-    const int nb = p.N / 8;
-    gemm_real<true, true>(st, st + 16384, row0, nb, acc);
-    if (p.split) {
-      gemm_real<true, true>(st, st + p.lo_off + 16384, row0, nb, acc);   // hi . lo
-      gemm_real<true, true>(st + p.lo_off, st + 16384, row0, nb, acc);   // lo . hi
-    }
+  template <int NB, bool SPLIT>
+  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, float (&acc)[NB][4]) {
+    gemm_real<Lay::MM, NB, SPLIT>(st, st + 16384, p.lo_off, row0, acc);
   }
   // column jp = pb * cp + c of the tile -> row (pb, c) of this order's slab of Z; orders without a contributing degree hold zero accumulators
-  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const Acc& acc) {
+  // In the MM layout a lane holds the latitude pair k, k + 1 (k even) of columns 32 J + 8 q + 4 e .. + 3: one 8-byte store per column in
+  // both layouts of Z (k is the contiguous index of the standard layout and k % 8 that of the tiled one).  The column is decoded once per run.
+  template <int NB>
+  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const float (&acc)[NB][4]) {
     const int JP = p.PB * p.cp;
-    for_each_acc(acc, row0, p.N / 8, [&](int r, int n, float v) {
-      const int k = t.k0 + r, jp = t.n0 + n;
-      if (k >= p.kc1 || jp >= JP) return;
-      const int pb = jp / p.cp, c = jp - pb * p.cp;
-      if (c >= p.C) return;
-      if (!p.tiled) {
-        p.Z[(size_t)t.m * p.PB * p.C * p.kp + (size_t)(pb * p.C + c) * p.kp + k] = v;
-      } else {   // pb = plane * B + b, image r = b * C + c:  Z[r][kt][plane][m2][c8][k8]
-        const int pl = pb / p.B, b = pb - pl * p.B;
-        const int o = (((b * p.C + c) * p.KT) * 2 + pl) * p.M2 * 64;
-        p.Z[(size_t)(k >> 3) * 2 * p.M2 * 64 + (t.m >> 3) * 64 + (t.m & 7) * 8 + (k & 7) + o] = v;
+    const int k = t.k0 + frag_row<Lay::MM>(row0, 0);
+    if (k >= p.kc1) return;
+    const bool pair = k + 1 < p.kc1;
+    const int q = threadIdx.x & 3;
+#pragma unroll
+    for (int J = 0; J < NB / 4; ++J)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int jp0 = t.n0 + 32 * J + 8 * q + 4 * e;
+        int pb = jp0 / p.cp, c = jp0 - pb * p.cp;
+#pragma unroll
+        for (int i = 0; i < 4; ++i, ++c) {
+          if (c == p.cp) { c = 0; ++pb; }
+          if (jp0 + i >= JP) break;
+          if (c >= p.C) continue;
+          const float v0 = acc[4 * J + i][e], v1 = acc[4 * J + i][2 + e];
+          float* dst;
+          if (!p.tiled) {
+            dst = p.Z + (size_t)t.m * p.PB * p.C * p.kp + (size_t)(pb * p.C + c) * p.kp + k;
+          } else {   // pb = plane * B + b, image r = b * C + c:  Z[r][kt][plane][m2][c8][k8]
+            const int pl = pb / p.B, b = pb - pl * p.B;
+            const int o = (((b * p.C + c) * p.KT) * 2 + pl) * p.M2 * 64;
+            dst = p.Z + (size_t)(k >> 3) * 2 * p.M2 * 64 + (t.m >> 3) * 64 + (t.m & 7) * 8 + (k & 7) + o;
+          }
+          if (pair) *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+          else *dst = v0;
+        }
       }
-    });
   }
 };
 
@@ -303,8 +467,15 @@ struct MixParams : EngineParams {
   uint32_t offA_i, offB_r, offB_i;  // stage offsets of the imaginary A tile and the two B tiles (A_r at 0)
 };
 
+template <int V>
+__device__ __forceinline__ void st_vec(float* dst, const float (&v)[V]) {   // dst 4 V-byte aligned
+  if constexpr (V == 4) *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+  else *reinterpret_cast<float2*>(dst) = make_float2(v[0], v[1]);
+}
+
 struct MixFwdTraits {
   using Params = MixParams;
+  static constexpr int kPlanes = 2;
   struct Tile { int l, m0, g, o0, lg; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.l = bz;
@@ -326,33 +497,52 @@ struct MixFwdTraits {
     }
   }
   // yr = xr wr - xi wi,  yi = xr wi + xi wr
-  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, Acc& acc) {
-    gemm_cplx<false, true, -1, 1, 1>(st, st + p.offA_i, st + p.offB_r, st + p.offB_i, row0, p.N / 8, acc);
+  template <int NB, bool>
+  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, float (&acc)[2 * NB][4]) {
+    gemm_cplx<Lay::KM, NB, -1, 1, 1>(st, st + p.offA_i, st + p.offB_r, st + p.offB_i, row0, acc);
   }
-  // rows (mi, b) -> spec rows; columns -> output channels of group g; handles cbias and the zero channel padding
-  __device__ __forceinline__ static void store_rows(const Params& p, int l, int m0, int g, int o0, int NOg, int cp_out, int row0, const Acc& acc,
-                                                    bool with_bias) {
+  // rows (mi, b) -> spec rows; columns -> output channels of group g; handles cbias and the zero channel padding.  A run of 2 or 4 columns
+  // never straddles `limit` (cp_out, and NOg when G > 1, are multiples of 4; o0 of 16 or 32), so it is stored as one vector.
+  template <Lay L, int NB>
+  __device__ __forceinline__ static void store_rows(const Params& p, int l, int m0, int g, int o0, int NOg, int cp_out, int row0,
+                                                    const float (&acc)[2 * NB][4], bool with_bias) {
     const int pad = cp_out - NOg * p.G;
     const int limit = NOg + ((g == p.G - 1) ? pad : 0);  // columns of this group incl. trailing zero padding
     const int mend = mend_d(l, p.M, p.dense);
-    for_each_cacc(acc, row0, p.N / 8, [&](int r, int n, float a, float c) {
-      const int m = m0 + r / p.B, b = r % p.B, o = o0 + n;
-      if (r >= p.Mt * p.B || m >= mend || o >= limit) return;
-      if (o >= NOg) { a = 0.f; c = 0.f; }
-      else if (with_bias) { const float2 cb = p.cbias[g * NOg + o]; a += cb.x; c += cb.y; }
-      float* yr = p.out + ((size_t)l * p.M + m) * 2 * p.B * cp_out + (size_t)b * cp_out + g * NOg + o;
-      yr[0] = tf32_rn(a);
-      yr[(size_t)p.B * cp_out] = tf32_rn(c);
+    float* yrow[2];
+    bool ok[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = frag_row<L>(row0, h), mi = r / p.B, b = r - mi * p.B, m = m0 + mi;
+      ok[h] = r < p.Mt * p.B && m < mend;
+      yrow[h] = p.out + ((size_t)l * p.M + m) * 2 * p.B * cp_out + (size_t)b * cp_out + g * NOg;
+    }
+    for_each_run<L, NB>(acc, [&](int h, int n, const auto& re, const auto& im) {
+      constexpr int V = sizeof(re) / sizeof(float);
+      const int o = o0 + n;
+      if (!ok[h] || o >= limit) return;
+      float a[V], c[V];
+#pragma unroll
+      for (int v = 0; v < V; ++v) {
+        a[v] = re[v]; c[v] = im[v];
+        if (o + v >= NOg) { a[v] = 0.f; c[v] = 0.f; }
+        else if (with_bias) { const float2 cb = p.cbias[g * NOg + o + v]; a[v] += cb.x; c[v] += cb.y; }
+        a[v] = tf32_rn(a[v]); c[v] = tf32_rn(c[v]);
+      }
+      st_vec<V>(yrow[h] + o, a);
+      st_vec<V>(yrow[h] + o + (size_t)p.B * cp_out, c);
     });
   }
-  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const Acc& acc) {
-    store_rows(p, t.l, t.m0, t.g, t.o0, p.Cog, p.cpo, row0, acc, p.cbias != nullptr);
+  template <int NB>
+  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const float (&acc)[2 * NB][4]) {
+    store_rows<Lay::KM, NB>(p, t.l, t.m0, t.g, t.o0, p.Cog, p.cpo, row0, acc, p.cbias != nullptr);
   }
 };
 
 struct MixDgradTraits {
   using Params = MixParams;   // tmX = gy (channels = Cout), out = gx; N tiles over i
   using Tile = MixFwdTraits::Tile;  // o0 is the first input channel i0 of the tile
+  static constexpr int kPlanes = 2;
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) { return MixFwdTraits::make_tile(p, t, bx, by, bz); }
   __device__ static void prefetch(const Params& p) { prefetch_tmap(&p.tmX); prefetch_tmap(&p.tmW); }
   __device__ static int num_kblocks(const Params& p, const Tile&) { return (p.Cog + 31) / 32; }
@@ -364,16 +554,19 @@ struct MixDgradTraits {
     tma_load_4d(st + p.offB_i, &p.tmW, bar, kb * 32, 1, t.o0, t.lg);
   }
   // gxr = gr wr + gi wi,  gxi = gi wr - gr wi
-  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, Acc& acc) {
-    gemm_cplx<false, false, 1, -1, 1>(st, st + p.offA_i, st + p.offB_r, st + p.offB_i, row0, p.N / 8, acc);
+  template <int NB, bool>
+  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, float (&acc)[2 * NB][4]) {
+    gemm_cplx<Lay::KK, NB, 1, -1, 1>(st, st + p.offA_i, st + p.offB_r, st + p.offB_i, row0, acc);
   }
-  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const Acc& acc) {
-    MixFwdTraits::store_rows(p, t.l, t.m0, t.g, t.o0, p.Cig, p.cpi, row0, acc, false);
+  template <int NB>
+  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const float (&acc)[2 * NB][4]) {
+    MixFwdTraits::store_rows<Lay::KK, NB>(p, t.l, t.m0, t.g, t.o0, p.Cig, p.cpi, row0, acc, false);
   }
 };
 
 struct MixWgradTraits {
   using Params = MixParams;   // tmX = x (A, rows i), tmX2 = gy (B, cols o); K = spectral rows (m, b)
+  static constexpr int kPlanes = 2;
   struct Tile { int lz, i0, g, o0; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.lz = bz;
@@ -409,17 +602,23 @@ struct MixWgradTraits {
     }
   }
   // gwr = xr gr + xi gi,  gwi = xr gi - xi gr
-  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, Acc& acc) {
-    gemm_cplx<true, true, 1, 1, -1>(st, st + p.offA_i, st + p.offB_r, st + p.offB_i, row0, p.N / 8, acc);
+  template <int NB, bool>
+  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, float (&acc)[2 * NB][4]) {
+    gemm_cplx<Lay::MM, NB, 1, 1, -1>(st, st + p.offA_i, st + p.offB_r, st + p.offB_i, row0, acc);
   }
-  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const Acc& acc) {
+  // runs of 4 output channels (cop and o0 are multiples of 4): one float4 per run and plane
+  template <int NB>
+  __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const float (&acc)[2 * NB][4]) {
     float* const out = p.out + (size_t)(p.shared_w ? 0 : t.lz) * p.wl_stride + (size_t)t.g * p.Cig * 2 * p.cop;
-    for_each_cacc(acc, row0, p.N / 8, [&](int r, int n, float a, float c) {
-      const int i = t.i0 + r, o = t.o0 + n;
+    for_each_run<Lay::MM, NB>(acc, [&](int h, int n, const float (&re)[4], const float (&im)[4]) {
+      const int i = t.i0 + frag_row<Lay::MM>(row0, h), o = t.o0 + n;
       if (i >= p.Cig || o >= p.cop) return;
       float* row = out + (size_t)i * 2 * p.cop;
-      row[o] = (o < p.Cog) ? a : 0.f;
-      row[p.cop + o] = (o < p.Cog) ? c : 0.f;
+      float a[4], c[4];
+#pragma unroll
+      for (int v = 0; v < 4; ++v) { a[v] = (o + v < p.Cog) ? re[v] : 0.f; c[v] = (o + v < p.Cog) ? im[v] : 0.f; }
+      st_vec<4>(row + o, a);
+      st_vec<4>(row + p.cop + o, c);
     });
   }
 };
@@ -504,23 +703,47 @@ static int sm_count() {   // of the current device (the launch device: _lib.call
   return n;
 }
 
-template <class T>
+template <class T, int NB, bool SPLIT>
+struct KernelTag {};   // one shared-memory grant per instantiation
+template <class T, int NB, bool SPLIT>
 static int launch(typename T::Params& p, dim3 grid, cudaStream_t st) {
   p.gx = (int)grid.x; p.gy = (int)grid.y; p.gz = (int)grid.z;
   const long long ntiles = (long long)grid.x * grid.y * grid.z;
   if (ntiles <= 0) return 0;
   const size_t smem = smem_bytes(p);
   if (smem > 232448) { set_error("umma: %zu bytes of shared memory needed", smem); return B200SHT_ERR_UNSUPPORTED; }
-  B200_CHECK_CUDA((ensure_dynamic_smem<T>(umma_kernel<T>, smem)));
+  B200_CHECK_CUDA((ensure_dynamic_smem<KernelTag<T, NB, SPLIT>>(umma_kernel<T, NB, SPLIT>, smem)));
   // static round-robin over tiles: an odd CTA count not divisible by 3 keeps tile-grid periods (2 l- or m-tiles, 3 or 6 n/k-tiles)
   // from locking heavy tiles onto the same CTAs
   const int sms = usable_sms(sm_count());
   int ctas = (int)(ntiles < sms ? ntiles : sms);
   while (ctas > 1 && (ctas % 2 == 0 || ctas % 3 == 0)) --ctas;
-  B200_CHECK_CUDA(launch_pdl(umma_kernel<T>, dim3(ctas), dim3(kUmmaThreads), smem, st, p));
+  B200_CHECK_CUDA(launch_pdl(umma_kernel<T, NB, SPLIT>, dim3(ctas), dim3(kUmmaThreads), smem, st, p));
   B200_CHECK_LAUNCH();
   return 0;
 }
+
+// The tile widths (8-column fragments per warp) an engine is built for.  The host pads a tile's columns up to the next built width; the
+// set is small because every width is a separate kernel (code size, build time).  Legendre: 20 fragments are the 152 + 8 columns of
+// C = 73, B = 1, and 32 the 256 of C = 384; mix (complex, 2 NB accumulator fragments): up to 128 columns.
+template <int... W>
+struct Widths {
+  static int pick(int nb) {
+    for (int w : {W...})
+      if (nb <= w) return w;
+    return -1;
+  }
+  template <class T, bool SPLIT>
+  static int launch_nb(typename T::Params& p, int nb, dim3 grid, cudaStream_t st) {
+    int rc = B200SHT_ERR_UNSUPPORTED;
+    const bool found = ((nb == W ? (rc = launch<T, W, SPLIT>(p, grid, st), true) : false) || ...);
+    if (!found) set_error("umma: no engine built for %d fragments per warp", nb);
+    return rc;
+  }
+};
+using LegendreWidths = Widths<4, 8, 12, 16, 20, 24, 32>;
+using SplitWidths = Widths<8, 16>;   // 3 x TF32 (precision fp32x3): residual fragments too, so tiles of at most 128 columns
+using MixWidths = Widths<4, 8, 12>;  // complex: 2 x 96 accumulator columns
 
 // ---------------------------------------------------------------------------------------------- Legendre
 // k_begin / k_end: latitude range [k_begin, k_end) to reduce over (k_begin a multiple of 32; k_end < 0: all rows); accumulate: add to the spec
@@ -537,10 +760,13 @@ int legendre_analysis_umma(const Plan* pl, const float* X, float* spec, int B, i
   p.round_out = (last && X_lo == nullptr) ? 1 : 0;
   const int cp = round_up(C, 4), PB = 2 * B;
   p.spec = spec; p.L = pl->lmax; p.M = pl->mmax; p.nlat = pl->nlat; p.C = C; p.cp = cp; p.PB = PB; p.m0 = pl->m0;
-  if (cp <= 128) { p.Cc = cp; p.n_ct = 1; p.PBc = 256 / cp < PB ? 256 / cp : PB; }
-  else { p.n_ct = ceil_div(cp, 128); p.Cc = round_up(ceil_div(cp, p.n_ct), 4); p.PBc = (2 * p.Cc <= 256 && PB >= 2) ? 2 : 1; }
+  const int maxc = X_lo ? 128 : 256;   // columns per tile (SplitWidths / LegendreWidths)
+  if (cp <= 128) { p.Cc = cp; p.n_ct = 1; p.PBc = maxc / cp < PB ? maxc / cp : PB; }
+  else { p.n_ct = ceil_div(cp, 128); p.Cc = round_up(ceil_div(cp, p.n_ct), 4); p.PBc = (2 * p.Cc <= maxc && PB >= 2) ? 2 : 1; }
   const int rows = p.Cc * p.PBc;
-  p.N = round_up(rows, 16);
+  const int nb = (X_lo ? SplitWidths::pick(ceil_div(rows, 8)) : LegendreWidths::pick(ceil_div(rows, 8)));
+  B200_REQUIRE(nb > 0, "legendre_analysis: %d columns per tile", rows);
+  p.N = 8 * nb;
   {
     long long d[3] = {pl->nlat, pl->lmax, pl->mmax}, s[3] = {1, pl->kp, (long long)pl->lmax * pl->kp};
     int bx[3] = {32, 128, 1};
@@ -569,7 +795,7 @@ int legendre_analysis_umma(const Plan* pl, const float* X, float* spec, int B, i
   pick_stages(&p, (16384 + bbytes) * (p.split ? 2 : 1), ceil_div(pl->nlat, 32));
   p.tx_bytes = (16384 + (uint32_t)rows * 128) * (p.split ? 2 : 1);
   dim3 grid(ceil_div(pl->lmax, 128), p.n_ct * ceil_div(PB, p.PBc), pl->mmax);
-  return launch<AnaTraits>(p, grid, st);
+  return p.split ? SplitWidths::launch_nb<AnaTraits, true>(p, nb, grid, st) : LegendreWidths::launch_nb<AnaTraits, false>(p, nb, grid, st);
 }
 
 // k_begin / k_end: latitude range [k_begin, k_end) to produce (k_begin a multiple of 128; k_end < 0: up to kp)
@@ -584,8 +810,10 @@ int legendre_synthesis_umma(const Plan* pl, const float* spec, float* Z, int B, 
   p.Z = Z; p.L = pl->lmax; p.M = pl->mmax; p.nlat = pl->nlat; p.kp = pl->kp; p.C = C; p.cp = cp; p.PB = PB; p.m0 = pl->m0;
   p.tiled = tiled; p.M2 = (pl->mmax + 7) / 8; p.KT = pl->kp / 8; p.B = B;
   B200_REQUIRE(!tiled || (long long)B * C * p.KT * 2 * p.M2 * 64 < (1ll << 31), "legendre_synthesis: tiled latspec of %d images exceeds 2^31 floats", B * C);
-  p.nblk = ceil_div(JP, 32) < 8 ? ceil_div(JP, 32) : 8;
-  p.N = 32 * p.nblk;
+  const int maxblk = spec_lo ? 4 : 8;   // column blocks of 32 per tile (SplitWidths / LegendreWidths)
+  const int nb = (spec_lo ? SplitWidths::pick : LegendreWidths::pick)(4 * (ceil_div(JP, 32) < maxblk ? ceil_div(JP, 32) : maxblk));
+  p.nblk = nb / 4;   // column blocks of 32 loaded per stage; those past JP are zero-filled by TMA and not stored
+  p.N = 8 * nb;
   {
     long long d[3] = {pl->nlat, pl->lmax, pl->mmax}, s[3] = {1, pl->kp, (long long)pl->lmax * pl->kp};
     int bx[3] = {32, 32, 1};
@@ -613,7 +841,7 @@ int legendre_synthesis_umma(const Plan* pl, const float* spec, float* Z, int B, 
   pick_stages(&p, (16384 + 4096 * p.nblk) * (p.split ? 2 : 1), ceil_div(pl->lmax, 32));
   p.tx_bytes = (16384 + 4096 * p.nblk) * (p.split ? 2 : 1);
   dim3 grid(ceil_div(k_end - k_begin, 128), ceil_div(JP, p.N), tiled ? 8 * p.M2 : pl->mmax);
-  return launch<SynTraits>(p, grid, st);
+  return p.split ? SplitWidths::launch_nb<SynTraits, true>(p, nb, grid, st) : LegendreWidths::launch_nb<SynTraits, false>(p, nb, grid, st);
 }
 
 // --------------------------------------------------------------------------------------------------- mix
@@ -643,11 +871,12 @@ static int fill_mix(const Plan* pl, int op, int B, int G, int Ci, int Co, MixPar
   return 0;
 }
 
-// Column tiling of a mix GEMM: equal tiles of at most 128 columns (no half-empty last tile: at C = 384 a 256 + 128 split wasted a quarter
-// of the MMAs), so that the complex accumulator of a tile, 2 N columns, fits the kMaxCols registers of the consumer warps.
+// Column tiling of a mix GEMM: equal tiles of at most 96 columns (no half-empty last tile: at C = 384 a 256 + 128 split wasted a quarter
+// of the MMAs), so that the complex accumulator of a tile, 2 N columns, and the fragments of a stage fit the registers of the consumer
+// warps without spilling (MixWidths).
 static void split_cols(int cols, int gran, int* N, int* n_nt) {
-  if (cols <= 128) { *n_nt = 1; *N = round_up(cols, gran); return; }
-  *n_nt = ceil_div(cols, 128);
+  if (cols <= 96) { *n_nt = 1; *N = round_up(cols, gran); return; }
+  *n_nt = ceil_div(cols, 96);
   *N = round_up(ceil_div(cols, *n_nt), 32);   // the epilogues drain 32 columns at a time: a tile must not end inside a chunk
 }
 
@@ -666,7 +895,7 @@ int mix_forward_umma(const Plan* pl, int op, const float* x, const void* w, cons
   pick_stages(&p, 32768 + 8192 * p.nblk, ceil_div(p.Cig, 32));
   p.tx_bytes = 2u * (uint32_t)(p.Mt * B) * 128 + 8192u * p.nblk;
   dim3 grid(ceil_div(p.M, p.Mt), p.n_nt * G, p.L);
-  return launch<MixFwdTraits>(p, grid, st);
+  return MixWidths::launch_nb<MixFwdTraits, false>(p, p.N / 8, grid, st);
 }
 
 int mix_backward_umma(const Plan* pl, int op, const float* x, const void* w, const float* gy, float* gx, void* gw, void* gcbias, int B, int G,
@@ -679,6 +908,7 @@ int mix_dgrad_umma(const Plan* pl, int op, const void* w, const float* gy, float
   p.out = gx;
   const int cols = p.Cig + ((p.cpi - Ci) > 0 ? (p.cpi - Ci) : 0);
   split_cols(cols, 16, &p.N, &p.n_nt);
+  p.N = 8 * MixWidths::pick(p.N / 8);   // one column tile when the width is padded (n_nt > 1 tiles are multiples of 32)
   const uint32_t bb = (uint32_t)round_up(p.N * 128, 1024);
   p.offA_i = 16384; p.offB_r = 32768; p.offB_i = 32768 + bb;
   rc = spec_tmap(&p.tmX, gy, p.L, p.M, B, Co, p.cpo, 32, B, p.Mt);
@@ -687,7 +917,7 @@ int mix_dgrad_umma(const Plan* pl, int op, const void* w, const float* gy, float
   pick_stages(&p, 32768 + 2 * bb, ceil_div(p.Cog, 32));
   p.tx_bytes = 2u * (uint32_t)(p.Mt * B) * 128 + 2u * (uint32_t)p.N * 128;
   dim3 grid(ceil_div(p.M, p.Mt), p.n_nt * G, p.L);
-  return launch<MixDgradTraits>(p, grid, st);
+  return MixWidths::launch_nb<MixDgradTraits, false>(p, p.N / 8, grid, st);
 }
 
 int mix_wgrad_umma(const Plan* pl, int op, const float* x, const float* gy, float* gw, int B, int G, int Ci, int Co, cudaStream_t st) {
@@ -704,7 +934,7 @@ int mix_wgrad_umma(const Plan* pl, int op, const float* x, const float* gy, floa
   pick_stages(&p, 32768 + 8192 * p.nblk, 8);
   p.tx_bytes = 32768u + 8192u * p.nblk;
   dim3 grid(ceil_div(p.Cig, 128), p.n_nt * G, p.shared_w ? 1 : p.L);
-  return launch<MixWgradTraits>(p, grid, st);
+  return MixWidths::launch_nb<MixWgradTraits, false>(p, p.N / 8, grid, st);
 }
 
 int mix_cbias_grad(const float* gy, void* gcb, int L, int M, int B, int Co, int dense, cudaStream_t st);  // mix.cu

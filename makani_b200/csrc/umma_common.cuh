@@ -101,13 +101,17 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) { asm volat
 // 1024-byte aligned).  Two layouts, both 32 floats wide:
 //   K-major:  row r (an M or N index) holds 32 consecutive K values
 //   MN-major: blocks of [32 K-rows][32 consecutive M / N values], 4096 bytes apart
-// Hopper's wgmma reads TF32 operands from shared memory only K-major; the m16n8k8 fragments below are loaded element by element, so
-// both layouts feed the same instruction.
+// Hopper's wgmma reads TF32 operands from shared memory only K-major; the m16n8k8 fragments below (used by dft.cu) are loaded element by
+// element, so both layouts feed the same instruction.  The GEMM engine of umma.cu loads permuted fragments with 8- and 16-byte loads instead.
+__device__ __forceinline__ uint32_t swz128(uint32_t off) { return off ^ ((off >> 3) & 0x70u); }
 template <bool MN>
 __device__ __forceinline__ uint32_t ld_op(const uint8_t* tile, int r, int k) {
   const uint32_t off = MN ? (uint32_t)((r >> 5) * 4096 + k * 128 + (r & 31) * 4) : (uint32_t)(r * 128 + k * 4);
-  return *reinterpret_cast<const uint32_t*>(tile + (off ^ ((off >> 3) & 0x70u)));
+  return *reinterpret_cast<const uint32_t*>(tile + swz128(off));
 }
+// 8 / 16 bytes at the unswizzled byte offset `off` of a swizzled tile (off a multiple of 8 / 16: the swizzle moves whole 16-byte chunks)
+__device__ __forceinline__ uint2 lds64(const uint8_t* tile, uint32_t off) { return *reinterpret_cast<const uint2*>(tile + swz128(off)); }
+__device__ __forceinline__ uint4 lds128(const uint8_t* tile, uint32_t off) { return *reinterpret_cast<const uint4*>(tile + swz128(off)); }
 // A fragment of mma.m16n8k8 (rows r0 + g, r0 + g + 8; K columns k0 + q, k0 + q + 4; g = lane / 4, q = lane % 4)
 template <bool MN>
 __device__ __forceinline__ void frag_a(const uint8_t* tile, int r0, int k0, uint32_t (&a)[4]) {
