@@ -14,6 +14,9 @@
  *   b200sht_mix_forward/backward <- makani/models/common/contractions.py:19-54 (_contract_* einsums) and :62-151
  *   b200sht_spectral_conv_forward<- SpectralConv.forward       (spectral_convolution.py:213-264), one call
  *   b200sht_complex_relu_*       <- makani/models/common/activations.py:88-127 (ComplexReLU)
+ *   b200sht_vsht_forward         <- torch_harmonics.RealVectorSHT.forward         (makani/utils/losses/base_loss.py:427-469 VortDivBaseLoss)
+ *   b200sht_vsht_inverse         <- torch_harmonics.InverseRealVectorSHT.forward  (base_loss.py:427-469 and :518-565 GradientBaseLoss)
+ *   b200sht_vsht_*_adjoint       <- autograd backward of the two vector transforms
  *
  * Conventions
  *   - every function returns 0 on success, a negative b200sht_status otherwise; b200sht_last_error() gives text.
@@ -83,21 +86,30 @@ int b200sht_version(void);
  * and stored as fp32 [mmax][lmax][kp]. */
 int b200sht_plan_create(b200sht_plan** plan, int nlat, int nlon, int lmax, int mmax,
                         const double* cost, const double* quad_w, int csphase, void* stream);
-/* Extended creation for the h x w model-parallel (distributed) SHT:
+/* Extended creation for the h x w model-parallel (distributed) SHT and for the vector SHT:
  *   m_offset : the plan's orders are m_offset .. m_offset + mmax - 1 (this rank's shard of the orders)
- *   flags & 1: FFT-only plan (no Legendre table): nlat is this rank's latitude count, quad_w its slice of the weights */
+ *   flags & B200SHT_PLAN_FFT_ONLY: no Legendre table: nlat is this rank's latitude count, quad_w its slice of the weights
+ *   flags & B200SHT_PLAN_VECTOR:   vector-SHT plan (m_offset 0).  Instead of P it holds, built on the device in fp64 and stored as fp32
+ *                                  [mmax][lmax][kp] each (exact zeros for l < m, zero at l = 0):
+ *                                    D[m][l][k] = dP_l^m(cos theta)/dtheta at theta_k,   Q[m][l][k] = m P_l^m(cos theta_k) / sin(theta_k)
+ *                                  (P the orthonormal table of the scalar plan, Condon-Shortley phase when csphase).  Only the vector entry
+ *                                  points (b200sht_vector_*, b200sht_vsht_*) and the longitude stages accept it. */
+#define B200SHT_PLAN_FFT_ONLY 1
+#define B200SHT_PLAN_VECTOR 2
 int b200sht_plan_create_ex(b200sht_plan** plan, int nlat, int nlon, int lmax, int mmax, int m_offset, int flags,
                            const double* cost, const double* quad_w, int csphase, void* stream);
 int b200sht_plan_destroy(b200sht_plan* plan);
-/* what: 0 nlat, 1 nlon, 2 lmax, 3 mmax, 4 kp, 5 table bytes, 6 tensor-core path available (0/1; sm_90 devices), 7 m_offset,
- *       8 tensor-core longitude DFT available for this grid (0/1) */
+/* what: 0 nlat, 1 nlon, 2 lmax, 3 mmax, 4 kp, 5 table bytes (both tables of a vector plan), 6 tensor-core path available (0/1; sm_90
+ *       devices), 7 m_offset, 8 tensor-core longitude DFT available for this grid (0/1), 9 vector plan (0/1) */
 int64_t b200sht_plan_query(const b200sht_plan* plan, int what);
 /* device pointer to the fp32 table [mmax][lmax][kp] (for tests) */
 const float* b200sht_plan_table(const b200sht_plan* plan);
-/* copy the table into caller-owned device memory (mmax*lmax*kp floats) */
+/* copy the table into caller-owned device memory (mmax*lmax*kp floats; a vector plan: D then Q, 2*mmax*lmax*kp floats).
+ * b200sht_plan_table of a vector plan points at its internal layout [mmax][2][lmax][kp] (D rows, then Q rows, of each order). */
 int b200sht_plan_copy_table(const b200sht_plan* plan, float* dst, void* stream);
 
 /* ------------------------------------------------------------------------------ packed-format sizes */
+/* (for the buffers of C vector fields on a vector plan pass 2C: see the vector SHT section) */
 int64_t b200sht_latspec_elems(const b200sht_plan* plan, int B, int C); /* floats in a latspec buffer */
 int64_t b200sht_spec_elems(const b200sht_plan* plan, int B, int C);    /* floats in a spec buffer    */
 int64_t b200sht_spec_elems_lm(int L, int M, int B, int C);
@@ -157,6 +169,39 @@ int b200sht_sht_forward_adjoint(const b200sht_plan* plan, const void* gcoeffs, v
 /* gradient of sht_inverse w.r.t. coeffs given dL/dy */
 int b200sht_sht_inverse_adjoint(const b200sht_plan* plan, const void* gy, int dtype, int B, int C, void* gcoeffs,
                                 void* workspace, int precision, void* stream);
+
+/* ------------------------------------------------------------------------------------- vector SHT */
+/* torch_harmonics.RealVectorSHT / InverseRealVectorSHT (norm "ortho") on a vector plan.  A field of C vector channels is
+ * x [B][C][2][nlat][nlon] (component 0 = colatitude theta, 1 = longitude phi; rows north to south); its coefficients are
+ * complex64 [B][C][2][lmax][mmax] (0 = spheroidal S, 1 = toroidal T; exact zeros for l < m).  With X = 2 pi rfft(x, norm="forward")[:mmax]
+ * and the quadrature weights w_k:
+ *   S_lm = sum_k w_k (D X_theta - i Q X_phi) / (l (l+1)),   T_lm = sum_k w_k (-i Q X_theta - D X_phi) / (l (l+1)),   S_0m = T_0m = 0
+ *   U_theta = irfft(sum_l D S + i Q T),   U_phi = irfft(sum_l i Q S - D T)   (n = nlon, norm "forward"; Im of m = 0 / Nyquist ignored)
+ * so that ivsht([f_lm, 0]) = (df/dtheta, df/dphi / sin theta) and ivsht([0, g_lm]) = -r x grad g.
+ * Stage formats: the 2C component rows (b, c, component) are read and written in place as the rows of a scalar latspec of 2C channels, and
+ * the Legendre stages produce a STACKED spec [2][lmax][mmax][2][B][cp] (cp = 2C rounded up to 4, column 2c + component): the D
+ * contractions, then the Q contractions (b200sht_spec_elems(plan, B, 2C) floats).  The +-i rotations and 1/(l(l+1)) happen in the
+ * spec <-> coefficient converters.  Precision FP32 or TF32 (3 x TF32 is refused with B200SHT_ERR_UNSUPPORTED). */
+int b200sht_vector_legendre_analysis(const b200sht_plan* plan, const float* latspec, float* spec, int B, int C, int precision, void* stream);
+int b200sht_vector_legendre_synthesis(const b200sht_plan* plan, const float* spec, float* latspec, int B, int C, int precision, void* stream);
+/* TF32 into the tiled latspec layout of the tensor-core DFT (see b200sht_legendre_synthesis_tiled); needs b200sht_plan_query(plan, 8) == 1 */
+int b200sht_vector_legendre_synthesis_tiled(const b200sht_plan* plan, const float* spec, float* latspec, int B, int C, void* stream);
+/* stacked spec <-> coefficients [B][C][2][lmax][mmax].  unpack: S = f (D x_theta - i Q x_phi), T = f (-i Q x_theta - D x_phi);
+ * pack: D_theta = f S, D_phi = -f T, Q_theta = i f T, Q_phi = i f S; f = 1 / (l (l+1)) (0 at l = 0) when scaled, else 1.
+ * pack(scaled) is the adjoint of unpack(scaled).  pack writes every entry of the stacked spec. */
+int b200sht_vector_spec_unpack(const b200sht_plan* plan, const float* spec, void* coeffs, int B, int C, int scaled, void* stream);
+int b200sht_vector_spec_pack(const b200sht_plan* plan, const void* coeffs, float* spec, int B, int C, int scaled, void* stream);
+/* One-call boundary, as b200sht_sht_* (workspace of b200sht_vsht_workspace_bytes; -1 for a scalar plan):
+ *   forward          x [B][C][2][nlat][nlon] (dtype) -> coeffs                        <- RealVectorSHT.forward
+ *   inverse          coeffs -> y [B][C][2][nlat][nlon] (dtype)                        <- InverseRealVectorSHT.forward
+ *   forward_adjoint  dL/dcoeffs -> dL/dx     inverse_adjoint  dL/dy -> dL/dcoeffs      <- their autograd backward (PyTorch complex-gradient convention) */
+int64_t b200sht_vsht_workspace_bytes(const b200sht_plan* plan, int B, int C);
+int b200sht_vsht_forward(const b200sht_plan* plan, const void* x, int dtype, int B, int C, void* coeffs, void* workspace, int precision, void* stream);
+int b200sht_vsht_inverse(const b200sht_plan* plan, const void* coeffs, void* y, int dtype, int B, int C, void* workspace, int precision, void* stream);
+int b200sht_vsht_forward_adjoint(const b200sht_plan* plan, const void* gcoeffs, void* gx, int dtype, int B, int C, void* workspace, int precision,
+                                 void* stream);
+int b200sht_vsht_inverse_adjoint(const b200sht_plan* plan, const void* gy, int dtype, int B, int C, void* gcoeffs, void* workspace, int precision,
+                                 void* stream);
 
 /* -------------------------------------------------------------------------------------- channel mix */
 /* weight re-layout: native torch parameter (complex64, shapes per b200sht_mix_op) -> packed
@@ -271,6 +316,8 @@ int b200sht_debug_set_lat_chunks_syn(int n);
 int b200sht_debug_fft_plan(int N, int* radices, int max_radices);
 /* table [mmax][lmax][nlat] (fp32) from cos(colatitude) cost[nlat] */
 int b200sht_debug_table_host(int nlat, int lmax, int mmax, const double* cost, int csphase, float* table);
+/* the vector plan's tables D and Q, each [mmax][lmax][nlat] (fp32), from cost[nlat] */
+int b200sht_debug_vector_table_host(int nlat, int lmax, int mmax, const double* cost, int csphase, float* D, float* Q);
 
 #ifdef __cplusplus
 }

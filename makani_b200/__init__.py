@@ -2,6 +2,7 @@
 
 Public surface (mirrors the reference, see INTEGRATION.md):
     RealSHT, InverseRealSHT                    <- torch_harmonics.{RealSHT, InverseRealSHT}
+    RealVectorSHT, InverseRealVectorSHT        <- torch_harmonics.{RealVectorSHT, InverseRealVectorSHT} (makani's vort/div and gradient losses)
     SpectralConv, SpectralAttention, ComplexReLU <- makani.models.common.*
     quadrature                                 <- torch_harmonics.quadrature
     distributed                                <- torch_harmonics.distributed (h x w spatial model parallelism)
@@ -13,6 +14,7 @@ Public surface (mirrors the reference, see INTEGRATION.md):
 from ._lib import B200ShtError, load as load_library  # noqa: F401
 from . import quadrature  # noqa: F401
 from .sht import RealSHT, InverseRealSHT, get_plan, resolve_precision  # noqa: F401
+from .vector_sht import RealVectorSHT, InverseRealVectorSHT  # noqa: F401
 from .spectral_convolution import SpectralConv, SpectralAttention, ComplexReLU, mix_packed  # noqa: F401
 from .host_pipeline import HostFeed  # noqa: F401
 

@@ -15,6 +15,7 @@ HEADER_PATH = os.path.join(_HERE, "..", "include", "b200sht.h")
 
 F32, BF16 = 0, 1
 PREC_FP32, PREC_TF32, PREC_FP32X3 = 0, 1, 2
+PLAN_FFT_ONLY, PLAN_VECTOR = 1, 2
 OP_DHCONV, OP_DIAGONAL, OP_SEP_DHCONV, OP_SEP_DIAGONAL, OP_SHARED, OP_LDEP = range(6)
 DENSE_FLAG = 0x100
 
@@ -65,6 +66,17 @@ _SIGNATURES = {
     "b200sht_mix_backward": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     "b200sht_complex_relu_forward": (c_int, [c_int, c_int, c_int, _P, _P, c_float, _P, c_int, c_int, _P]),
     "b200sht_complex_relu_backward": (c_int, [c_int, c_int, c_int, _P, _P, c_float, _P, _P, _P, c_int, c_int, _P]),
+    # vector SHT
+    "b200sht_vector_legendre_analysis": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P]),
+    "b200sht_vector_legendre_synthesis": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P]),
+    "b200sht_vector_legendre_synthesis_tiled": (c_int, [_P, _P, _P, c_int, c_int, _P]),
+    "b200sht_vector_spec_unpack": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P]),
+    "b200sht_vector_spec_pack": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P]),
+    "b200sht_vsht_workspace_bytes": (c_int64, [_P, c_int, c_int]),
+    "b200sht_vsht_forward": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_int, _P]),
+    "b200sht_vsht_inverse": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P, c_int, _P]),
+    "b200sht_vsht_forward_adjoint": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P, c_int, _P]),
+    "b200sht_vsht_inverse_adjoint": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, c_int, _P]),
     "b200sht_spectral_conv_workspace_bytes": (c_int64, [_P, _P, _P]),
     "b200sht_spectral_conv_forward": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "b200sht_spectral_conv_backward": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
@@ -86,6 +98,7 @@ _SIGNATURES = {
     "b200sht_debug_set_pdl": (c_int, [c_int]),
     "b200sht_debug_fft_plan": (c_int, [c_int, _P, c_int]),
     "b200sht_debug_table_host": (c_int, [c_int, c_int, c_int, _P, c_int, _P]),
+    "b200sht_debug_vector_table_host": (c_int, [c_int, c_int, c_int, _P, c_int, _P, _P]),
 }
 
 

@@ -32,6 +32,8 @@ def install_torch_harmonics_shim(force=False):
     th.__version__ = "0.9.0+b200"
     th.RealSHT = mb.RealSHT
     th.InverseRealSHT = mb.InverseRealSHT
+    th.RealVectorSHT = mb.RealVectorSHT
+    th.InverseRealVectorSHT = mb.InverseRealVectorSHT
     th.quadrature = mbq
     th.distributed = mbd
     th.__path__ = []  # mark as package so that submodule imports resolve through sys.modules

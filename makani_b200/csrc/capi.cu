@@ -71,6 +71,7 @@ static inline int cp_of(int C) { return round_up(C, 4); }
 // dims-only plan for the entry points that depend on (L, M) alone
 static inline Plan lm_plan(int L, int M, int m0 = 0, int dense = 0) { Plan p; memset(&p, 0, sizeof(p)); p.lmax = L; p.mmax = M; p.m0 = m0; p.dense = dense; return p; }
 int latspec_convert(const Plan* pl, float* lat, void* coeffs, int B, int C, int to_packed, cudaStream_t st);
+int vector_spec_convert(const Plan* pl, float* spec, void* coeffs, int B, int C, int to_packed, int scaled, cudaStream_t st);
 int umma_available();
 
 }  // namespace b200sht
@@ -93,10 +94,13 @@ int b200sht_plan_create_ex(b200sht_plan** out, int nlat, int nlon, int lmax, int
   B200_REQUIRE(nlat >= 1 && nlon >= 2 && lmax >= 1 && mmax >= 1 && m_offset >= 0, "plan_create: bad sizes nlat=%d nlon=%d lmax=%d mmax=%d m_offset=%d", nlat,
                nlon, lmax, mmax, m_offset);
   B200_REQUIRE(m_offset + mmax <= nlon / 2 + 1, "plan_create: m_offset+mmax=%d exceeds nlon/2+1=%d", m_offset + mmax, nlon / 2 + 1);
+  const int vector = (flags & B200SHT_PLAN_VECTOR) ? 1 : 0;
+  B200_REQUIRE(!vector || (m_offset == 0 && !(flags & B200SHT_PLAN_FFT_ONLY)), "plan_create: a vector plan has no order offset and holds tables");
+  B200_REQUIRE(!vector || lmax <= (1 << 29), "plan_create: lmax=%d too large", lmax);
   b200sht_plan* pl = new b200sht_plan();
   memset(static_cast<Plan*>(pl), 0, sizeof(Plan));
-  pl->nlat = nlat; pl->nlon = nlon; pl->lmax = lmax; pl->mmax = mmax; pl->kp = round_up(nlat, 8); pl->csphase = csphase;
-  pl->m0 = m_offset; pl->no_table = (flags & 1) ? 1 : 0;
+  pl->nlat = nlat; pl->nlon = nlon; pl->lmax = vector ? 2 * lmax : lmax; pl->mmax = mmax; pl->kp = round_up(nlat, 8); pl->csphase = csphase;
+  pl->m0 = m_offset; pl->no_table = (flags & B200SHT_PLAN_FFT_ONLY) ? 1 : 0; pl->vector = vector;
   if (!make_fft_plan(nlon, &pl->fft)) {
     set_error("plan_create: nlon=%d has a prime factor > 13 (unsupported FFT length)", nlon);
     delete pl;
@@ -106,7 +110,7 @@ int b200sht_plan_create_ex(b200sht_plan** out, int nlat, int nlon, int lmax, int
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&pl->sm_count, cudaDevAttrMultiProcessorCount, dev);
-  const size_t tbytes = pl->no_table ? 16 : sizeof(float) * (size_t)mmax * lmax * pl->kp;
+  const size_t tbytes = pl->no_table ? 16 : sizeof(float) * (size_t)mmax * pl->lmax * pl->kp;
   double* d_cost = nullptr;
   if (e == cudaSuccess) e = cudaMalloc(&pl->d_table, tbytes);
   if (e == cudaSuccess) e = cudaMalloc(&pl->d_rowscale, sizeof(float) * pl->kp);
@@ -164,13 +168,14 @@ int64_t b200sht_plan_query(const b200sht_plan* pl, int what) {
   switch (what) {
     case 0: return pl->nlat;
     case 1: return pl->nlon;
-    case 2: return pl->lmax;
+    case 2: return pl->vector ? pl->lmax / 2 : pl->lmax;
     case 3: return pl->mmax;
     case 4: return pl->kp;
     case 5: return (int64_t)sizeof(float) * pl->mmax * pl->lmax * pl->kp;
     case 6: return pl->umma_ok;
     case 7: return pl->m0;
     case 8: return (pl->umma_ok && dft_usable(pl)) ? 1 : 0;
+    case 9: return pl->vector;
     default: return -1;
   }
 }
@@ -178,6 +183,13 @@ int64_t b200sht_plan_query(const b200sht_plan* pl, int what) {
 const float* b200sht_plan_table(const b200sht_plan* pl) { return pl ? pl->d_table : nullptr; }
 int b200sht_plan_copy_table(const b200sht_plan* pl, float* dst, void* stream) {
   B200_REQUIRE(pl && dst, "plan_copy_table: null argument");
+  if (pl->vector) {   // D [mmax][lmax][kp], then Q: the two halves of each order's rows
+    const size_t half = sizeof(float) * (size_t)(pl->lmax / 2) * pl->kp;
+    for (int t = 0; t < 2; ++t)
+      B200_CHECK_CUDA(cudaMemcpy2DAsync(reinterpret_cast<char*>(dst) + t * half * pl->mmax, half, reinterpret_cast<const char*>(pl->d_table) + t * half,
+                                        2 * half, half, pl->mmax, cudaMemcpyDeviceToDevice, S(stream)));
+    return 0;
+  }
   B200_CHECK_CUDA(cudaMemcpyAsync(dst, pl->d_table, sizeof(float) * (size_t)pl->mmax * pl->lmax * pl->kp, cudaMemcpyDeviceToDevice, S(stream)));
   return 0;
 }
@@ -235,7 +247,10 @@ static int check_precision(int umma_ok, int precision, const char* who) {
   return B200SHT_ERR_INVALID;
 }
 
-int b200sht_legendre_analysis(const b200sht_plan* pl, const float* latspec, float* spec, int B, int C, int precision, void* stream) {
+}  // extern "C"
+// The Legendre stages on any plan with a table: the scalar entry points below serve scalar plans, the vector ones (b200sht_vector_*) run the
+// same contractions on a vector plan's stacked D / Q table with the 2C component rows of C vector fields.
+static int legendre_analysis_any(const b200sht_plan* pl, const float* latspec, float* spec, int B, int C, int precision, void* stream) {
   B200_REQUIRE(pl && latspec && spec && B > 0 && C > 0, "legendre_analysis: bad argument");
   B200_REQUIRE(!pl->no_table, "legendre_analysis: FFT-only plan");
   int rc = check_precision(pl->umma_ok, precision, "legendre_analysis");
@@ -253,7 +268,7 @@ int b200sht_legendre_analysis(const b200sht_plan* pl, const float* latspec, floa
   return legendre_analysis_simt(pl, latspec, spec, B, C, S(stream));
 }
 
-int b200sht_legendre_synthesis(const b200sht_plan* pl, const float* spec, float* latspec, int B, int C, int precision, void* stream) {
+static int legendre_synthesis_any(const b200sht_plan* pl, const float* spec, float* latspec, int B, int C, int precision, void* stream) {
   B200_REQUIRE(pl && latspec && spec && B > 0 && C > 0, "legendre_synthesis: bad argument");
   B200_REQUIRE(!pl->no_table, "legendre_synthesis: FFT-only plan");
   int rc = check_precision(pl->umma_ok, precision, "legendre_synthesis");
@@ -271,11 +286,28 @@ int b200sht_legendre_synthesis(const b200sht_plan* pl, const float* spec, float*
   return legendre_synthesis_simt(pl, spec, latspec, B, C, S(stream));
 }
 
-int b200sht_legendre_synthesis_tiled(const b200sht_plan* pl, const float* spec, float* latspec, int B, int C, void* stream) {
+static int legendre_synthesis_tiled_any(const b200sht_plan* pl, const float* spec, float* latspec, int B, int C, void* stream) {
   B200_REQUIRE(pl && latspec && spec && B > 0 && C > 0, "legendre_synthesis_tiled: bad argument");
   B200_REQUIRE(!pl->no_table, "legendre_synthesis_tiled: FFT-only plan");
   B200_REQUIRE(pl->umma_ok && dft_usable(pl), "legendre_synthesis_tiled: the tensor-core DFT is not available for this plan (b200sht_plan_query(plan, 8) == 0)");
   return legendre_synthesis_umma(pl, spec, latspec, B, C, 1, S(stream));
+}
+extern "C" {
+
+#define B200_SCALAR_PLAN(pl, who) B200_REQUIRE((pl) == nullptr || !(pl)->vector, who ": vector plan given to a scalar-transform entry point (use b200sht_vector_* / b200sht_vsht_*)")
+#define B200_VECTOR_PLAN(pl, who) B200_REQUIRE((pl) != nullptr && (pl)->vector, who ": needs a vector plan (b200sht_plan_create_ex with B200SHT_PLAN_VECTOR)")
+
+int b200sht_legendre_analysis(const b200sht_plan* pl, const float* latspec, float* spec, int B, int C, int precision, void* stream) {
+  B200_SCALAR_PLAN(pl, "legendre_analysis");
+  return legendre_analysis_any(pl, latspec, spec, B, C, precision, stream);
+}
+int b200sht_legendre_synthesis(const b200sht_plan* pl, const float* spec, float* latspec, int B, int C, int precision, void* stream) {
+  B200_SCALAR_PLAN(pl, "legendre_synthesis");
+  return legendre_synthesis_any(pl, spec, latspec, B, C, precision, stream);
+}
+int b200sht_legendre_synthesis_tiled(const b200sht_plan* pl, const float* spec, float* latspec, int B, int C, void* stream) {
+  B200_SCALAR_PLAN(pl, "legendre_synthesis_tiled");
+  return legendre_synthesis_tiled_any(pl, spec, latspec, B, C, stream);
 }
 
 // Longitude analysis + Legendre analysis.  At TF32 with the tensor-core DFT the pair can run in latitude chunks: the DFT writes the latspec
@@ -322,11 +354,11 @@ static int synthesis_pair(const b200sht_plan* pl, const float* spec, float* lat,
       }
       return rc;
     }
-    int rc = b200sht_legendre_synthesis_tiled(pl, spec, lat, B, C, stream);
+    int rc = legendre_synthesis_tiled_any(pl, spec, lat, B, C, stream);
     if (!rc) rc = b200sht_fft_synthesis(pl, lat, y, dtype, B, C, bias, mode | 2, stream);
     return rc;
   }
-  int rc = b200sht_legendre_synthesis(pl, spec, lat, B, C, precision, stream);
+  int rc = legendre_synthesis_any(pl, spec, lat, B, C, precision, stream);
   if (!rc) rc = b200sht_fft_synthesis(pl, lat, y, dtype, B, C, bias, mode, stream);
   return rc;
 }
@@ -337,7 +369,7 @@ static int analysis_pair(const b200sht_plan* pl, const void* x, int dtype, int B
   const int n = dft ? lat_chunks(pl, B, C) : 1;
   if (n <= 1) {
     int rc = b200sht_fft_analysis(pl, x, dtype, B, C, lat, mode | (precision == B200SHT_PREC_TF32 ? 2 : 0), stream);
-    if (!rc) rc = b200sht_legendre_analysis(pl, lat, spec, B, C, precision, stream);
+    if (!rc) rc = legendre_analysis_any(pl, lat, spec, B, C, precision, stream);
     return rc;
   }
   B200_REQUIRE(B > 0 && C > 0 && (long long)B * C <= 65535, "analysis: B*C=%lld out of range", (long long)B * C);
@@ -400,6 +432,7 @@ static void split_ws(const b200sht_plan* pl, int B, int C, void* ws, float** lat
 
 int b200sht_sht_forward(const b200sht_plan* pl, const void* x, int dtype, int B, int C, void* coeffs, void* ws, int precision, void* stream) {
   B200_REQUIRE(pl && x && coeffs && ws, "sht_forward: null argument");
+  B200_SCALAR_PLAN(pl, "sht_forward");
   float *X, *sp;
   split_ws(pl, B, C, ws, &X, &sp);
   int rc = analysis_pair(pl, x, dtype, B, C, X, sp, 0, precision, stream);
@@ -409,6 +442,7 @@ int b200sht_sht_forward(const b200sht_plan* pl, const void* x, int dtype, int B,
 
 int b200sht_sht_inverse(const b200sht_plan* pl, const void* coeffs, void* y, int dtype, int B, int C, void* ws, int precision, void* stream) {
   B200_REQUIRE(pl && y && coeffs && ws, "sht_inverse: null argument");
+  B200_SCALAR_PLAN(pl, "sht_inverse");
   float *Z, *sp;
   split_ws(pl, B, C, ws, &Z, &sp);
   int rc = b200sht_spec_pack(pl->lmax, pl->mmax, coeffs, sp, B, C, stream);
@@ -419,6 +453,7 @@ int b200sht_sht_inverse(const b200sht_plan* pl, const void* coeffs, void* y, int
 int b200sht_sht_forward_adjoint(const b200sht_plan* pl, const void* gcoeffs, void* gx, int dtype, int B, int C, void* ws, int precision,
                                 void* stream) {
   B200_REQUIRE(pl && gx && gcoeffs && ws, "sht_forward_adjoint: null argument");
+  B200_SCALAR_PLAN(pl, "sht_forward_adjoint");
   float *Z, *sp;
   split_ws(pl, B, C, ws, &Z, &sp);
   int rc = b200sht_spec_pack(pl->lmax, pl->mmax, gcoeffs, sp, B, C, stream);
@@ -429,10 +464,95 @@ int b200sht_sht_forward_adjoint(const b200sht_plan* pl, const void* gcoeffs, voi
 int b200sht_sht_inverse_adjoint(const b200sht_plan* pl, const void* gy, int dtype, int B, int C, void* gcoeffs, void* ws, int precision,
                                 void* stream) {
   B200_REQUIRE(pl && gy && gcoeffs && ws, "sht_inverse_adjoint: null argument");
+  B200_SCALAR_PLAN(pl, "sht_inverse_adjoint");
   float *X, *sp;
   split_ws(pl, B, C, ws, &X, &sp);
   int rc = analysis_pair(pl, gy, dtype, B, C, X, sp, 1, precision, stream);
   if (!rc) rc = b200sht_spec_unpack(pl->lmax, pl->mmax, sp, gcoeffs, B, C, stream);
+  return rc;
+}
+
+// ---------------------------------------------------------------------------------- vector SHT boundary
+// Stage buffers of C vector fields are the scalar formats of their 2C component rows (b, c, component), with the vector plan's 2 lmax table rows.
+static int vector_precision(int precision, const char* who) {
+  if (precision == B200SHT_PREC_FP32X3) {
+    set_error("%s: the vector transforms have no 3 x TF32 mode (use B200SHT_PREC_FP32 or B200SHT_PREC_TF32)", who);
+    return B200SHT_ERR_UNSUPPORTED;
+  }
+  return 0;
+}
+#define B200_VECTOR_ARGS(pl, C, precision, who)                                                              \
+  B200_VECTOR_PLAN(pl, who);                                                                                 \
+  B200_REQUIRE((C) > 0 && (C) <= (1 << 28), who ": bad channel count %d", (C));                             \
+  if (int _rc = vector_precision(precision, who)) return _rc
+
+int b200sht_vector_legendre_analysis(const b200sht_plan* pl, const float* latspec, float* spec, int B, int C, int precision, void* stream) {
+  B200_VECTOR_ARGS(pl, C, precision, "vector_legendre_analysis");
+  return legendre_analysis_any(pl, latspec, spec, B, 2 * C, precision, stream);
+}
+int b200sht_vector_legendre_synthesis(const b200sht_plan* pl, const float* spec, float* latspec, int B, int C, int precision, void* stream) {
+  B200_VECTOR_ARGS(pl, C, precision, "vector_legendre_synthesis");
+  return legendre_synthesis_any(pl, spec, latspec, B, 2 * C, precision, stream);
+}
+int b200sht_vector_legendre_synthesis_tiled(const b200sht_plan* pl, const float* spec, float* latspec, int B, int C, void* stream) {
+  B200_VECTOR_ARGS(pl, C, B200SHT_PREC_TF32, "vector_legendre_synthesis_tiled");
+  return legendre_synthesis_tiled_any(pl, spec, latspec, B, 2 * C, stream);
+}
+int b200sht_vector_spec_unpack(const b200sht_plan* pl, const float* spec, void* coeffs, int B, int C, int scaled, void* stream) {
+  B200_VECTOR_ARGS(pl, C, B200SHT_PREC_FP32, "vector_spec_unpack");
+  B200_REQUIRE(spec && coeffs && B > 0, "vector_spec_unpack: bad argument");
+  return vector_spec_convert(pl, const_cast<float*>(spec), coeffs, B, C, 0, scaled ? 1 : 0, S(stream));
+}
+int b200sht_vector_spec_pack(const b200sht_plan* pl, const void* coeffs, float* spec, int B, int C, int scaled, void* stream) {
+  B200_VECTOR_ARGS(pl, C, B200SHT_PREC_FP32, "vector_spec_pack");
+  B200_REQUIRE(spec && coeffs && B > 0, "vector_spec_pack: bad argument");
+  return vector_spec_convert(pl, spec, const_cast<void*>(coeffs), B, C, 1, scaled ? 1 : 0, S(stream));
+}
+
+int64_t b200sht_vsht_workspace_bytes(const b200sht_plan* pl, int B, int C) {
+  if (!pl || !pl->vector || B <= 0 || C <= 0 || C > (1 << 28)) return -1;
+  return b200sht_sht_workspace_bytes(pl, B, 2 * C);
+}
+
+int b200sht_vsht_forward(const b200sht_plan* pl, const void* x, int dtype, int B, int C, void* coeffs, void* ws, int precision, void* stream) {
+  B200_VECTOR_ARGS(pl, C, precision, "vsht_forward");
+  B200_REQUIRE(x && coeffs && ws && B > 0, "vsht_forward: bad argument");
+  float *X, *sp;
+  split_ws(pl, B, 2 * C, ws, &X, &sp);
+  int rc = analysis_pair(pl, x, dtype, B, 2 * C, X, sp, 0, precision, stream);
+  if (!rc) rc = vector_spec_convert(pl, sp, coeffs, B, C, 0, 1, S(stream));
+  return rc;
+}
+
+int b200sht_vsht_inverse(const b200sht_plan* pl, const void* coeffs, void* y, int dtype, int B, int C, void* ws, int precision, void* stream) {
+  B200_VECTOR_ARGS(pl, C, precision, "vsht_inverse");
+  B200_REQUIRE(y && coeffs && ws && B > 0, "vsht_inverse: bad argument");
+  float *Z, *sp;
+  split_ws(pl, B, 2 * C, ws, &Z, &sp);
+  int rc = vector_spec_convert(pl, sp, const_cast<void*>(coeffs), B, C, 1, 0, S(stream));
+  if (!rc) rc = synthesis_pair(pl, sp, Z, y, dtype, B, 2 * C, nullptr, 0, precision, stream);
+  return rc;
+}
+
+int b200sht_vsht_forward_adjoint(const b200sht_plan* pl, const void* gcoeffs, void* gx, int dtype, int B, int C, void* ws, int precision,
+                                 void* stream) {
+  B200_VECTOR_ARGS(pl, C, precision, "vsht_forward_adjoint");
+  B200_REQUIRE(gx && gcoeffs && ws && B > 0, "vsht_forward_adjoint: bad argument");
+  float *Z, *sp;
+  split_ws(pl, B, 2 * C, ws, &Z, &sp);
+  int rc = vector_spec_convert(pl, sp, const_cast<void*>(gcoeffs), B, C, 1, 1, S(stream));
+  if (!rc) rc = synthesis_pair(pl, sp, Z, gx, dtype, B, 2 * C, nullptr, 1, precision, stream);
+  return rc;
+}
+
+int b200sht_vsht_inverse_adjoint(const b200sht_plan* pl, const void* gy, int dtype, int B, int C, void* gcoeffs, void* ws, int precision,
+                                 void* stream) {
+  B200_VECTOR_ARGS(pl, C, precision, "vsht_inverse_adjoint");
+  B200_REQUIRE(gy && gcoeffs && ws && B > 0, "vsht_inverse_adjoint: bad argument");
+  float *X, *sp;
+  split_ws(pl, B, 2 * C, ws, &X, &sp);
+  int rc = analysis_pair(pl, gy, dtype, B, 2 * C, X, sp, 1, precision, stream);
+  if (!rc) rc = vector_spec_convert(pl, sp, gcoeffs, B, C, 0, 0, S(stream));
   return rc;
 }
 
@@ -533,6 +653,7 @@ static ConvWs conv_ws(const b200sht_plan* f, const b200sht_plan* v, const b200sh
 
 static int check_conv(const b200sht_plan* f, const b200sht_plan* v, const b200sht_conv_desc* d) {
   B200_REQUIRE(f && v && d, "spectral_conv: null argument");
+  B200_REQUIRE(!f->vector && !v->vector, "spectral_conv: vector plan given to a scalar-transform entry point");
   B200_REQUIRE(f->lmax == v->lmax && f->mmax == v->mmax, "spectral_conv: forward (%d,%d) and inverse (%d,%d) mode counts differ", f->lmax, f->mmax,
                v->lmax, v->mmax);
   B200_REQUIRE(d->B > 0 && d->G > 0 && d->Cin % d->G == 0 && d->Cout % d->G == 0, "spectral_conv: channels (%d,%d) not divisible by groups %d", d->Cin,

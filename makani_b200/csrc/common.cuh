@@ -61,7 +61,8 @@ struct FftPlan {
 
 // The immutable plan object behind b200sht_plan.
 struct Plan {
-  int nlat, nlon, lmax, mmax, kp;
+  int nlat, nlon, lmax, mmax, kp;   // lmax: table rows; a vector plan stacks D over Q, so there it is twice the caller's lmax
+  int vector;           // vector-SHT plan: d_table[m] holds D (rows 0 .. lmax/2 - 1) then Q (rows lmax/2 .. lmax - 1), see legendre.cu
   int csphase;
   int m0;               // global order of local order 0 (m-sharded plans of the distributed SHT); 0 otherwise
   int no_table;         // FFT-only plan (latitude-sharded stage of the distributed SHT)

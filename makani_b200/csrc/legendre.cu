@@ -38,6 +38,41 @@ HD void legendre_column(int m, int lmax, double x, int csphase, float* out, size
   }
 }
 
+// Tables of the vector SHT for order m at x = cos(theta), fp64 recurrence, fp32 storage, exact zeros for l < m:
+//   D[l] = dP_l^m(cos theta) / dtheta,   Q[l] = m P_l^m(cos theta) / sin(theta)   (orthonormal P, optional Condon-Shortley phase).
+// Pole-safe without a division by sin(theta): for m >= 1 the recurrence runs on P / sin(theta) (seeded with sin^(m-1) theta), and
+//   D_l = l cos(theta) P_l / sin(theta) - sqrt((2l+1)/(2l-1) (l-m)(l+m)) P_{l-1} / sin(theta),
+// for m = 0 it runs on P_l^1 (no phase) and D_l = -sqrt(l (l+1)) P_l^1.
+HD void legendre_vector_column(int m, int lmax, double x, int csphase, float* D, float* Q, size_t stride) {
+  const double s = sqrt((1.0 + x) * (1.0 - x));
+  const double sgn = (csphase && (m & 1)) ? -1.0 : 1.0;
+  for (int l = 0; l < m && l < lmax; ++l) D[(size_t)l * stride] = Q[(size_t)l * stride] = 0.f;
+  if (m >= lmax) return;
+  const int mu = m == 0 ? 1 : m;   // order of the recurrence
+  double cur = 0.28209479177387814347;
+  for (int l = 1; l <= mu; ++l) cur *= sqrt((2.0 * l + 1.0) / (2.0 * l)) * ((m == 0 || l > 1) ? s : 1.0);
+  double prev = 0.0;
+  if (m == 0) D[0] = Q[0] = 0.f;
+  for (int l = mu; l < lmax; ++l) {
+    if (l > mu) {
+      const double nxt = (l == mu + 1) ? sqrt(2.0 * mu + 3.0) * x * cur
+                                       : x * sqrt((2.0 * l - 1.0) / (double)(l - mu) * (2.0 * l + 1.0) / (double)(l + mu)) * cur -
+                                             sqrt((double)(l + mu - 1) / (double)(l - mu) * (2.0 * l + 1.0) / (2.0 * l - 3.0) * (double)(l - mu - 1) /
+                                                  (double)(l + mu)) * prev;
+      prev = cur;
+      cur = nxt;
+    }
+    if (m == 0) {
+      D[(size_t)l * stride] = (float)(-sqrt((double)l * (l + 1)) * cur);
+      Q[(size_t)l * stride] = 0.f;
+    } else {
+      const double a = sqrt((2.0 * l + 1.0) / (2.0 * l - 1.0) * (double)(l - m) * (double)(l + m));
+      D[(size_t)l * stride] = (float)(sgn * (l * x * cur - a * prev));
+      Q[(size_t)l * stride] = (float)(sgn * m * cur);
+    }
+  }
+}
+
 __global__ void round_tf32_kernel(const float* __restrict__ src, float* __restrict__ dst, size_t n) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) dst[i] = tf32_rn(src[i]);
@@ -93,9 +128,26 @@ __global__ void build_table_kernel(float* __restrict__ table, const double* __re
   legendre_column(m0 + m, lmax, cost[k], csphase, out, kp);
 }
 
+// vector plan: table[m] = D rows [0, L) then Q rows [L, 2L)   (L = lmax / 2)
+__global__ void build_vector_table_kernel(float* __restrict__ table, const double* __restrict__ cost, int nlat, int kp, int L, int csphase) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  const int m = blockIdx.y;
+  if (k >= kp) return;
+  float* D = table + (size_t)m * 2 * L * kp + k;
+  float* Q = D + (size_t)L * kp;
+  if (k >= nlat) {
+    for (int l = 0; l < L; ++l) D[(size_t)l * kp] = Q[(size_t)l * kp] = 0.f;
+    return;
+  }
+  legendre_vector_column(m, L, cost[k], csphase, D, Q, kp);
+}
+
 int build_table(Plan* pl, const double* d_cost, cudaStream_t st) {
   dim3 grid(ceil_div(pl->kp, 128), pl->mmax);
-  build_table_kernel<<<grid, 128, 0, st>>>(pl->d_table, d_cost, pl->nlat, pl->kp, pl->lmax, pl->mmax, pl->csphase, pl->m0);
+  if (pl->vector)
+    build_vector_table_kernel<<<grid, 128, 0, st>>>(pl->d_table, d_cost, pl->nlat, pl->kp, pl->lmax / 2, pl->csphase);
+  else
+    build_table_kernel<<<grid, 128, 0, st>>>(pl->d_table, d_cost, pl->nlat, pl->kp, pl->lmax, pl->mmax, pl->csphase, pl->m0);
   B200_CHECK_LAUNCH();
   return 0;
 }
@@ -317,6 +369,91 @@ int spec_pack(const Plan* pl, const void* coeffs, float* spec, int B, int C, cud
   return 0;
 }
 
+// ------------------------------------------------------------------------------- vector SHT boundary
+// stacked vector spec [2L][M][2][B][cp] (cp = round_up(2C, 4); column 2c + component, component 0 = theta, 1 = phi; rows l hold the
+// D contractions, rows L + l the Q contractions)  <->  (S, T) complex64 [B*C][2][L][M] (exact zeros for l < m):
+//   unpack:  S = f (D x_theta - i Q x_phi),   T = f (-i Q x_theta - D x_phi)
+//   pack:    D_theta = f S,  D_phi = -f T,  Q_theta = i f T,  Q_phi = i f S
+// f = 1 / (l (l + 1)) (0 at l = 0) when `scaled`, else 1.  pack(scaled) is the adjoint of unpack(scaled): the forward transform ends in
+// unpack(1) and its adjoint starts with pack(1); the inverse transform starts with pack(0) and its adjoint ends in unpack(0).
+// block: 32 orders x 16 vector channels (32 spec columns) of one (l, b)
+__global__ void __launch_bounds__(256) vector_spec_unpack_kernel(const float* __restrict__ spec, float2* __restrict__ coeffs, int L, int M, int B,
+                                                                 int C, int cp, int scaled) {
+  __shared__ float tile[4][32][33];   // D re, D im, Q re, Q im  x  [m][column]
+  const int l = blockIdx.z / B, b = blockIdx.z % B;
+  const int m0 = blockIdx.x * 32, c0 = blockIdx.y * 16;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const size_t JP = 2 * (size_t)B * cp, pstride = (size_t)B * cp;
+  const int j = 2 * c0 + tx;
+  for (int mm = ty; mm < 32; mm += 8) {
+    const int m = m0 + mm;
+    float v[4] = {0.f, 0.f, 0.f, 0.f};
+    if (m < M && j < 2 * C && l >= m) {
+      const float* d = spec + ((size_t)l * M + m) * JP + (size_t)b * cp + j;
+      const float* q = d + (size_t)L * M * JP;
+      v[0] = d[0]; v[1] = d[pstride]; v[2] = q[0]; v[3] = q[pstride];
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) tile[i][mm][tx] = v[i];
+  }
+  __syncthreads();
+  const float f = scaled ? (l > 0 ? 1.f / ((float)l * (float)(l + 1)) : 0.f) : 1.f;
+  for (int cc = ty; cc < 16; cc += 8) {
+    const int c = c0 + cc, m = m0 + tx;
+    if (c >= C || m >= M) continue;
+    const int jt = 2 * cc, jf = 2 * cc + 1;
+    const float2 S = make_float2(f * (tile[0][tx][jt] + tile[3][tx][jf]), f * (tile[1][tx][jt] - tile[2][tx][jf]));
+    const float2 T = make_float2(f * (tile[3][tx][jt] - tile[0][tx][jf]), f * (-tile[2][tx][jt] - tile[1][tx][jf]));
+    float2* out = coeffs + ((size_t)(b * C + c) * 2 * L + l) * M + m;
+    out[0] = S;
+    out[(size_t)L * M] = T;
+  }
+}
+
+// writes every entry of the stacked spec (zeros for l < m and in the channel padding): the Legendre kernels read all rows l >= lstart(m)
+__global__ void __launch_bounds__(256) vector_spec_pack_kernel(const float2* __restrict__ coeffs, float* __restrict__ spec, int L, int M, int B,
+                                                               int C, int cp, int scaled) {
+  __shared__ float tile[4][32][33];
+  const int l = blockIdx.z / B, b = blockIdx.z % B;
+  const int m0 = blockIdx.x * 32, c0 = blockIdx.y * 16;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const size_t JP = 2 * (size_t)B * cp, pstride = (size_t)B * cp;
+  const float f = scaled ? (l > 0 ? 1.f / ((float)l * (float)(l + 1)) : 0.f) : 1.f;
+  for (int cc = ty; cc < 16; cc += 8) {
+    const int c = c0 + cc, m = m0 + tx;
+    float2 S = make_float2(0.f, 0.f), T = S;
+    if (c < C && m < M && l >= m) {
+      const float2* in = coeffs + ((size_t)(b * C + c) * 2 * L + l) * M + m;
+      S = in[0];
+      T = in[(size_t)L * M];
+      S.x *= f; S.y *= f; T.x *= f; T.y *= f;
+    }
+    const int jt = 2 * cc, jf = 2 * cc + 1;
+    tile[0][tx][jt] = S.x;  tile[1][tx][jt] = S.y;  tile[2][tx][jt] = -T.y; tile[3][tx][jt] = T.x;
+    tile[0][tx][jf] = -T.x; tile[1][tx][jf] = -T.y; tile[2][tx][jf] = -S.y; tile[3][tx][jf] = S.x;
+  }
+  __syncthreads();
+  for (int mm = ty; mm < 32; mm += 8) {
+    const int m = m0 + mm, j = 2 * c0 + tx;
+    if (m >= M || j >= cp) continue;
+    float* d = spec + ((size_t)l * M + m) * JP + (size_t)b * cp + j;
+    float* q = d + (size_t)L * M * JP;
+    d[0] = tile[0][mm][tx]; d[pstride] = tile[1][mm][tx]; q[0] = tile[2][mm][tx]; q[pstride] = tile[3][mm][tx];
+  }
+}
+
+int vector_spec_convert(const Plan* pl, float* spec, void* coeffs, int B, int C, int to_packed, int scaled, cudaStream_t st) {
+  const int L = pl->lmax / 2, cp = round_up(2 * C, 4);
+  dim3 grid(ceil_div(pl->mmax, 32), to_packed ? ceil_div(cp, 32) : ceil_div(C, 16), L * B);
+  B200_REQUIRE(grid.z <= 65535, "vector spec conversion: lmax*B=%u exceeds grid limit", grid.z);
+  if (to_packed)
+    vector_spec_pack_kernel<<<grid, 256, 0, st>>>(static_cast<const float2*>(coeffs), spec, L, pl->mmax, B, C, cp, scaled);
+  else
+    vector_spec_unpack_kernel<<<grid, 256, 0, st>>>(spec, static_cast<float2*>(coeffs), L, pl->mmax, B, C, cp, scaled);
+  B200_CHECK_LAUNCH();
+  return 0;
+}
+
 // latspec [M][2][R][kp]  <->  complex64 [R][nlat][M]   (the layout the distributed transposes exchange).  block: 32 k x 32 m of one row r
 __global__ void __launch_bounds__(256) latspec_convert_kernel(float* __restrict__ lat, float2* __restrict__ coeffs, int M, int R, int nlat, int kp,
                                                               int to_packed) {
@@ -399,5 +536,16 @@ extern "C" int b200sht_debug_table_host(int nlat, int lmax, int mmax, const doub
   for (int m = 0; m < mmax; ++m)
     for (int k = 0; k < nlat; ++k)
       b200sht::legendre_column(m, lmax, cost[k], csphase, table + (size_t)m * lmax * nlat + k, nlat);
+  return 0;
+}
+
+extern "C" int b200sht_debug_vector_table_host(int nlat, int lmax, int mmax, const double* cost, int csphase, float* D /*[mmax][lmax][nlat]*/,
+                                               float* Q /*[mmax][lmax][nlat]*/) {
+  if (nlat < 1 || lmax < 1 || mmax < 1 || !cost || !D || !Q) return B200SHT_ERR_INVALID;
+  for (int m = 0; m < mmax; ++m)
+    for (int k = 0; k < nlat; ++k) {
+      const size_t o = (size_t)m * lmax * nlat + k;
+      b200sht::legendre_vector_column(m, lmax, cost[k], csphase, D + o, Q + o, nlat);
+    }
   return 0;
 }

@@ -58,7 +58,8 @@ def resolve_precision(precision="auto"):
 class Plan:
     """Owns one `b200sht_plan` (Legendre table, FFT twiddles, TMA descriptors) on one CUDA device."""
 
-    def __init__(self, nlat, nlon, lmax, mmax, grid, csphase, device):
+    def __init__(self, nlat, nlon, lmax, mmax, grid, csphase, device, vector=False):
+        """vector=True: a vector-SHT plan (tables D and Q instead of P) for RealVectorSHT / InverseRealVectorSHT."""
         if device.type != "cuda":
             raise B200ShtError("makani_b200 transforms run on CUDA devices only (no CPU fallback)")
         lib = _lib.load()
@@ -67,8 +68,12 @@ class Plan:
         w = np.ascontiguousarray(w, dtype=np.float64)
         handle = _VP()
         with torch.cuda.device(device):
-            rc = lib.b200sht_plan_create(ctypes.byref(handle), nlat, nlon, lmax, mmax, cost.ctypes.data_as(_VP), w.ctypes.data_as(_VP),
-                                         1 if csphase else 0, _stream(device))
+            if vector:
+                rc = lib.b200sht_plan_create_ex(ctypes.byref(handle), nlat, nlon, lmax, mmax, 0, _lib.PLAN_VECTOR, cost.ctypes.data_as(_VP),
+                                                w.ctypes.data_as(_VP), 1 if csphase else 0, _stream(device))
+            else:
+                rc = lib.b200sht_plan_create(ctypes.byref(handle), nlat, nlon, lmax, mmax, cost.ctypes.data_as(_VP), w.ctypes.data_as(_VP),
+                                             1 if csphase else 0, _stream(device))
         _lib.check(rc, "b200sht_plan_create")
         self._finish(handle, device, nlat, nlon, lmax, mmax, 0)
 
@@ -80,9 +85,11 @@ class Plan:
         self.kp = int(lib.b200sht_plan_query(handle, 4))
         self.umma_ok = bool(lib.b200sht_plan_query(handle, 6))
         self.dft_ok = bool(lib.b200sht_plan_query(handle, 8))
+        self.vector = bool(lib.b200sht_plan_query(handle, 9))
 
     def query(self, what):
-        """b200sht_plan_query: 0 nlat, 1 nlon, 2 lmax, 3 mmax, 4 kp, 5 table bytes, 6 tensor-core path available, 7 m_offset, 8 tensor-core DFT available."""
+        """b200sht_plan_query: 0 nlat, 1 nlon, 2 lmax, 3 mmax, 4 kp, 5 table bytes, 6 tensor-core path available, 7 m_offset, 8 tensor-core DFT available,
+        9 vector plan."""
         return int(_lib.load().b200sht_plan_query(self.handle, what))
 
     @classmethod
@@ -109,11 +116,11 @@ class Plan:
         return int(_lib.load().b200sht_spec_elems(self.handle, B, C))
 
     def table(self):
-        """Device view of the fp32 Legendre table [mmax][lmax][kp] (testing / inspection)."""
-        n = self.mmax * self.lmax * self.kp
-        out = torch.empty(n, dtype=torch.float32, device=self.device)
+        """Device copy of the fp32 Legendre table [mmax][lmax][kp]; of a vector plan the tables D and Q as [2][mmax][lmax][kp] (testing / inspection)."""
+        nt = 2 if self.vector else 1
+        out = torch.empty(nt * self.mmax * self.lmax * self.kp, dtype=torch.float32, device=self.device)
         _lib.call("b200sht_plan_copy_table", self.handle, _ptr(out), _stream(self.device))
-        return out.view(self.mmax, self.lmax, self.kp)
+        return out.view(nt, self.mmax, self.lmax, self.kp) if self.vector else out.view(self.mmax, self.lmax, self.kp)
 
     def __del__(self):
         try:
@@ -128,16 +135,19 @@ _plan_cache = {}
 _plan_lock = threading.Lock()
 
 
-def get_plan(nlat, nlon, lmax, mmax, grid, csphase, device):
-    """Plans are shared between modules with the same geometry on the same device (SFNO builds 4 transforms, FCN3 2)."""
+def get_plan(nlat, nlon, lmax, mmax, grid, csphase, device, vector=False):
+    """Plans are shared between modules with the same geometry on the same device (SFNO builds 4 transforms, FCN3 2).  vector=True: the
+    vector-SHT plan of that geometry (shared by RealVectorSHT and InverseRealVectorSHT), cached under its own key."""
     device = torch.device(device)
     if device.type == "cuda" and device.index is None:
         device = torch.device("cuda", torch.cuda.current_device())
     key = (nlat, nlon, lmax, mmax, grid, bool(csphase), device.index)
+    if vector:
+        key = key + ("vector",)
     with _plan_lock:
         p = _plan_cache.get(key)
         if p is None:
-            p = Plan(nlat, nlon, lmax, mmax, grid, csphase, device)
+            p = Plan(nlat, nlon, lmax, mmax, grid, csphase, device, vector=vector)
             _plan_cache[key] = p
         return p
 
