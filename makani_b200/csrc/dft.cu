@@ -9,14 +9,14 @@
 // pipe at TF32 and only one radix-8 stage stays on the CUDA cores; no shared-memory exchange between stages is left.
 //
 // synthesis kernel (latspec -> rows):   D[j2][(class c, latitude k)] for the columns j2 <= N2/2 and an 8-row tile.  A = E^T resident in
-//   shared memory (32 KB), B = the raw latspec tile [m2][(c, k)] streamed by TMA (16 KB per 8 rows) through an mbarrier ring, four
-//   accumulators S1..S4 (cos/sin x re/im) in registers.  A warp owns 16 columns j2; its m16n8 fragments give each thread the two
-//   latitudes 2 (lane % 4), + 1 of the columns j2 = lane / 4 (+ 8) for all eight classes, i.e. the inputs of its own butterflies:
-//   S -> V(j2), V(N2-j2) -> twiddle -> radix-8 -> scale/bias -> bf16 without any exchange.
+//   shared memory (32 KB), B = the raw latspec tile [m2][(c, k)] streamed by TMA (16 KB per 8 rows) through an mbarrier ring, the cosine
+//   and sine sums of Zr and Zi in registers.  A task owns 8 columns j2; its m16n8 fragments give each thread the two latitudes
+//   2 (lane % 4), + 1 of the column j2 = lane / 4 for all eight classes, i.e. the inputs of its own butterflies:
+//   S -> V(j2), V(N2-j2) -> twiddle -> radix-8 -> scale/bias -> bf16 into a shared-memory output tile, written out by TMA bulk stores.
 // analysis kernel (rows -> latspec):    producer warps load the eight samples x[N2 j1 + j2] of a column (lanes = consecutive j2),
 //   butterfly + twiddle them and write the even/odd combinations (Ye, Yo) as K-major TF32 operand tiles [(c, k)][j2] (128-byte
-//   swizzle, conflict-free row stores); B = E resident (<= 24 KB); four MMA warps accumulate D[(c,k)][m2] in registers over the K-blocks
-//   and write latspec straight from their fragments (32-byte runs along k).
+//   swizzle, conflict-free row stores); B = E resident (<= 24 KB); eight MMA warps (one class each) accumulate D[(c,k)][m2] in registers
+//   over the K-blocks and write latspec straight from their fragments (32-byte runs along k).
 #include "umma_common.cuh"
 #include "dft_math.cuh"
 #include <cmath>
@@ -28,15 +28,20 @@ namespace b200sht {
 int umma_available();   // umma.cu
 
 constexpr int kDftMaxHalf = 95;    // N2 / 2 <= 95: three 32-lane quadrants (synthesis) / three K-blocks (analysis)
-constexpr int kDftSynWorkers = 7;                        // MMA + epilogue warps of the synthesis kernel
-constexpr int kDftSynThreads = 32 * (kDftSynWorkers + 1);   // + one TMA warp
-constexpr int kDftSynStages = 8;   // 16 KB each
+constexpr int kDftSynWorkers = 10;   // MMA + epilogue warps of the synthesis kernel
+constexpr int kDftSynThreads = 32 * (kDftSynWorkers + 2);   // + a TMA load warp and a TMA store warp: 3 warps per SM sub-partition, 168 registers
+constexpr int kDftSynStages = 4;   // 16 KB each
+// width of the output store box: the largest 8 d <= 256 (the TMA box limit) with d | N2, so that a row is a whole number of boxes
+__host__ __device__ constexpr int dft_out_box(int N2) {
+  int d = N2 < 32 ? N2 : 32;
+  while (N2 % d != 0) --d;
+  return 8 * d;
+}
 
 struct DftTables {
-  float* et;      // synthesis A: [2][128 rows j2][32 m2]  (cos, sin), TF32-rounded; rows j2 > N2 / 2 are zero
+  float* et;      // synthesis A: [16 blocks of 8 j2][cos, sin][8 rows j2][32 m2], TF32-rounded; rows j2 > N2 / 2 are zero
   float* eb;      // analysis  B: [nkb][2][32 rows m2][32 j2 local]  (cos, sin), TF32-rounded
   float2* tw;     // [8][N2]  exp(+2 pi i c j2 / nlon)
-  float* trash;   // 64 x (4 * nlon + 256) floats: store target of the synthesis rows / lanes without output (keeps the stores unconditional); one slab per CTA % 64
   float* zeros;   // 8 * N2 floats of zeros: load target of the analysis lanes / rows that carry no sample (keeps the loads unconditional)
   int N2, half, M2, nkb;
 };
@@ -49,9 +54,9 @@ bool dft_shape_ok(int nlon, int mmax) {
 
 __global__ void dft_tables_kernel(float* et, float* eb, float2* tw, int N2, int half, int M2, int nkb, int nlon) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  // E^T tiles: [2][128][32]
+  // E^T tile: [16 blocks][cos, sin][8 rows j2][32 m2]
   if (i < 2 * 128 * 32) {
-    const int m2 = i % 32, j2 = (i / 32) % 128, p = i / (32 * 128);
+    const int m2 = i % 32, row = i / 32, p = (row >> 3) & 1, j2 = 8 * (row >> 4) + (row & 7);
     float v = 0.f;
     if (j2 <= half && m2 < M2) {
       const long long t = ((long long)m2 * j2) % N2;
@@ -86,14 +91,13 @@ int dft_plan_init(Plan* pl) {
   DftTables* t = new DftTables();
   t->N2 = pl->nlon / 8; t->half = t->N2 / 2; t->M2 = (pl->mmax + 7) / 8;
   t->nkb = (t->half + 1 + 31) / 32;   // 32-column K-blocks of j2 = 0 .. N2 / 2 (analysis)
-  t->et = nullptr; t->eb = nullptr; t->tw = nullptr; t->zeros = nullptr; t->trash = nullptr;
+  t->et = nullptr; t->eb = nullptr; t->tw = nullptr; t->zeros = nullptr;
   const size_t neb = (size_t)t->nkb * 2 * 32 * 32;
   cudaError_t e = cudaMalloc(&t->et, sizeof(float) * 2 * 128 * 32);
   if (e == cudaSuccess) e = cudaMalloc(&t->eb, sizeof(float) * neb);
   if (e == cudaSuccess) e = cudaMalloc(&t->tw, sizeof(float2) * 8 * t->N2);
   if (e == cudaSuccess) e = cudaMalloc(&t->zeros, sizeof(float) * 8 * t->N2);
   if (e == cudaSuccess) e = cudaMemset(t->zeros, 0, sizeof(float) * 8 * t->N2);
-  if (e == cudaSuccess) e = cudaMalloc(&t->trash, sizeof(float) * 64 * (4 * (size_t)pl->nlon + 256));   // + 256: idle lanes index up to j2 = 127 + 7 N2 past a row
   if (e == cudaSuccess) {
     const int n = 8192 > 8 * t->N2 ? 8192 : 8 * t->N2;
     dft_tables_kernel<<<(n + 255) / 256, 256>>>(t->et, t->eb, t->tw, t->N2, t->half, t->M2, t->nkb, pl->nlon);
@@ -101,7 +105,7 @@ int dft_plan_init(Plan* pl) {
     if (e == cudaSuccess) e = cudaStreamSynchronize(0);
   }
   if (e != cudaSuccess) {
-    cudaFree(t->et); cudaFree(t->eb); cudaFree(t->tw); cudaFree(t->zeros); cudaFree(t->trash);
+    cudaFree(t->et); cudaFree(t->eb); cudaFree(t->tw); cudaFree(t->zeros);
     delete t;
     return -1;
   }
@@ -112,7 +116,7 @@ int dft_plan_init(Plan* pl) {
 void dft_plan_destroy(Plan* pl) {
   DftTables* t = static_cast<DftTables*>(pl->dft_state);
   if (!t) return;
-  cudaFree(t->et); cudaFree(t->eb); cudaFree(t->tw); cudaFree(t->zeros); cudaFree(t->trash);
+  cudaFree(t->et); cudaFree(t->eb); cudaFree(t->tw); cudaFree(t->zeros);
   delete t;
   pl->dft_state = nullptr;
 }
@@ -155,6 +159,42 @@ __device__ __forceinline__ void prof_wait(unsigned long long* prof, int slot, ui
   const long long t0 = clock64();
   mbar_wait(bar, parity);
   if (lead) atomicAdd(prof + slot, (unsigned long long)(clock64() - t0));
+}
+
+// bulk tensor stores from shared memory (one bulk async-group per output tile, issued and waited for by one thread)
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, uint32_t src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(tm), "r"(src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// 3-D view (nlon, nlat, rows) of the synthesis output, box (ow, 8, 1), no swizzle
+static int make_tmap_out(CUtensorMap* tm, void* base, bool bf16, int nlon, int nlat, long long rows, int ow) {
+  TmapKey key;
+  memset(&key, 0, sizeof(key));
+  key.base = base; key.rank = 3; key.kind = bf16 ? 7 : 6;
+  key.dims[0] = nlon; key.dims[1] = nlat; key.dims[2] = rows; key.box[0] = ow;
+  int slot = 0;
+  if (tmap_lookup(key, tm, &slot)) return 0;
+  PFN_encodeTiled enc = get_encode();
+  if (!enc) { set_error("cuTensorMapEncodeTiled is unavailable"); return B200SHT_ERR_UNSUPPORTED; }
+  static thread_local bool ctx_bound = false;
+  if (!ctx_bound) { cudaFree(nullptr); ctx_bound = true; }
+  const int es = bf16 ? 2 : 4;
+  cuuint64_t gd[3] = {(cuuint64_t)nlon, (cuuint64_t)nlat, (cuuint64_t)rows};
+  cuuint64_t gst[2] = {(cuuint64_t)nlon * es, (cuuint64_t)nlon * nlat * es};
+  cuuint32_t bx[3] = {(cuuint32_t)ow, 8, 1}, el[3] = {1, 1, 1};
+  if (gst[0] % 16 != 0 || (reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ow * es) % 16 != 0) {
+    set_error("tensor map (output): base / row pitch / box row not 16-byte aligned");
+    return B200SHT_ERR_INVALID;
+  }
+  CUresult r = enc(tm, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, base, gd, gst, bx, el,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (output) failed (%d)", (int)r); return B200SHT_ERR_CUDA; }
+  tmap_store(key, tm, slot);
+  return 0;
 }
 
 template <typename T> __device__ __forceinline__ void st_out(T* p, float v);
@@ -211,22 +251,32 @@ template <> __device__ __forceinline__ float ld_in<__nv_bfloat16>(const __nv_bfl
 struct DftSynParams {
   alignas(64) CUtensorMap tmZ;   // tiled latspec as ((c % 4, k % 8), c / 4, m2, p, tile), box (32, 1, 32, 1, 1): MN-major B operand, N = (c, k)
   alignas(64) CUtensorMap tmE;   // E^T tiles (m2, 256 rows), box (32, 128): K-major A operand
+  alignas(64) CUtensorMap tmY;   // the output as (nlon, nlat, R), box (ow, 8, 1), no swizzle: TMA clips the rows k >= nlat of an image's last tile
   const float* Z;
-  void* y;
   const float2* tw;
   const float* rowscale;
   const float* bias;
-  void* trash;
   unsigned long long* prof;
-  int R, C, nlat, nlon, kp, mmax, N2, half, M2, mode, ntiles, ktiles, has_nyq;
+  int R, C, nlat, nlon, kp, mmax, N2, half, M2, mode, ntiles, ktiles, has_nyq, ow;
   int kt0, kt_all;   // latitude range of this launch: first 8-row tile, tiles per image in the whole tensor (ktiles = tiles per image in the range)
 };
 
-// shared memory: [A: cos 16 KB | sin 16 KB][B ring: kDftSynStages x 16 KB][tw table 8 x N2 float2][barriers]
-// warps 0..6: MMA + epilogue, in groups of `nmt` warps (one per 16 columns j2 <= N2 / 2); group i takes the tiles i, i + ngroups, ... of this
-// CTA.  Warp 7: TMA.  The m16n8 accumulator fragment of a warp holds, per thread, the columns j2 = 16 mt + lane / 4 (+ 8) and the latitude pair
-// 2 (lane % 4), + 1 for all eight classes: exactly the inputs of the radix-8 epilogue of those two columns.
-template <typename T, int N2T>
+// shared memory: [A: 16 blocks x (cos 8 rows | sin 8 rows), 32 KB][B ring: kDftSynStages x 16 KB][output: 2 x 8 rows x nlon]
+//                [tw table 8 x N2 float2][barriers]
+// warps 0 .. kDftSynWorkers - 1: MMA + epilogue; then the TMA load warp and the TMA store warp.  The work of a tile is split into `nblk` tasks, one per 8 columns j2 <= N2 / 2,
+// and the tasks (tile n, block b) of this CTA are dealt round-robin over `nwork` worker warps (task n * nblk + b), so each SM sub-partition
+// holds several tasks in flight: the epilogue of one overlaps the MMAs of another.  nwork <= 2 nblk bounds the lead of a warp: consecutive
+// tasks of a warp are at most two tiles apart, so when a warp reaches tile m, its previous task has seen tile m - 4 loaded (full) and
+// stored (ofree).  Every mbarrier wait is then for the next phase of its barrier and never for one two phases away, which the parity test
+// cannot tell apart.  All kDftSynWorkers warps work when nblk >= 5 (N2 >= 72).  The A tile of block b
+// stacks the cos and sin rows of its 8 columns, so the m16n8 accumulator fragment holds, per thread, S1 / S3 (B = Zr) and S4 / S2 (B = Zi) of
+// the column j2 = 8 b + lane / 4 and the latitude pair 2 (lane % 4), + 1 for all eight classes: exactly the inputs of the radix-8 epilogue of
+// j2 and N2 - j2, in 64 accumulator registers.
+// Output: the epilogues write the finished values of tile n into the shared-memory tile n % 2, laid out as the TMA boxes of ow columns
+// x 8 rows; when all nblk tasks of the tile have arrived on staged[n % 2], the store warp writes it with bulk tensor stores (whole 128-byte
+// lines instead of 16-byte pieces of four rows per store instruction) and frees the buffer once the stores have read it.
+// N2 is a run-time value here: the compile-time instantiations spilled at the 168-register cap, this one does not.
+template <typename T>
 __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const __grid_constant__ DftSynParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ unsigned long long prof_s[16];   // wait-time profile (B200SHT_DFT_PROF): accumulated per CTA, flushed once at the end
@@ -235,27 +285,34 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* gbase = smem_raw + (base - raw);
-  const uint32_t sA = base, sB = base + 32768;
-  float2* tws = reinterpret_cast<float2*>(gbase + 32768 + kDftSynStages * 16384);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(gbase + 32768 + kDftSynStages * 16384 + ((8 * p.N2 * 8 + 15) & ~15));
+  const int N2 = p.N2;
+  const int nlon = 8 * N2;
+  const int ow = p.ow;
+  const uint32_t obytes = (8u * nlon * sizeof(T) + 1023u) & ~1023u;   // one output tile
+  const uint32_t sA = base, sB = base + 32768, sO = sB + kDftSynStages * 16384;
+  T* const outS = reinterpret_cast<T*>(gbase + (sO - base));
+  float2* tws = reinterpret_cast<float2*>(gbase + (sO - base) + 2 * obytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(tws) + ((8 * N2 * 8 + 15) & ~15));
   uint64_t* full = bars;
   uint64_t* empty = full + kDftSynStages;
   uint64_t* e_full = empty + kDftSynStages;
+  uint64_t* staged = e_full + 1;   // [2] output tile written by all its tasks
+  uint64_t* ofree = staged + 2;    // [2] output tile read by its bulk stores
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
   pdl_trigger();
-  const int nmt = (p.half + 16) / 16;          // 16-column blocks of j2 = 0 .. N2 / 2
-  const int ngroups = kDftSynWorkers / nmt;
-  const bool is_tma = (warp == kDftSynWorkers);
-  const int grp = warp / nmt, mt = warp - grp * nmt;
-  const bool is_work = !is_tma && grp < ngroups;
+  const int nblk = (p.half + 8) / 8;          // 8-column blocks of j2 = 0 .. N2 / 2
+  const int nwork = kDftSynWorkers < 2 * nblk ? kDftSynWorkers : 2 * nblk;   // see above
+  const bool is_tma = (warp == kDftSynWorkers), is_store = (warp == kDftSynWorkers + 1);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kDftSynStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], nmt); }
+    for (int s = 0; s < kDftSynStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], nblk); }
     mbar_init(e_full, 1);
+    for (int b = 0; b < 2; ++b) { mbar_init(&staged[b], 32 * nblk); mbar_init(&ofree[b], 1); }
     fence_barrier_init();
     prefetch_tmap(&p.tmZ);
     prefetch_tmap(&p.tmE);
+    prefetch_tmap(&p.tmY);
   }
   for (int i = threadIdx.x; i < 8 * p.N2; i += blockDim.x) tws[i] = p.tw[i];
   __syncthreads();
@@ -281,19 +338,33 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
       }
     }
     __syncwarp();
-  } else if (is_work) {
-    const int N2 = N2T > 0 ? N2T : p.N2;
-    const int nlon = 8 * N2;
+  } else if (is_store) {
+    if (lane == 0) {
+      int n = 0;
+      for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
+        const int b = n & 1;
+        prof_wait(prof, 11, &staged[b], (n >> 1) & 1, true);
+        const int r = ti / p.ktiles, k0 = (p.kt0 + ti - r * p.ktiles) * 8;
+        if (k0 < p.nlat)   // tiles of the padding rows kp > nlat: nothing to store (rows k >= nlat of a partial tile are clipped by TMA)
+          for (int bx = 0; bx * ow < nlon; ++bx) tma_store_3d(&p.tmY, sO + b * obytes + bx * 8 * ow * (uint32_t)sizeof(T), bx * ow, k0, r);
+        bulk_commit();
+        bulk_wait_read0();
+        mbar_arrive(&ofree[b]);
+      }
+      bulk_wait0();
+    }
+    __syncwarp();
+  } else {
     const int kpi = lane & 3;
     const bool n2odd = (N2 & 1) != 0;
-    T* const y = static_cast<T*>(p.y);
     const float smul = p.mode == 0 ? 2.f : 1.f;
     const int nyq_m = nlon / 2;
-    T* const trash = static_cast<T*>(p.trash) + (size_t)(blockIdx.x & 63) * (4 * nlon + 256);
     const uint8_t* const gE = gbase;
     mbar_wait(e_full, 0);
-    int n = grp;
-    for (int ti = blockIdx.x + grp * gridDim.x; ti < p.ntiles; ti += ngroups * gridDim.x, n += ngroups) {
+    for (int task = warp; warp < nwork; task += nwork) {
+      const int n = task / nblk, blk = task - n * nblk;   // tile n of this CTA, 8-column block blk
+      const int ti = blockIdx.x + n * gridDim.x;
+      if (ti >= p.ntiles) break;
       const int r = ti / p.ktiles, k0 = (p.kt0 + ti - r * p.ktiles) * 8;
       const int ta = r * p.kt_all + p.kt0 + (ti - r * p.ktiles);   // tile index in the whole tensor
       const int ka = k0 + 2 * kpi;
@@ -319,36 +390,33 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
       const pr off_o = make_pr(bias - rsa * (z0a - zna), bias - rsb * (z0b - znb));   // odd longitude j
       prof_wait(prof, 9, &full[s], it & 1, lane == 0);
       if (prof && lane == 0) atomicAdd(prof + 13, 1ull);
-      // S1 = cos . Zr, S2 = sin . Zi, S3 = sin . Zr, S4 = cos . Zi over the 32 orders m2 of the tile; rows j2, columns (class c, latitude)
-      float acc[4][8][4];
+      // rows of the A tile blk: cos then sin of the columns j2 = 8 blk + lane / 4, so the accumulator elements 0, 1 / 2, 3 of
+      // acc[0] are S1 = cos . Zr / S3 = sin . Zr, of acc[1] S4 = cos . Zi / S2 = sin . Zi (32 orders m2; columns (class c, latitude))
+      float acc[2][8][4];
 #pragma unroll
-      for (int a = 0; a < 4; ++a)
+      for (int a = 0; a < 2; ++a)
 #pragma unroll
         for (int c = 0; c < 8; ++c) acc[a][c][0] = acc[a][c][1] = acc[a][c][2] = acc[a][c][3] = 0.f;
       {
         const uint8_t* const zs = gbase + 32768 + (size_t)s * 16384;
 #pragma unroll
         for (int kk = 0; kk < 32; kk += 8) {
-          uint32_t fc[4], fs[4];
-          frag_a<false>(gE, 16 * mt, kk, fc);
-          frag_a<false>(gE + 16384, 16 * mt, kk, fs);
+          uint32_t fa[4];
+          frag_a<false>(gE, 16 * blk, kk, fa);
 #pragma unroll
           for (int c = 0; c < 8; ++c) {
             uint32_t zr[2], zi[2];
             frag_b<true>(zs, 8 * c, kk, zr);
             frag_b<true>(zs + 8192, 8 * c, kk, zi);
-            mma_tf32(acc[0][c], fc, zr);
-            mma_tf32(acc[1][c], fs, zi);
-            mma_tf32(acc[2][c], fs, zr);
-            mma_tf32(acc[3][c], fc, zi);
+            mma_tf32(acc[0][c], fa, zr);
+            mma_tf32(acc[1][c], fa, zi);
           }
         }
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[s]);   // this warp's reads of the stage are done
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int j2 = 16 * mt + (lane >> 2) + 8 * h;
+      {
+        const int j2 = 8 * blk + (lane >> 2);
         const bool valid = j2 <= p.half;
         const bool paired = valid && j2 != 0 && 2 * j2 != N2;
         const int jp = N2 - j2;
@@ -357,44 +425,43 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
 #pragma unroll
         for (int c = 1; c < 8; ++c) tw[c] = valid ? tws[c * N2 + j2] : make_float2(1.f, 0.f);
         dft_partner_twiddles(tw, tp);
-        // rows beyond nlat (last tile of an image) are stored into a scratch row: no predicates / branches around the 32 stores
-        T* const pa = (valid && ka < p.nlat) ? y + ((size_t)r * p.nlat + ka) * nlon + j2 : trash + j2;
-        T* const pb = (valid && ka + 1 < p.nlat) ? y + ((size_t)r * p.nlat + ka + 1) * nlon + j2 : trash + nlon + j2;
-        const int dq = paired ? jp - j2 : 0;
+        // output tile element (row kr, longitude j) at ((j / ow) * 8 + kr) * ow + j % ow
+        T* const ob = outS + (size_t)(n & 1) * (obytes / sizeof(T)) + 2 * kpi * ow;
+        if (n >= 2) prof_wait(prof, 10, &ofree[n & 1], ((n >> 1) - 1) & 1, lane == 0);
         {
           pr vr[8], vi[8], x[8];
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            vr[c] = make_pr(acc[0][c][2 * h], acc[0][c][2 * h + 1]) - make_pr(acc[1][c][2 * h], acc[1][c][2 * h + 1]);
-            vi[c] = make_pr(acc[2][c][2 * h], acc[2][c][2 * h + 1]) + make_pr(acc[3][c][2 * h], acc[3][c][2 * h + 1]);
+          for (int c = 0; c < 8; ++c) {   // V(j2) = (S1 - S2, S3 + S4)
+            vr[c] = make_pr(acc[0][c][0], acc[0][c][1]) - make_pr(acc[1][c][2], acc[1][c][3]);
+            vi[c] = make_pr(acc[0][c][2], acc[0][c][3]) + make_pr(acc[1][c][0], acc[1][c][1]);
           }
           dft_syn_radix8<pr>(vr, vi, tw, x);
           const pr o0 = (j2 & 1) ? off_o : off_e, o1 = (j2 & 1) ? off_e : off_o;
 #pragma unroll
-          for (int j1 = 0; j1 < 8; ++j1) {
+          for (int j1 = 0, bx = j2 / ow, jx = j2 - bx * ow; j1 < 8; ++j1) {   // longitude N2 j1 + j2 = bx ow + jx
             const pr o = rfma(x[j1], sc, (n2odd && (j1 & 1)) ? o1 : o0);
-            st_out<T>(pa + N2 * j1, o.v.x);
-            st_out<T>(pb + N2 * j1, o.v.y);
+            if (valid) { st_out<T>(ob + bx * 8 * ow + jx, o.v.x); st_out<T>(ob + bx * 8 * ow + jx + ow, o.v.y); }
+            for (jx += N2; jx >= ow; jx -= ow) ++bx;
           }
         }
         {
           pr vr[8], vi[8], x[8];
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            vr[c] = make_pr(acc[0][c][2 * h], acc[0][c][2 * h + 1]) + make_pr(acc[1][c][2 * h], acc[1][c][2 * h + 1]);
-            vi[c] = make_pr(acc[3][c][2 * h], acc[3][c][2 * h + 1]) - make_pr(acc[2][c][2 * h], acc[2][c][2 * h + 1]);
+          for (int c = 0; c < 8; ++c) {   // V(N2 - j2) = (S1 + S2, S4 - S3)
+            vr[c] = make_pr(acc[0][c][0], acc[0][c][1]) + make_pr(acc[1][c][2], acc[1][c][3]);
+            vi[c] = make_pr(acc[1][c][0], acc[1][c][1]) - make_pr(acc[0][c][2], acc[0][c][3]);
           }
           dft_syn_radix8<pr>(vr, vi, tp, x);
-          T* const qa = paired ? pa + dq : trash + 2 * nlon + j2;     // unpaired columns (j2 = 0, N2 / 2) and idle rows: scratch
-          T* const qb = paired ? pb + dq : trash + 3 * nlon + j2;
           const pr o0 = (jp & 1) ? off_o : off_e, o1 = (jp & 1) ? off_e : off_o;
 #pragma unroll
-          for (int j1 = 0; j1 < 8; ++j1) {
+          for (int j1 = 0, bx = jp / ow, jx = jp - bx * ow; j1 < 8; ++j1) {   // not for the unpaired columns 0 and N2 / 2
             const pr o = rfma(x[j1], sc, (n2odd && (j1 & 1)) ? o1 : o0);
-            st_out<T>(qa + N2 * j1, o.v.x);
-            st_out<T>(qb + N2 * j1, o.v.y);
+            if (paired) { st_out<T>(ob + bx * 8 * ow + jx, o.v.x); st_out<T>(ob + bx * 8 * ow + jx + ow, o.v.y); }
+            for (jx += N2; jx >= ow; jx -= ow) ++bx;
           }
         }
+        fence_proxy_async();   // the bulk stores read the tile through the async proxy: every writing thread fences and arrives
+        mbar_arrive(&staged[n & 1]);
       }
     }
   }
@@ -411,7 +478,7 @@ int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int
   const int R = B * C;
   DftSynParams p;
   memset(&p, 0, sizeof(p));
-  p.Z = Z; p.y = y; p.tw = t->tw; p.rowscale = pl->d_rowscale; p.bias = bias; p.trash = t->trash; p.prof = dft_prof_buffer();
+  p.Z = Z; p.tw = t->tw; p.rowscale = pl->d_rowscale; p.bias = bias; p.prof = dft_prof_buffer();
   p.R = R; p.C = C; p.nlat = pl->nlat; p.nlon = pl->nlon; p.kp = pl->kp; p.mmax = pl->mmax;
   p.N2 = t->N2; p.half = t->half; p.mode = mode;
   if (k_end < 0 || k_end > pl->kp) k_end = pl->kp;
@@ -434,24 +501,24 @@ int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int
     int rc = make_tmap(&p.tmE, t->et, 2, d, s, bx);
     if (rc) return rc;
   }
-  const size_t smem = 1024 + 32768 + (size_t)kDftSynStages * 16384 + ((8 * (size_t)t->N2 * 8 + 15) & ~(size_t)15) + (2 * kDftSynStages + 1) * 8;
+  const bool bf16 = (dtype == B200SHT_BF16);
+  p.ow = dft_out_box(t->N2);
+  {
+    int rc = make_tmap_out(&p.tmY, y, bf16, pl->nlon, pl->nlat, R, p.ow);
+    if (rc) return rc;
+  }
+  const size_t obytes = (8 * (size_t)pl->nlon * (bf16 ? 2 : 4) + 1023) & ~(size_t)1023;
+  const size_t smem = 1024 + 32768 + (size_t)kDftSynStages * 16384 + 2 * obytes + ((8 * (size_t)t->N2 * 8 + 15) & ~(size_t)15) +
+                      (2 * kDftSynStages + 5) * 8;
   const int sms = usable_sms(pl->sm_count > 0 ? pl->sm_count : 132);
   const int ctas = p.ntiles < sms ? p.ntiles : sms;
-#define B200_LAUNCH_SYN(TT, NN)                                                                                                          \
-  do {                                                                                                                                  \
-    struct Tag {};                                                                                                                        \
-    B200_CHECK_CUDA((ensure_dynamic_smem<Tag>(dft_synthesis_kernel<TT, NN>, smem)));                                                     \
-    B200_CHECK_CUDA(launch_pdl(dft_synthesis_kernel<TT, NN>, dim3(ctas), dim3(kDftSynThreads), smem, st, p));                                                                 \
+#define B200_LAUNCH_SYN(TT)                                                                                          \
+  do {                                                                                                                \
+    struct Tag {};                                                                                                    \
+    B200_CHECK_CUDA((ensure_dynamic_smem<Tag>(dft_synthesis_kernel<TT>, smem)));                                     \
+    B200_CHECK_CUDA(launch_pdl(dft_synthesis_kernel<TT>, dim3(ctas), dim3(kDftSynThreads), smem, st, p));            \
   } while (0)
-#define B200_DISPATCH_SYN(TT)                                            \
-  switch (t->N2) {                                                       \
-    case 180: B200_LAUNCH_SYN(TT, 180); break; /* nlon 1440 */           \
-    case 90: B200_LAUNCH_SYN(TT, 90); break;   /* nlon  720 */           \
-    case 60: B200_LAUNCH_SYN(TT, 60); break;   /* nlon  480 */           \
-    default: B200_LAUNCH_SYN(TT, 0); break;                              \
-  }
-  if (dtype == B200SHT_BF16) { B200_DISPATCH_SYN(__nv_bfloat16) } else { B200_DISPATCH_SYN(float) }
-#undef B200_DISPATCH_SYN
+  if (bf16) { B200_LAUNCH_SYN(__nv_bfloat16); } else { B200_LAUNCH_SYN(float); }
 #undef B200_LAUNCH_SYN
   B200_CHECK_LAUNCH();
   return 0;
@@ -488,6 +555,7 @@ static int make_tmap_segments(CUtensorMap* tm, const void* base, bool bf16, int 
 }
 
 constexpr int kDftAnaStages = 2;   // operand ring: one stage = one K-block (32 columns) of a 16-row tile = 4 planes x 16 KB
+constexpr int kDftAnaMma = 8, kDftAnaLoader = 8, kDftAnaProd0 = 9, kDftAnaThreads = 512;   // warp roles (below)
 
 struct DftAnaParams {
   alignas(64) CUtensorMap tmB;   // E tiles (32 j2 local, nkb * 64 rows), box (32, 32): K-major B operand
@@ -501,17 +569,20 @@ struct DftAnaParams {
   int kt0;   // first 16-row tile of the latitude range this launch transforms (ktiles = tiles in the range; latitude-chunked analysis, capi.cu)
 };
 
-// warps: 0..3 MMA + epilogue (rows 32 w .. + 31 of the tile = classes 2 w, 2 w + 1), 4 loads the resident B, 5 sample loader (TMA), 6.. producers
+// warps: 0..7 MMA + epilogue (rows 16 w .. + 15 of the tile = class w), 8 loader (TMA: the resident B, then the samples), 9..15 producers.
+// 16 warps = 4 per SM sub-partition, so every warp gets 128 registers: no spills.  The MMA warps were the bottleneck with four warps of two
+// classes each (the producers waited for a free operand stage 63 % of the time); one class per warp halves their serial MMA + epilogue work
+// per tile and gives each sub-partition two of them.
 // shared memory: [B resident: nkb x (cos 4 KB | sin 4 KB)][A ring: 2 x 4 planes x 16 KB][raw ring: nraw x 16 boxes][twiddles][barriers]
 //
 // Data flow of one (tile, K-block): the loader thread brings the 8 + 8 sample boxes the K-block needs -- for each j1 the 32 columns
 // j2 = 32 kb .. + 31 and their 32 partner columns N2 - j2, 16 rows each -- into a raw stage with 16 TMA boxes (deep asynchronous prefetch,
 // no registers: the first version's LDG -> register path stalled 2.1 cycles per issued instruction on the loads, with the 96-register cap
-// allowing only half an item of prefetch).  Eight producer warps (one row pair each) read their samples with LDS, run the two radix-8
+// allowing only half an item of prefetch).  The producer warps (one row pair per item) read their samples with LDS, run the two radix-8
 // butterflies + twiddles on the two rows of a pair, and write Ye / Yo of the 8 classes into the operand stage; then the MMA warps contract
 // the stage with E.  N2T > 0: nlon / 8 as a compile-time constant.
 template <typename T, int N2T>
-__global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_constant__ DftAnaParams p) {
+__global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const __grid_constant__ DftAnaParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ unsigned long long prof_s[16];   // wait-time profile (B200SHT_DFT_PROF): accumulated per CTA, flushed once at the end
   unsigned long long* const prof = (kDftProfile && p.prof) ? prof_s : nullptr;
@@ -554,7 +625,7 @@ __global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_const
     twS[i] = w;
   }
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kDftAnaStages; ++s) { mbar_init(&full[s], 8); mbar_init(&empty[s], 4); }   // a K-block = 8 row pairs; 4 MMA warps
+    for (int s = 0; s < kDftAnaStages; ++s) { mbar_init(&full[s], 8); mbar_init(&empty[s], kDftAnaMma); }   // a K-block = 8 row pairs
     for (int s = 0; s < p.nraw; ++s) { mbar_init(&raw_full[s], 1); mbar_init(&raw_empty[s], 8); }
     mbar_init(b_full, 1);
     fence_barrier_init();
@@ -571,18 +642,14 @@ __global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_const
   const long long t_cta0 = (kDftProfile && p.prof && threadIdx.x == 0) ? clock64() : 0;
   pdl_wait();   // the prologue read plan constants only (twiddles); samples and latspec belong to other kernels until here
 
-  if (warp == 4) {
+  if (warp == kDftAnaLoader) {
+    // ------------------------------------------------------------------------------------- resident B, then the samples
     if (lane == 0) {
       mbar_expect_tx(b_full, (uint32_t)nkb * 8192);
       for (int kb = 0; kb < nkb; ++kb) {
         tma_load_2d(sBm + kb * 8192, &p.tmB, b_full, 0, kb * 64);
         tma_load_2d(sBm + kb * 8192 + 4096, &p.tmB, b_full, 0, kb * 64 + 32);
       }
-    }
-    __syncwarp();
-  } else if (warp == 5) {
-    // ------------------------------------------------------------------------------------- sample loader
-    if (lane == 0) {
       int n = 0;
       for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
         const int r = ti / p.ktiles, row0 = r * p.nlat + (p.kt0 + ti - r * p.ktiles) * 16;
@@ -603,49 +670,60 @@ __global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_const
       }
     }
     __syncwarp();
-  } else if (warp < 4) {
+  } else if (warp < kDftAnaMma) {
     // ------------------------------------------------------------------------------------------- MMA + epilogue
-    // D[(c, kr)][m2] = Xre: Ye_r cos + Yo_i sin,  Xim: Ye_i cos - Yo_r sin over the j2 of all K-blocks.  m16 tile mt of this warp is class
-    // c = 2 warp + mt, its fragment rows are the latitudes kr = lane / 4 (+ 8), its columns the orders m2 = 8 j + 2 (lane % 4) (+ 1).
+    // D[(c, kr)][m2] = Xre: Ye_r cos + Yo_i sin,  Xim: Ye_i cos - Yo_r sin over the j2 of all K-blocks.  The m16 tile of this warp is class
+    // c = warp, its fragment rows are the latitudes kr = lane / 4 (+ 8), its columns the orders m2 = 8 j + 2 (lane % 4) (+ 1).
+    // K order: the sum over j2 is order-free, so within a K-block the thread of q = lane % 4 takes the columns 8 q .. 8 q + 7 -- two
+    // 16-byte loads per operand row, conflict-free under the 128-byte swizzle -- and step t of the four m16n8k8 steps contracts the columns
+    // 8 q + 2 t (fragment column q) and 8 q + 2 t + 1 (fragment column q + 4) of both operands.
     const size_t plane = (size_t)p.R * p.kp;
     const float tcomp = p.round_tf32 ? kTruncComp : 1.f;
+    const int c = warp, gq = lane >> 2, q = lane & 3;
     mbar_wait(b_full, 0);
     int n = 0;
     for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
       const int r = ti / p.ktiles, k0 = (p.kt0 + ti - r * p.ktiles) * 16;
-      float xr[2][4][4], xi[2][4][4];
+      float xr[4][4], xi[4][4];
 #pragma unroll
-      for (int mt = 0; mt < 2; ++mt)
+      for (int j = 0; j < 4; ++j)
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) { xr[mt][j][e] = 0.f; xi[mt][j][e] = 0.f; }
+        for (int e = 0; e < 4; ++e) { xr[j][e] = 0.f; xi[j][e] = 0.f; }
       for (int kb = 0; kb < nkb; ++kb) {
         const int g = n * nkb + kb, s = g % kDftAnaStages, it = g / kDftAnaStages;
         prof_wait(prof, 3, &full[s], it & 1, lane == 0);
         const uint8_t* const a0 = gA + (size_t)s * 65536;
         const uint8_t* const bc = gbase + oB + kb * 8192;
-        const uint8_t* const bs = bc + 4096;
 #pragma unroll
-        for (int kk = 0; kk < 32; kk += 8) {
-          uint32_t fc[4][2], fs[4][2];
+        for (int half = 0; half < 2; ++half) {   // columns 8 q + 4 half .. + 3: steps t = 2 half, 2 half + 1
+          const uint32_t col = 32 * q + 16 * half;
+          uint4 av[4][2];   // [plane][row g, g + 8]
 #pragma unroll
-          for (int j = 0; j < 4; ++j) { frag_b<false>(bc, 8 * j, kk, fc[j]); frag_b<false>(bs, 8 * j, kk, fs[j]); }
+          for (int pl = 0; pl < 4; ++pl)
 #pragma unroll
-          for (int mt = 0; mt < 2; ++mt) {
-            const int row0 = 32 * warp + 16 * mt;
-            uint32_t er[4], ei[4], orr[4], oi[4];
-            frag_a<false>(a0, row0, kk, er);
-            frag_a<false>(a0 + 16384, row0, kk, ei);
-            frag_a<false>(a0 + 32768, row0, kk, orr);
-            frag_a<false>(a0 + 49152, row0, kk, oi);
-            frag_neg(orr, orr);
+            for (int h = 0; h < 2; ++h) av[pl][h] = lds128(a0 + pl * 16384, (16 * c + gq + 8 * h) * 128 + col);
+          // cos: Xre += Ye_r cos, Xim += Ye_i cos;  sin: Xre += Yo_i sin, Xim -= Yo_r sin.  Consecutive MMAs into the same accumulator are
+          // eight apart, so the dependent ones do not issue back to back.
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              mma_tf32(xr[mt][j], er, fc[j]);
-              mma_tf32(xr[mt][j], oi, fs[j]);
-              mma_tf32(xi[mt][j], ei, fc[j]);
-              mma_tf32(xi[mt][j], orr, fs[j]);
+          for (int cs = 0; cs < 2; ++cs) {
+            uint4 bv[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) bv[j] = lds128(bc + cs * 4096, (8 * j + gq) * 128 + col);
+            const int pr_ = cs ? 3 : 0, pi_ = cs ? 2 : 1;
+#pragma unroll
+            for (int t = 0; t < 2; ++t) {
+              uint32_t far_[4], fai[4];
+              far_[0] = t ? av[pr_][0].z : av[pr_][0].x; far_[1] = t ? av[pr_][1].z : av[pr_][1].x;
+              far_[2] = t ? av[pr_][0].w : av[pr_][0].y; far_[3] = t ? av[pr_][1].w : av[pr_][1].y;
+              fai[0] = t ? av[pi_][0].z : av[pi_][0].x; fai[1] = t ? av[pi_][1].z : av[pi_][1].x;
+              fai[2] = t ? av[pi_][0].w : av[pi_][0].y; fai[3] = t ? av[pi_][1].w : av[pi_][1].y;
+              if (cs) frag_neg(fai, fai);   // - Yo_r
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const uint32_t fb[2] = {t ? bv[j].z : bv[j].x, t ? bv[j].w : bv[j].y};
+                mma_tf32(xr[j], far_, fb);
+                mma_tf32(xi[j], fai, fb);
+              }
             }
           }
         }
@@ -654,46 +732,42 @@ __global__ void __launch_bounds__(576, 1) dft_analysis_kernel(const __grid_const
       }
       if (prof && lane == 0) atomicAdd(prof + 5, 1ull);
 #pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        const int c = 2 * warp + mt;
+      for (int h = 0; h < 2; ++h) {
+        const int k = k0 + gq + 8 * h;
+        if (k >= p.kp) continue;
+        const float rs = (p.mode == 0) ? ((k < p.nlat) ? __ldg(p.rowscale + k) : 0.f) : 1.f;
+        float* xb = p.X + (size_t)r * p.kp + k;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int k = k0 + (lane >> 2) + 8 * h;
-          if (k >= p.kp) continue;
-          const float rs = (p.mode == 0) ? ((k < p.nlat) ? __ldg(p.rowscale + k) : 0.f) : 1.f;
-          float* xb = p.X + (size_t)r * p.kp + k;
+        for (int j = 0; j < 4; ++j)
 #pragma unroll
-          for (int j = 0; j < 4; ++j)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int m = c + 8 * (8 * j + 2 * (lane & 3) + e);
-              if (m >= p.mmax) continue;
-              // round_tf32: the consumer is the TF32 Legendre GEMM, which truncates its operands -> bias-compensated truncation folded
-              // into the scale factor (see B200_DFT_TF32_MODE above) instead of 3 instructions of cvt.rna per value
-              const float sc = ((p.mode == 0) ? rs : ((m == 0 || 2 * m == p.nlon) ? 1.f : 2.f)) * tcomp;
-              float* dst = xb + (size_t)m * 2 * plane;
-              dst[0] = xr[mt][j][2 * h + e] * sc;
-              dst[plane] = xi[mt][j][2 * h + e] * sc;
-            }
-        }
+          for (int e = 0; e < 2; ++e) {
+            const int m = c + 8 * (8 * j + 2 * q + e);
+            if (m >= p.mmax) continue;
+            // round_tf32: the consumer is the TF32 Legendre GEMM, which truncates its operands -> bias-compensated truncation folded
+            // into the scale factor (see B200_DFT_TF32_MODE above) instead of 3 instructions of cvt.rna per value
+            const float sc = ((p.mode == 0) ? rs : ((m == 0 || 2 * m == p.nlon) ? 1.f : 2.f)) * tcomp;
+            float* dst = xb + (size_t)m * 2 * plane;
+            dst[0] = xr[j][2 * h + e] * sc;
+            dst[plane] = xi[j][2 * h + e] * sc;
+          }
       }
     }
   } else {
     // ------------------------------------------------------------------------------------------- producers
     // Work item = (K-block kb, row pair q): rows 2q, 2q + 1 of the tile in the halves of register pairs (pr), lanes = the 32 columns of the
     // K-block.  Items are taken in K-block-major order (item = kb * 8 + q; warp w does w, w + nprod, ...): the MMAs of K-block kb run while
-    // the warps work on kb + 1.  12 producer warps for three K-blocks (2 items per warp and tile), 8 otherwise: the kernel is bound by the
-    // latency of the dependent butterfly chains, so the tile time is (items per warp) x (item latency).
-    const int pw = warp - 6;
-    const int nprod = (int)(blockDim.x >> 5) - 6;
-    const int ipw = (8 * nkb) / nprod;
+    // the warps work on kb + 1.  Each warp takes its items in increasing order, so every wait is on an earlier K-block: no cycle.  With
+    // nprod <= 8 every warp has an item in every K-block (8 consecutive items cover all warps), so the raw_full and empty waits of a warp
+    // are for consecutive uses of a stage and never alias a phase two uses old.
+    const int pw = warp - kDftAnaProd0;
+    constexpr int nprod = kDftAnaThreads / 32 - kDftAnaProd0;
+    static_assert(nprod >= 1 && nprod <= 8, "every producer warp must take an item of every K-block (8 items each)");
     constexpr bool kBf16 = (sizeof(T) == 2);
     const T* const rawS = reinterpret_cast<const T*>(gR);
     int n = 0;
     for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
       const int r = ti / p.ktiles, kt16 = (p.kt0 + ti - r * p.ktiles) * 16;
-      for (int ii = 0; ii < ipw; ++ii) {
-        const int item = pw + ii * nprod;
+      for (int item = pw; item < 8 * nkb; item += nprod) {
         const int kb = item >> 3, q = item & 7;
         const int k0 = kt16 + 2 * q;
         const int g = n * nkb + kb;
@@ -815,7 +889,7 @@ int dft_analysis(const Plan* pl, const void* x, int dtype, int B, int C, float* 
   const size_t smem = 1024 + 3 * 8192 + (size_t)kDftAnaStages * 65536 + p.nraw * raw_bytes + 3 * 7 * 32 * 8 + 256;
   const int sms = usable_sms(pl->sm_count > 0 ? pl->sm_count : 132);
   const int ctas = p.ntiles < sms ? p.ntiles : sms;
-  const int threads = 32 * (6 + (t->nkb == 3 ? 12 : 8));
+  const int threads = kDftAnaThreads;
 #define B200_LAUNCH_ANA(TT, NN)                                                                                                          \
   do {                                                                                                                                  \
     struct Tag {};                                                                                                                        \

@@ -35,7 +35,7 @@ ctas = torch.cuda.get_device_properties(0).multi_processor_count   # one persist
 life = a[6] / ctas
 print(f"analysis: CTA lifetime {life:.0f} clk; items {a[7]:.0f}")
 names = ["producers wait samples (per warp)", "producers wait operand stage (per warp)", "loader waits raw stage", "MMA warps wait operand (per warp)"]
-div = [12, 12, 1, 4]
+div = [7, 7, 1, 8]   # warps per role in dft_analysis_kernel: producers, producers, loader, MMA
 for i, nme in enumerate(names):
     print(f"  {nme:45s} {a[i] / ctas / div[i]:10.0f} clk  = {100 * a[i] / ctas / div[i] / life:5.1f}% of the CTA lifetime")
 for _ in range(2):
@@ -44,6 +44,7 @@ read()
 _lib.call("b200sht_fft_synthesis", plan.handle, _ptr(lat), _ptr(y), 1, B, C, _VP(0), 0 | 2, st)
 a = read().astype(float)
 life = a[12] / ctas
-print(f"synthesis: CTA lifetime {life:.0f} clk; epilogue tile visits {a[13]:.0f}")
-for i, nme, d in ((8, "TMA waits stage free", 1), (9, "MMA waits stage full", 1), (10, "MMA waits accumulator free", 1), (11, "epilogue waits accumulator (per warp)", 12)):
+print(f"synthesis: CTA lifetime {life:.0f} clk; tasks (8 columns of a tile) {a[13]:.0f}")
+for i, nme, d in ((8, "TMA load waits stage free", 1), (9, "MMA + epilogue warps wait stage full (per warp)", 10),
+                  (10, "epilogues wait output tile free (per warp)", 10), (11, "TMA store waits output tile written", 1)):
     print(f"  {nme:45s} {a[i] / ctas / d:10.0f} clk  = {100 * a[i] / ctas / d / life:5.1f}% of the CTA lifetime")
