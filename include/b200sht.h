@@ -89,11 +89,14 @@ int b200sht_plan_create(b200sht_plan** plan, int nlat, int nlon, int lmax, int m
 /* Extended creation for the h x w model-parallel (distributed) SHT and for the vector SHT:
  *   m_offset : the plan's orders are m_offset .. m_offset + mmax - 1 (this rank's shard of the orders)
  *   flags & B200SHT_PLAN_FFT_ONLY: no Legendre table: nlat is this rank's latitude count, quad_w its slice of the weights
- *   flags & B200SHT_PLAN_VECTOR:   vector-SHT plan (m_offset 0).  Instead of P it holds, built on the device in fp64 and stored as fp32
+ *   flags & B200SHT_PLAN_VECTOR:   vector-SHT plan.  Instead of P it holds, built on the device in fp64 and stored as fp32
  *                                  [mmax][lmax][kp] each (exact zeros for l < m, zero at l = 0):
  *                                    D[m][l][k] = dP_l^m(cos theta)/dtheta at theta_k,   Q[m][l][k] = m P_l^m(cos theta_k) / sin(theta_k)
  *                                  (P the orthonormal table of the scalar plan, Condon-Shortley phase when csphase).  Only the vector entry
- *                                  points (b200sht_vector_*, b200sht_vsht_*) and the longitude stages accept it. */
+ *                                  points (b200sht_vector_*, b200sht_vsht_*) and the longitude stages accept it.  With m_offset > 0 its
+ *                                  local order m holds the columns of the global order m_offset + m, bit-identical to those of the plan of
+ *                                  all orders: an order shard of the distributed vector transforms, served by the Legendre stages and the
+ *                                  converters only (see the vector SHT section).  B200SHT_PLAN_VECTOR | B200SHT_PLAN_FFT_ONLY is refused. */
 #define B200SHT_PLAN_FFT_ONLY 1
 #define B200SHT_PLAN_VECTOR 2
 int b200sht_plan_create_ex(b200sht_plan** plan, int nlat, int nlon, int lmax, int mmax, int m_offset, int flags,
@@ -181,7 +184,11 @@ int b200sht_sht_inverse_adjoint(const b200sht_plan* plan, const void* gy, int dt
  * Stage formats: the 2C component rows (b, c, component) are read and written in place as the rows of a scalar latspec of 2C channels, and
  * the Legendre stages produce a STACKED spec [2][lmax][mmax][2][B][cp] (cp = 2C rounded up to 4, column 2c + component): the D
  * contractions, then the Q contractions (b200sht_spec_elems(plan, B, 2C) floats).  The +-i rotations and 1/(l(l+1)) happen in the
- * spec <-> coefficient converters.  Precision FP32 or TF32 (3 x TF32 is refused with B200SHT_ERR_UNSUPPORTED). */
+ * spec <-> coefficient converters.  Precision FP32 or TF32 (3 x TF32 is refused with B200SHT_ERR_UNSUPPORTED).
+ * Order shards (a vector plan with m_offset > 0, the distributed vector transforms): b200sht_vector_legendre_analysis / _synthesis and
+ * b200sht_vector_spec_pack / _unpack serve them, with mmax the shard's order count and "l < m" read as l < m_offset + m; their outputs are
+ * the order slice of the plan of all orders.  b200sht_vector_legendre_synthesis_tiled and the one-call b200sht_vsht_* entries return
+ * B200SHT_ERR_INVALID on them (b200sht_vsht_workspace_bytes returns -1): their longitude stage covers orders 0 .. mmax - 1. */
 int b200sht_vector_legendre_analysis(const b200sht_plan* plan, const float* latspec, float* spec, int B, int C, int precision, void* stream);
 int b200sht_vector_legendre_synthesis(const b200sht_plan* plan, const float* spec, float* latspec, int B, int C, int precision, void* stream);
 /* TF32 into the tiled latspec layout of the tensor-core DFT (see b200sht_legendre_synthesis_tiled); needs b200sht_plan_query(plan, 8) == 1 */
@@ -191,7 +198,7 @@ int b200sht_vector_legendre_synthesis_tiled(const b200sht_plan* plan, const floa
  * pack(scaled) is the adjoint of unpack(scaled).  pack writes every entry of the stacked spec. */
 int b200sht_vector_spec_unpack(const b200sht_plan* plan, const float* spec, void* coeffs, int B, int C, int scaled, void* stream);
 int b200sht_vector_spec_pack(const b200sht_plan* plan, const void* coeffs, float* spec, int B, int C, int scaled, void* stream);
-/* One-call boundary, as b200sht_sht_* (workspace of b200sht_vsht_workspace_bytes; -1 for a scalar plan):
+/* One-call boundary, as b200sht_sht_* (workspace of b200sht_vsht_workspace_bytes; -1 for a scalar plan or an order shard):
  *   forward          x [B][C][2][nlat][nlon] (dtype) -> coeffs                        <- RealVectorSHT.forward
  *   inverse          coeffs -> y [B][C][2][nlat][nlon] (dtype)                        <- InverseRealVectorSHT.forward
  *   forward_adjoint  dL/dcoeffs -> dL/dx     inverse_adjoint  dL/dy -> dL/dcoeffs      <- their autograd backward (PyTorch complex-gradient convention) */

@@ -95,7 +95,7 @@ int b200sht_plan_create_ex(b200sht_plan** out, int nlat, int nlon, int lmax, int
                nlon, lmax, mmax, m_offset);
   B200_REQUIRE(m_offset + mmax <= nlon / 2 + 1, "plan_create: m_offset+mmax=%d exceeds nlon/2+1=%d", m_offset + mmax, nlon / 2 + 1);
   const int vector = (flags & B200SHT_PLAN_VECTOR) ? 1 : 0;
-  B200_REQUIRE(!vector || (m_offset == 0 && !(flags & B200SHT_PLAN_FFT_ONLY)), "plan_create: a vector plan has no order offset and holds tables");
+  B200_REQUIRE(!vector || !(flags & B200SHT_PLAN_FFT_ONLY), "plan_create: a vector plan holds tables (B200SHT_PLAN_VECTOR with B200SHT_PLAN_FFT_ONLY)");
   B200_REQUIRE(!vector || lmax <= (1 << 29), "plan_create: lmax=%d too large", lmax);
   b200sht_plan* pl = new b200sht_plan();
   memset(static_cast<Plan*>(pl), 0, sizeof(Plan));
@@ -485,6 +485,10 @@ static int vector_precision(int precision, const char* who) {
   B200_VECTOR_PLAN(pl, who);                                                                                 \
   B200_REQUIRE((C) > 0 && (C) <= (1 << 28), who ": bad channel count %d", (C));                             \
   if (int _rc = vector_precision(precision, who)) return _rc
+// the one-call entries and the tiled synthesis run the longitude stage (or the tensor-core DFT's tiled layout) over orders 0 .. mmax - 1: they
+// need the plan of all orders, not an order shard of the distributed transforms
+#define B200_VECTOR_ALL_ORDERS(pl, who) \
+  B200_REQUIRE((pl)->m0 == 0, who ": vector plan with order offset %d (an order shard serves the stage entry points only)", (pl)->m0)
 
 int b200sht_vector_legendre_analysis(const b200sht_plan* pl, const float* latspec, float* spec, int B, int C, int precision, void* stream) {
   B200_VECTOR_ARGS(pl, C, precision, "vector_legendre_analysis");
@@ -496,6 +500,7 @@ int b200sht_vector_legendre_synthesis(const b200sht_plan* pl, const float* spec,
 }
 int b200sht_vector_legendre_synthesis_tiled(const b200sht_plan* pl, const float* spec, float* latspec, int B, int C, void* stream) {
   B200_VECTOR_ARGS(pl, C, B200SHT_PREC_TF32, "vector_legendre_synthesis_tiled");
+  B200_VECTOR_ALL_ORDERS(pl, "vector_legendre_synthesis_tiled");
   return legendre_synthesis_tiled_any(pl, spec, latspec, B, 2 * C, stream);
 }
 int b200sht_vector_spec_unpack(const b200sht_plan* pl, const float* spec, void* coeffs, int B, int C, int scaled, void* stream) {
@@ -510,12 +515,13 @@ int b200sht_vector_spec_pack(const b200sht_plan* pl, const void* coeffs, float* 
 }
 
 int64_t b200sht_vsht_workspace_bytes(const b200sht_plan* pl, int B, int C) {
-  if (!pl || !pl->vector || B <= 0 || C <= 0 || C > (1 << 28)) return -1;
+  if (!pl || !pl->vector || pl->m0 != 0 || B <= 0 || C <= 0 || C > (1 << 28)) return -1;
   return b200sht_sht_workspace_bytes(pl, B, 2 * C);
 }
 
 int b200sht_vsht_forward(const b200sht_plan* pl, const void* x, int dtype, int B, int C, void* coeffs, void* ws, int precision, void* stream) {
   B200_VECTOR_ARGS(pl, C, precision, "vsht_forward");
+  B200_VECTOR_ALL_ORDERS(pl, "vsht_forward");
   B200_REQUIRE(x && coeffs && ws && B > 0, "vsht_forward: bad argument");
   float *X, *sp;
   split_ws(pl, B, 2 * C, ws, &X, &sp);
@@ -526,6 +532,7 @@ int b200sht_vsht_forward(const b200sht_plan* pl, const void* x, int dtype, int B
 
 int b200sht_vsht_inverse(const b200sht_plan* pl, const void* coeffs, void* y, int dtype, int B, int C, void* ws, int precision, void* stream) {
   B200_VECTOR_ARGS(pl, C, precision, "vsht_inverse");
+  B200_VECTOR_ALL_ORDERS(pl, "vsht_inverse");
   B200_REQUIRE(y && coeffs && ws && B > 0, "vsht_inverse: bad argument");
   float *Z, *sp;
   split_ws(pl, B, 2 * C, ws, &Z, &sp);
@@ -537,6 +544,7 @@ int b200sht_vsht_inverse(const b200sht_plan* pl, const void* coeffs, void* y, in
 int b200sht_vsht_forward_adjoint(const b200sht_plan* pl, const void* gcoeffs, void* gx, int dtype, int B, int C, void* ws, int precision,
                                  void* stream) {
   B200_VECTOR_ARGS(pl, C, precision, "vsht_forward_adjoint");
+  B200_VECTOR_ALL_ORDERS(pl, "vsht_forward_adjoint");
   B200_REQUIRE(gx && gcoeffs && ws && B > 0, "vsht_forward_adjoint: bad argument");
   float *Z, *sp;
   split_ws(pl, B, 2 * C, ws, &Z, &sp);
@@ -548,6 +556,7 @@ int b200sht_vsht_forward_adjoint(const b200sht_plan* pl, const void* gcoeffs, vo
 int b200sht_vsht_inverse_adjoint(const b200sht_plan* pl, const void* gy, int dtype, int B, int C, void* gcoeffs, void* ws, int precision,
                                  void* stream) {
   B200_VECTOR_ARGS(pl, C, precision, "vsht_inverse_adjoint");
+  B200_VECTOR_ALL_ORDERS(pl, "vsht_inverse_adjoint");
   B200_REQUIRE(gy && gcoeffs && ws && B > 0, "vsht_inverse_adjoint: bad argument");
   float *X, *sp;
   split_ws(pl, B, 2 * C, ws, &X, &sp);

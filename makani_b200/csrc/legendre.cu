@@ -128,8 +128,9 @@ __global__ void build_table_kernel(float* __restrict__ table, const double* __re
   legendre_column(m0 + m, lmax, cost[k], csphase, out, kp);
 }
 
-// vector plan: table[m] = D rows [0, L) then Q rows [L, 2L)   (L = lmax / 2)
-__global__ void build_vector_table_kernel(float* __restrict__ table, const double* __restrict__ cost, int nlat, int kp, int L, int csphase) {
+// vector plan: table[m] = D rows [0, L) then Q rows [L, 2L) of the global order m0 + m   (L = lmax / 2)
+__global__ void build_vector_table_kernel(float* __restrict__ table, const double* __restrict__ cost, int nlat, int kp, int L, int csphase,
+                                          int m0) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   const int m = blockIdx.y;
   if (k >= kp) return;
@@ -139,13 +140,13 @@ __global__ void build_vector_table_kernel(float* __restrict__ table, const doubl
     for (int l = 0; l < L; ++l) D[(size_t)l * kp] = Q[(size_t)l * kp] = 0.f;
     return;
   }
-  legendre_vector_column(m, L, cost[k], csphase, D, Q, kp);
+  legendre_vector_column(m0 + m, L, cost[k], csphase, D, Q, kp);
 }
 
 int build_table(Plan* pl, const double* d_cost, cudaStream_t st) {
   dim3 grid(ceil_div(pl->kp, 128), pl->mmax);
   if (pl->vector)
-    build_vector_table_kernel<<<grid, 128, 0, st>>>(pl->d_table, d_cost, pl->nlat, pl->kp, pl->lmax / 2, pl->csphase);
+    build_vector_table_kernel<<<grid, 128, 0, st>>>(pl->d_table, d_cost, pl->nlat, pl->kp, pl->lmax / 2, pl->csphase, pl->m0);
   else
     build_table_kernel<<<grid, 128, 0, st>>>(pl->d_table, d_cost, pl->nlat, pl->kp, pl->lmax, pl->mmax, pl->csphase, pl->m0);
   B200_CHECK_LAUNCH();
@@ -376,9 +377,10 @@ int spec_pack(const Plan* pl, const void* coeffs, float* spec, int B, int C, cud
 //   pack:    D_theta = f S,  D_phi = -f T,  Q_theta = i f T,  Q_phi = i f S
 // f = 1 / (l (l + 1)) (0 at l = 0) when `scaled`, else 1.  pack(scaled) is the adjoint of unpack(scaled): the forward transform ends in
 // unpack(1) and its adjoint starts with pack(1); the inverse transform starts with pack(0) and its adjoint ends in unpack(0).
+// Local order m is the global order mo + m (the plan's order offset): only the l >= mo + m test depends on it.
 // block: 32 orders x 16 vector channels (32 spec columns) of one (l, b)
 __global__ void __launch_bounds__(256) vector_spec_unpack_kernel(const float* __restrict__ spec, float2* __restrict__ coeffs, int L, int M, int B,
-                                                                 int C, int cp, int scaled) {
+                                                                 int C, int cp, int mo, int scaled) {
   __shared__ float tile[4][32][33];   // D re, D im, Q re, Q im  x  [m][column]
   const int l = blockIdx.z / B, b = blockIdx.z % B;
   const int m0 = blockIdx.x * 32, c0 = blockIdx.y * 16;
@@ -388,7 +390,7 @@ __global__ void __launch_bounds__(256) vector_spec_unpack_kernel(const float* __
   for (int mm = ty; mm < 32; mm += 8) {
     const int m = m0 + mm;
     float v[4] = {0.f, 0.f, 0.f, 0.f};
-    if (m < M && j < 2 * C && l >= m) {
+    if (m < M && j < 2 * C && l >= mo + m) {
       const float* d = spec + ((size_t)l * M + m) * JP + (size_t)b * cp + j;
       const float* q = d + (size_t)L * M * JP;
       v[0] = d[0]; v[1] = d[pstride]; v[2] = q[0]; v[3] = q[pstride];
@@ -410,9 +412,10 @@ __global__ void __launch_bounds__(256) vector_spec_unpack_kernel(const float* __
   }
 }
 
-// writes every entry of the stacked spec (zeros for l < m and in the channel padding): the Legendre kernels read all rows l >= lstart(m)
+// writes every entry of the stacked spec (zeros for l < mo + m and in the channel padding): the Legendre kernels read all rows
+// l >= lstart(mo + m)
 __global__ void __launch_bounds__(256) vector_spec_pack_kernel(const float2* __restrict__ coeffs, float* __restrict__ spec, int L, int M, int B,
-                                                               int C, int cp, int scaled) {
+                                                               int C, int cp, int mo, int scaled) {
   __shared__ float tile[4][32][33];
   const int l = blockIdx.z / B, b = blockIdx.z % B;
   const int m0 = blockIdx.x * 32, c0 = blockIdx.y * 16;
@@ -422,7 +425,7 @@ __global__ void __launch_bounds__(256) vector_spec_pack_kernel(const float2* __r
   for (int cc = ty; cc < 16; cc += 8) {
     const int c = c0 + cc, m = m0 + tx;
     float2 S = make_float2(0.f, 0.f), T = S;
-    if (c < C && m < M && l >= m) {
+    if (c < C && m < M && l >= mo + m) {
       const float2* in = coeffs + ((size_t)(b * C + c) * 2 * L + l) * M + m;
       S = in[0];
       T = in[(size_t)L * M];
@@ -447,9 +450,9 @@ int vector_spec_convert(const Plan* pl, float* spec, void* coeffs, int B, int C,
   dim3 grid(ceil_div(pl->mmax, 32), to_packed ? ceil_div(cp, 32) : ceil_div(C, 16), L * B);
   B200_REQUIRE(grid.z <= 65535, "vector spec conversion: lmax*B=%u exceeds grid limit", grid.z);
   if (to_packed)
-    vector_spec_pack_kernel<<<grid, 256, 0, st>>>(static_cast<const float2*>(coeffs), spec, L, pl->mmax, B, C, cp, scaled);
+    vector_spec_pack_kernel<<<grid, 256, 0, st>>>(static_cast<const float2*>(coeffs), spec, L, pl->mmax, B, C, cp, pl->m0, scaled);
   else
-    vector_spec_unpack_kernel<<<grid, 256, 0, st>>>(spec, static_cast<float2*>(coeffs), L, pl->mmax, B, C, cp, scaled);
+    vector_spec_unpack_kernel<<<grid, 256, 0, st>>>(spec, static_cast<float2*>(coeffs), L, pl->mmax, B, C, cp, pl->m0, scaled);
   B200_CHECK_LAUNCH();
   return 0;
 }

@@ -9,6 +9,11 @@ The local stages run on the CUDA kernels of this package: an FFT-only plan for t
 this rank's orders (`b200sht_plan_create_ex`); the exchanged tensors use the plain complex layout, converted by
 `b200sht_latspec_(un)pack` / `b200sht_spec_(un)pack_ex`.  The local-stage backend is replaceable (`set_local_ops`) so that the
 choreography is unit-tested on CPU with gloo against the serial oracle.
+
+DistributedRealVectorSHT / DistributedInverseRealVectorSHT (torch_harmonics' distributed vector transforms, built by makani's VortDivCRPSLoss
+and GradientCRPSLoss with spatial_distributed=True) run the same choreography on (B, C, 2, ., .) fields: the transposes split the vector
+channels, the longitude stages see the 2C component rows and the Legendre stage runs on a vector plan of this rank's orders
+(B200SHT_PLAN_VECTOR with an order offset, `b200sht_vector_*`).
 """
 import ctypes
 
@@ -114,9 +119,28 @@ class CudaLocalOps:
                 _plan_cache[key] = p
             return p
 
+    def _vleg_plan(self, device):
+        """vector plan (tables D and Q) of this rank's orders m_offset .. m_offset + mmax_local - 1 over all latitudes"""
+        from .. import _lib as L
+        from ..sht import Plan, _plan_cache, _plan_lock
+        from ..quadrature import _grid_np
+        t = self.t
+        key = ("dist-vleg", t.nlat, t.nlon, t.lmax, t.mmax, t.grid, t.m_offset, t.mmax_local, bool(t.csphase), device.index)
+        with _plan_lock:
+            p = _plan_cache.get(key)
+            if p is None:
+                cost, w = _grid_np(t.nlat, t.grid)
+                p = Plan.create_ex(t.nlat, t.nlon, t.lmax, t.mmax_local, t.m_offset, L.PLAN_VECTOR, cost, w, t.csphase, device)
+                _plan_cache[key] = p
+            return p
+
     def _prec(self):
         from ..sht import resolve_precision
         return resolve_precision(self.t.precision)
+
+    def _vprec(self):
+        from ..vector_sht import _vector_precision
+        return _vector_precision(self.t.precision)
 
     # -- stages --------------------------------------------------------------------------------------------------
     def fft(self, x):
@@ -132,6 +156,14 @@ class CudaLocalOps:
 
     def ilegendre(self, xc):
         return _LocalILegendre.apply(xc.to(torch.complex64).contiguous(), self._leg_plan(xc.device), self._prec())
+
+    def vlegendre(self, xc):
+        """complex (B, C, 2, nlat, m_loc) -> complex (B, C, 2, lmax, m_loc): (theta, phi) components -> (S, T) coefficients"""
+        return _LocalVLegendre.apply(xc.to(torch.complex64).contiguous(), self._vleg_plan(xc.device), self._vprec())
+
+    def ivlegendre(self, xc):
+        """complex (B, C, 2, lmax, m_loc) -> complex (B, C, 2, nlat, m_loc)"""
+        return _LocalIVLegendre.apply(xc.to(torch.complex64).contiguous(), self._vleg_plan(xc.device), self._vprec())
 
 
 def _lib():
@@ -244,12 +276,62 @@ class _LocalILegendre(torch.autograd.Function):
         return _legendre_call(ctx.plan, ctx.prec, g.contiguous(), 0), None, None
 
 
+def _vlegendre_call(plan, prec, xc, direction, scaled):
+    """vector plan of an order shard.  direction 0: (B,C,2,nlat,m) -> (B,C,2,L,m), latspec pack -> analysis -> vector_spec_unpack(scaled);
+    1: (B,C,2,L,m) -> (B,C,2,nlat,m), vector_spec_pack(scaled) -> synthesis -> latspec unpack.  The C vector fields are 2C component rows."""
+    L = _lib()
+    B, C = xc.shape[:2]
+    dev = xc.device
+    lat = torch.empty(plan.latspec_elems(B, 2 * C), dtype=torch.float32, device=dev)
+    spec = torch.empty(plan.spec_elems(B, 2 * C), dtype=torch.float32, device=dev)
+    if direction == 0:
+        out = torch.empty(B, C, 2, plan.lmax, plan.mmax, dtype=torch.complex64, device=dev)
+        L.call("b200sht_latspec_pack", plan.handle, _p(xc), _p(lat), B, 2 * C, _st(dev))
+        L.call("b200sht_vector_legendre_analysis", plan.handle, _p(lat), _p(spec), B, C, prec, _st(dev))
+        L.call("b200sht_vector_spec_unpack", plan.handle, _p(spec), _p(out), B, C, scaled, _st(dev))
+    else:
+        out = torch.empty(B, C, 2, plan.nlat, plan.mmax, dtype=torch.complex64, device=dev)
+        L.call("b200sht_vector_spec_pack", plan.handle, _p(xc), _p(spec), B, C, scaled, _st(dev))
+        L.call("b200sht_vector_legendre_synthesis", plan.handle, _p(spec), _p(lat), B, C, prec, _st(dev))
+        L.call("b200sht_latspec_unpack", plan.handle, _p(lat), _p(out), B, 2 * C, _st(dev))
+    return out
+
+
+class _LocalVLegendre(torch.autograd.Function):
+    """analysis with the 1 / (l (l + 1)) scaling; backward: its adjoint, vector_spec_pack(scaled=1) -> synthesis"""
+
+    @staticmethod
+    def forward(ctx, xc, plan, prec):
+        ctx.plan, ctx.prec = plan, prec
+        return _vlegendre_call(plan, prec, xc, 0, 1)
+
+    @staticmethod
+    def backward(ctx, g):
+        return _vlegendre_call(ctx.plan, ctx.prec, g.to(torch.complex64).contiguous(), 1, 1), None, None
+
+
+class _LocalIVLegendre(torch.autograd.Function):
+    """synthesis without scaling; backward: its adjoint, analysis -> vector_spec_unpack(scaled=0)"""
+
+    @staticmethod
+    def forward(ctx, xc, plan, prec):
+        ctx.plan, ctx.prec = plan, prec
+        return _vlegendre_call(plan, prec, xc, 1, 0)
+
+    @staticmethod
+    def backward(ctx, g):
+        return _vlegendre_call(ctx.plan, ctx.prec, g.to(torch.complex64).contiguous(), 0, 0), None, None
+
+
 _LOCAL_OPS_FACTORY = CudaLocalOps
 
 
 def set_local_ops(factory):
     """Replace the local-stage backend (tests: a CPU implementation built on the oracle).  `factory(transform)` -> object with
-    fft / ifft / legendre / ilegendre."""
+    fft / ifft / legendre / ilegendre, and for DistributedRealVectorSHT / DistributedInverseRealVectorSHT also
+    vlegendre(xc): complex (B, C, 2, nlat, m_loc) -> (B, C, 2, lmax, m_loc), the Legendre stage of the forward vector transform on this rank's
+    orders (theta / phi components in, spheroidal / toroidal coefficients out, 1 / (l (l + 1)) applied), and ivlegendre, its inverse-transform
+    counterpart (B, C, 2, lmax, m_loc) -> (B, C, 2, nlat, m_loc)."""
     global _LOCAL_OPS_FACTORY
     _LOCAL_OPS_FACTORY = factory if factory is not None else CudaLocalOps
 
@@ -345,3 +427,58 @@ class DistributedInverseRealSHT(_DistributedBase):
         if bias is not None:
             y = y + bias.to(y.dtype)
         return y
+
+
+# ----------------------------------------------------------------------------------------------------- vector modules
+def _as_vector_fields(x, tail, who):
+    """(..., 2, a, b) -> (B, C, 2, a, b) (leading dimensions flattened into vector channels unless x is 5-D) plus the leading shape"""
+    if x.dim() < 3 or tuple(x.shape[-3:]) != tail:
+        raise ValueError(f"{who}: expected local shape (..., {tail[0]}, {tail[1]}, {tail[2]}), got {tuple(x.shape)}")
+    return (x if x.dim() == 5 else x.reshape(1, -1, *tail)), x.shape[:-3]
+
+
+class DistributedRealVectorSHT(_DistributedBase):
+    """x local (..., 2, nlat_loc, nlon_loc) float32 / bf16 -> coefficients local complex (..., 2, l_loc, m_loc) (component 0 theta, 1 phi in;
+    spheroidal S, toroidal T out).  The transposes of DistributedRealSHT on the 5-D (B, C, 2, ., .) tensor: they split the vector channels
+    (dim 1), so both components of a field stay on one rank; the longitude stages see its 2C component rows."""
+
+    def forward(self, x):
+        from ..vector_sht import _vector_precision
+        _vector_precision(self.precision)
+        x5, lead = _as_vector_fields(x, (2, self.nlat_local, self.nlon_local), "DistributedRealVectorSHT")
+        num_chans = x5.shape[1]
+        if self.comm_size_azimuth > 1:
+            x5 = distributed_transpose_azimuth(x5, (1, -1), self.lon_shapes)
+        B, C = x5.shape[:2]
+        xc = self._ops.fft(x5.reshape(B, 2 * C, self.nlat_local, self.nlon)).reshape(B, C, 2, self.nlat_local, self.mmax)
+        if self.comm_size_azimuth > 1:
+            xc = distributed_transpose_azimuth(xc, (-1, 1), compute_split_shapes(num_chans, self.comm_size_azimuth))
+        if self.comm_size_polar > 1:
+            xc = distributed_transpose_polar(xc, (1, -2), self.lat_shapes)
+        xc = self._ops.vlegendre(xc)
+        if self.comm_size_polar > 1:
+            xc = distributed_transpose_polar(xc, (-2, 1), compute_split_shapes(num_chans, self.comm_size_polar))
+        return xc if x.dim() == 5 else xc.reshape(*lead, 2, self.lmax_local, self.mmax_local)
+
+
+class DistributedInverseRealVectorSHT(_DistributedBase):
+    """coefficients local complex (..., 2, l_loc, m_loc) -> x local (..., 2, nlat_loc, nlon_loc) (float32 unless `dtype` says otherwise);
+    the transposes of DistributedInverseRealSHT on the vector channels, as in DistributedRealVectorSHT."""
+
+    def forward(self, x, dtype=torch.float32):
+        from ..vector_sht import _vector_precision
+        _vector_precision(self.precision)
+        x5, lead = _as_vector_fields(x, (2, self.lmax_local, self.mmax_local), "DistributedInverseRealVectorSHT")
+        num_chans = x5.shape[1]
+        if self.comm_size_polar > 1:
+            x5 = distributed_transpose_polar(x5, (1, -2), self.l_shapes)
+        xc = self._ops.ivlegendre(x5)
+        if self.comm_size_polar > 1:
+            xc = distributed_transpose_polar(xc, (-2, 1), compute_split_shapes(num_chans, self.comm_size_polar))
+        if self.comm_size_azimuth > 1:
+            xc = distributed_transpose_azimuth(xc, (1, -1), self.m_shapes)
+        B, C = xc.shape[:2]
+        y = self._ops.ifft(xc.reshape(B, 2 * C, self.nlat_local, self.mmax), dtype).reshape(B, C, 2, self.nlat_local, self.nlon)
+        if self.comm_size_azimuth > 1:
+            y = distributed_transpose_azimuth(y, (-1, 1), compute_split_shapes(num_chans, self.comm_size_azimuth))
+        return y if x.dim() == 5 else y.reshape(*lead, 2, self.nlat_local, self.nlon_local)
