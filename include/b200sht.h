@@ -122,9 +122,12 @@ int64_t b200sht_spec_elems_lm(int L, int M, int B, int C);
  *   X[m][p][r][k] = row_scale[k] * mode_scale[m] * sum_j x[r][k][j] exp(-2 pi i m j / nlon)
  * scale_mode 0: SHT forward     (row_scale = quad_w[k] * 2 pi / nlon, mode_scale = 1)
  * scale_mode 1: adjoint of irfft (row_scale = 1, mode_scale = 1 for m = 0 and Nyquist, 2 otherwise)
- * scale_mode | 2: TF32 precision: the output is rounded to the nearest TF32 value (it is the operand of a TF32 GEMM) and,
- *                 for nlon = 8 * N2 <= 1520 and mmax <= 256, the transform itself runs on the tensor cores (radix-8 butterflies on
- *                 the CUDA cores x a [mmax/8 x nlon/16] DFT matrix as a TF32 GEMM, csrc/dft.cu) */
+ * scale_mode | 2: TF32 precision: the output is a TF32 value (it is the operand of a TF32 GEMM) and, for nlon = 8 * N2 <= 1520 and
+ *                 mmax <= 256, the transform itself runs on the tensor cores (radix-8 butterflies on the CUDA cores x a
+ *                 [mmax/8 x nlon/16] DFT matrix as a TF32 GEMM, csrc/dft.cu) when also x is 16-byte aligned and, for fp32 rows,
+ *                 nlon % 32 == 0 (bf16 rows: any such nlon); otherwise the CUDA-core FFT serves the call.  The CUDA-core FFT
+ *                 rounds its output to the nearest TF32 value; the tensor-core DFT stores a bias-compensated truncation
+ *                 (the value scaled by 1 + 2^-10/3, then its 13 low mantissa bits cleared), unbiased over a binade. */
 int b200sht_fft_analysis(const b200sht_plan* plan, const void* x, int dtype, int B, int C,
                          float* latspec, int scale_mode, void* stream);
 /* Longitude synthesis: truncated half spectrum -> real rows (+ optional per-channel bias, cast to dtype).

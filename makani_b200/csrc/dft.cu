@@ -679,6 +679,7 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
     // 8 q + 2 t (fragment column q) and 8 q + 2 t + 1 (fragment column q + 4) of both operands.
     const size_t plane = (size_t)p.R * p.kp;
     const float tcomp = p.round_tf32 ? kTruncComp : 1.f;
+    const uint32_t tmask = p.round_tf32 ? 0xffffe000u : 0xffffffffu;
     const int c = warp, gq = lane >> 2, q = lane & 3;
     mbar_wait(b_full, 0);
     int n = 0;
@@ -743,12 +744,14 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
           for (int e = 0; e < 2; ++e) {
             const int m = c + 8 * (8 * j + 2 * q + e);
             if (m >= p.mmax) continue;
-            // round_tf32: the consumer is the TF32 Legendre GEMM, which truncates its operands -> bias-compensated truncation folded
-            // into the scale factor (see B200_DFT_TF32_MODE above) instead of 3 instructions of cvt.rna per value
+            // round_tf32: the output is a TF32 value -- the bias-compensated truncation (see B200_DFT_TF32_MODE above) folded into the
+            // scale factor, then the 13 low bits cleared (one LOP3 instead of the 3 instructions of cvt.rna).  The TF32 Legendre GEMM
+            // ignores those bits anyway; readers of the fp32 value (the bias gradient, latspec_unpack) then see an unbiased TF32 value
+            // instead of one scaled by 1 + 2^-10 / 3.
             const float sc = ((p.mode == 0) ? rs : ((m == 0 || 2 * m == p.nlon) ? 1.f : 2.f)) * tcomp;
             float* dst = xb + (size_t)m * 2 * plane;
-            dst[0] = xr[j][2 * h + e] * sc;
-            dst[plane] = xi[j][2 * h + e] * sc;
+            dst[0] = __uint_as_float(__float_as_uint(xr[j][2 * h + e] * sc) & tmask);
+            dst[plane] = __uint_as_float(__float_as_uint(xi[j][2 * h + e] * sc) & tmask);
           }
       }
     }
