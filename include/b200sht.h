@@ -17,6 +17,7 @@
  *   b200sht_vsht_forward         <- torch_harmonics.RealVectorSHT.forward         (makani/utils/losses/base_loss.py:427-469 VortDivBaseLoss)
  *   b200sht_vsht_inverse         <- torch_harmonics.InverseRealVectorSHT.forward  (base_loss.py:427-469 and :518-565 GradientBaseLoss)
  *   b200sht_vsht_*_adjoint       <- autograd backward of the two vector transforms
+ *   b200sht_disco_forward/adjoint<- the psi contraction of torch_harmonics.DiscreteContinuousConvS2 and its adjoint (fourcastnet3.py:117-252, :511-543)
  *
  * Conventions
  *   - every function returns 0 on success, a negative b200sht_status otherwise; b200sht_last_error() gives text.
@@ -308,6 +309,39 @@ int b200sht_instance_norm_backward(const void* x, const void* dy, void* dx, cons
 int b200sht_bias_gelu_forward(const void* x, const float* bias, void* y, int dtype, int B, int C, int64_t hw, void* stream);
 int b200sht_bias_gelu_backward(const void* x, const float* bias, const void* dy, void* dx, float* row_sums, float* workspace, int dtype, int B, int C, int64_t hw,
                                void* stream);
+
+/* ------------------------------------------------------------------ DISCO convolution on the sphere (SURVEY row N1)
+ * Replaces the two sparse contractions of torch_harmonics.DiscreteContinuousConvS2 (built at makani/models/networks/fourcastnet3.py:117-252,
+ * :364-381, :511-543, snonet.py).  The filter tensor psi[k, t, i, j] (K kernel functions, output latitude t, input latitude i, input longitude
+ * j, quadrature merged in) is restated in makani_b200/disco.py and DESIGN.md section 5:
+ *   output point (colatitude theta_t, longitude 0), input point (theta_i, phi_j = 2 pi j / nlon_in);
+ *   r = arccos(cos theta_t cos theta_i + sin theta_t sin theta_i cos phi_j),
+ *   phi' = atan2(sin phi_j sin theta_i, cos theta_t sin theta_i cos phi_j - cos theta_i sin theta_t) in [0, 2 pi)   (YZY rotation by -theta_t);
+ *   support r <= r_c = (1 + 1e-3) theta_cutoff; morlet: rho = r / r_c, x = rho sin phi', y = rho cos phi',
+ *   psi_k = cos^2(pi rho / 2) h_n(x) h_m(y), n = k mod n1, m = k / n1, h_j(u) = sin(ceil(j/2) pi u) (j odd), cos(ceil(j/2) pi u) (j even);
+ *   stored psi_hat = psi q_i / (d + 1e-9), q_i = 2 pi w_i / nlon_in, d per basis_norm_mode ("mean": mean over t of sum |psi| q, "individual":
+ *   that sum at t, "support": sum q at t, "none": 1).
+ * Contractions, with pscale = nlon_in / nlon_out (nlon_in % nlon_out == 0):
+ *   forward  X[b,c,k,t,p] = sum_{i,j} psi_hat[k,t,i,j] x[b,c,i,(j + pscale p) mod nlon_in]            x: [B][C][nlat_in][nlon_in] fp32 or bf16
+ *   adjoint  dx[b,c,i,j'] = sum_{k,t,p,j: (j + pscale p) mod nlon_in = j'} psi_hat[k,t,i,j] dX[b,c,k,t,p]   X, dX: [B][C][K][nlat_out][nlon_out] fp32
+ * The channel contraction y = W X (+ bias) is a grouped GEMM left to the caller.
+ *
+ * b200sht_disco_plan_create: nnz entries (ker[n], lat_out[n], col_in[n] = i * nlon_in + j, vals[n]) in HOST memory, any order; entries with the
+ *   same (k, t, col) are summed in fp64.  Both device layouts (by output latitude, sorted by (i, j); by input latitude, sorted by (t, j)) hold the
+ *   values rounded to fp32.  Synchronises `stream` once, after the upload.  nlon_in and nlon_out at most 16384 (B200SHT_ERR_UNSUPPORTED).
+ * b200sht_disco_plan_query: 0 nlat_in, 1 nlon_in, 2 nlat_out, 3 nlon_out, 4 K, 5 nnz, 6 support points (distinct (t, i, j)), 7 device bytes,
+ *   8 pscale; -1 otherwise.
+ * b200sht_disco_forward: writes every element of X; fp32 accumulation, each X element summed over its points in (i, j) order.
+ * b200sht_disco_adjoint: writes every element of dx (dtype: fp32 or bf16, rounded once at the end); each dx element is summed by one thread in a
+ *   fixed order, without atomics: results are bit-identical run to run.
+ * B * C rows at most 65535 per call. */
+typedef struct b200sht_disco_plan b200sht_disco_plan;
+int b200sht_disco_plan_create(b200sht_disco_plan** plan, int nlat_in, int nlon_in, int nlat_out, int nlon_out, int K, int64_t nnz, const int* ker,
+                              const int* lat_out, const int* col_in, const double* vals, void* stream);
+int b200sht_disco_plan_destroy(b200sht_disco_plan* plan);
+int64_t b200sht_disco_plan_query(const b200sht_disco_plan* plan, int what);
+int b200sht_disco_forward(const b200sht_disco_plan* plan, const void* x, int dtype, int B, int C, float* X, void* stream);
+int b200sht_disco_adjoint(const b200sht_disco_plan* plan, const float* dX, void* dx, int dtype, int B, int C, void* stream);
 
 /* Programmatic dependent launch between the tensor-core kernels of a call sequence (prologue of kernel i+1 under the tail of kernel i; environment
  * B200SHT_PDL sets the initial value, default on).  Returns the previous setting.  Results do not depend on it. */

@@ -17,13 +17,14 @@ import types
 
 
 def install_torch_harmonics_shim(force=False):
-    """Register `torch_harmonics`, `.quadrature`, `.distributed`, `.distributed.primitives` backed by makani_b200."""
+    """Register `torch_harmonics`, `.quadrature`, `.filter_basis`, `.distributed`, `.distributed.primitives` backed by makani_b200."""
     if "torch_harmonics" in sys.modules and not force:
         mod = sys.modules["torch_harmonics"]
         if getattr(mod, "__b200_shim__", False):
             return mod
         raise RuntimeError("a real torch_harmonics is already imported; pass force=True to replace it")
     import makani_b200 as mb
+    from makani_b200 import disco as mbdisco
     from makani_b200 import distributed as mbd
     from makani_b200 import quadrature as mbq
 
@@ -34,11 +35,18 @@ def install_torch_harmonics_shim(force=False):
     th.InverseRealSHT = mb.InverseRealSHT
     th.RealVectorSHT = mb.RealVectorSHT
     th.InverseRealVectorSHT = mb.InverseRealVectorSHT
+    th.DiscreteContinuousConvS2 = mb.DiscreteContinuousConvS2
+    fb = types.ModuleType("torch_harmonics.filter_basis")
+    fb.get_filter_basis, fb.MorletFilterBasis = mbdisco.get_filter_basis, mbdisco.MorletFilterBasis
+    th.filter_basis = fb
+    # makani builds the distributed DISCO convolution at spatial model parallelism > 1: a clear NotImplementedError instead of an AttributeError
+    mbd.DistributedDiscreteContinuousConvS2 = mbdisco.DistributedDiscreteContinuousConvS2
     th.quadrature = mbq
     th.distributed = mbd
     th.__path__ = []  # mark as package so that submodule imports resolve through sys.modules
     sys.modules["torch_harmonics"] = th
     sys.modules["torch_harmonics.quadrature"] = mbq
+    sys.modules["torch_harmonics.filter_basis"] = fb
     sys.modules["torch_harmonics.distributed"] = mbd
     sys.modules["torch_harmonics.distributed.primitives"] = mbd.primitives
     sys.modules["torch_harmonics.distributed.utils"] = mbd

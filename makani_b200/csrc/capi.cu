@@ -73,6 +73,12 @@ static inline Plan lm_plan(int L, int M, int m0 = 0, int dense = 0) { Plan p; me
 int latspec_convert(const Plan* pl, float* lat, void* coeffs, int B, int C, int to_packed, cudaStream_t st);
 int vector_spec_convert(const Plan* pl, float* spec, void* coeffs, int B, int C, int to_packed, int scaled, cudaStream_t st);
 int umma_available();
+int disco_plan_create(b200sht_disco_plan** out, int nlat_in, int nlon_in, int nlat_out, int nlon_out, int K, long long nnz, const int* ker,
+                      const int* lat_out, const int* col_in, const double* vals, cudaStream_t st);
+int disco_plan_destroy(b200sht_disco_plan* pl);
+long long disco_plan_query(const b200sht_disco_plan* pl, int what);
+int disco_forward(const b200sht_disco_plan* pl, const void* x, int dtype, int B, int C, float* X, cudaStream_t st);
+int disco_adjoint(const b200sht_disco_plan* pl, const float* dX, void* dx, int dtype, int B, int C, cudaStream_t st);
 
 }  // namespace b200sht
 
@@ -851,6 +857,24 @@ int b200sht_debug_dft_profile(uint64_t* counters16) {
 int b200sht_debug_dft_host(int N, int mmax, int direction, int scale_mode, float row_scale, const float* in, float* out) {
   B200_REQUIRE(in && out && N > 0 && mmax > 0, "debug_dft_host: bad argument");
   return dft_host(N, mmax, direction, scale_mode & 1, &row_scale, in, out);
+}
+
+// ---- DISCO convolution (disco.cu)
+int b200sht_disco_plan_create(b200sht_disco_plan** plan, int nlat_in, int nlon_in, int nlat_out, int nlon_out, int K, int64_t nnz, const int* ker,
+                              const int* lat_out, const int* col_in, const double* vals, void* stream) {
+  return disco_plan_create(plan, nlat_in, nlon_in, nlat_out, nlon_out, K, nnz, ker, lat_out, col_in, vals, S(stream));
+}
+
+int b200sht_disco_plan_destroy(b200sht_disco_plan* plan) { return disco_plan_destroy(plan); }
+
+int64_t b200sht_disco_plan_query(const b200sht_disco_plan* plan, int what) { return disco_plan_query(plan, what); }
+
+int b200sht_disco_forward(const b200sht_disco_plan* plan, const void* x, int dtype, int B, int C, float* X, void* stream) {
+  return disco_forward(plan, x, dtype, B, C, X, S(stream));
+}
+
+int b200sht_disco_adjoint(const b200sht_disco_plan* plan, const float* dX, void* dx, int dtype, int B, int C, void* stream) {
+  return disco_adjoint(plan, dX, dx, dtype, B, C, S(stream));
 }
 
 }  // extern "C"
