@@ -18,6 +18,7 @@
  *   b200sht_vsht_inverse         <- torch_harmonics.InverseRealVectorSHT.forward  (base_loss.py:427-469 and :518-565 GradientBaseLoss)
  *   b200sht_vsht_*_adjoint       <- autograd backward of the two vector transforms
  *   b200sht_disco_forward/adjoint<- the psi contraction of torch_harmonics.DiscreteContinuousConvS2 and its adjoint (fourcastnet3.py:117-252, :511-543)
+ *   b200sht_resample_forward/adjoint <- torch_harmonics.ResampleS2(mode="bilinear") and its adjoint (fourcastnet3.py:356-358)
  *
  * Conventions
  *   - every function returns 0 on success, a negative b200sht_status otherwise; b200sht_last_error() gives text.
@@ -342,6 +343,35 @@ int b200sht_disco_plan_destroy(b200sht_disco_plan* plan);
 int64_t b200sht_disco_plan_query(const b200sht_disco_plan* plan, int what);
 int b200sht_disco_forward(const b200sht_disco_plan* plan, const void* x, int dtype, int B, int C, float* X, void* stream);
 int b200sht_disco_adjoint(const b200sht_disco_plan* plan, const float* dX, void* dx, int dtype, int B, int C, void* stream);
+
+/* ------------------------------------------------------------------ bilinear resampling on the sphere
+ * Replaces torch_harmonics.ResampleS2(mode="bilinear"), the upsampling of FCN3's DiscreteContinuousDecoder with upsample_sht=False
+ * (makani/models/networks/fourcastnet3.py:356-358) and of SNO's decoder.  The tables are built on the host in fp64 (makani_b200/resample.py,
+ * DESIGN.md section 4.8) and passed here rounded to fp32:
+ *   lat_idx[t] = a, lat_w[t] = wt (t < nlat_out): output row t interpolates the expanded input rows a and a + 1; lon_left[p] = l, lon_right[p] = r,
+ *   lon_w[p] = wp (p < nlon_out).  With expand_poles the expanded input has nlat_in + 2 rows: row 0 is the longitude mean of input row 0, row
+ *   nlat_in + 1 the mean of input row nlat_in - 1, and row e otherwise input row e - 1; without it the expanded input is the input.
+ *   forward  y[b,t,p] = lerp(lerp(X[b,a,l], X[b,a,r], wp), lerp(X[b,a+1,l], X[b,a+1,r], wp), wt),  lerp(u, v, w) = u + w (v - u) (w < 1/2),
+ *            v - (v - u)(1 - w) otherwise, so w = 0 and w = 1 reproduce u and v exactly;     x: [planes][nlat_in][nlon_in], y: [planes][nlat_out][nlon_out]
+ *   adjoint  dx = R^T dy, the weights of the adjoint being 1 - wt, wt, 1 - wp, wp (1 - w rounded once from fp64).  A pole pseudo-row adds
+ *            (1 / nlon_in) sum_{t: a_t or a_t + 1 is the pseudo-row} w sum_p dy[b,t,p] to every element of input row 0 (nlat_in - 1).
+ * All data fp32.
+ *
+ * b200sht_resample_plan_create: the tables in HOST memory; checks 0 <= a, a + 1 < nlat_in + 2 expand_poles and 0 <= l, r < nlon_in.  Builds the
+ *   adjoint's two CSR lists (by expanded input row, t ascending; by input column, p ascending) and synchronises `stream` once, after the upload.
+ *   nlon_in at most 8192 and nlon_out at most 16384 (B200SHT_ERR_UNSUPPORTED).
+ * b200sht_resample_plan_query: 0 nlat_in, 1 nlon_in, 2 nlat_out, 3 nlon_out, 4 expand_poles, 5 device bytes; -1 otherwise.
+ * b200sht_resample_forward: writes every element of y; a pole mean is one fp32 sum over the row in a fixed order, divided by nlon_in.
+ * b200sht_resample_adjoint: writes every element of dx; each element is summed by one thread (the pole term by one warp) in a fixed order, without
+ *   atomics: results are bit-identical run to run.
+ * planes: up to 65535 per call (more where the row lengths let several planes share a CTA). */
+typedef struct b200sht_resample_plan b200sht_resample_plan;
+int b200sht_resample_plan_create(b200sht_resample_plan** plan, int nlat_in, int nlon_in, int nlat_out, int nlon_out, int expand_poles, const int* lat_idx,
+                                 const float* lat_w, const int* lon_left, const int* lon_right, const float* lon_w, void* stream);
+int b200sht_resample_plan_destroy(b200sht_resample_plan* plan);
+int64_t b200sht_resample_plan_query(const b200sht_resample_plan* plan, int what);
+int b200sht_resample_forward(const b200sht_resample_plan* plan, const float* x, float* y, int planes, void* stream);
+int b200sht_resample_adjoint(const b200sht_resample_plan* plan, const float* dy, float* dx, int planes, void* stream);
 
 /* Programmatic dependent launch between the tensor-core kernels of a call sequence (prologue of kernel i+1 under the tail of kernel i; environment
  * B200SHT_PDL sets the initial value, default on).  Returns the previous setting.  Results do not depend on it. */

@@ -95,6 +95,12 @@ _SIGNATURES = {
     "b200sht_disco_plan_query": (c_int64, [_P, c_int]),
     "b200sht_disco_forward": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P]),
     "b200sht_disco_adjoint": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P]),
+    # bilinear resampling on the sphere
+    "b200sht_resample_plan_create": (c_int, [ctypes.POINTER(_P), c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P]),
+    "b200sht_resample_plan_destroy": (c_int, [_P]),
+    "b200sht_resample_plan_query": (c_int64, [_P, c_int]),
+    "b200sht_resample_forward": (c_int, [_P, _P, _P, c_int, _P]),
+    "b200sht_resample_adjoint": (c_int, [_P, _P, _P, c_int, _P]),
     # debug / CPU-testable entry points (same device code compiled for the host)
     "b200sht_debug_fft_host": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P]),
     "b200sht_debug_dft_host": (c_int, [c_int, c_int, c_int, c_int, c_float, _P, _P]),

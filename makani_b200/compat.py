@@ -27,6 +27,7 @@ def install_torch_harmonics_shim(force=False):
     from makani_b200 import disco as mbdisco
     from makani_b200 import distributed as mbd
     from makani_b200 import quadrature as mbq
+    from makani_b200 import resample as mbres
 
     th = types.ModuleType("torch_harmonics")
     th.__b200_shim__ = True
@@ -36,11 +37,13 @@ def install_torch_harmonics_shim(force=False):
     th.RealVectorSHT = mb.RealVectorSHT
     th.InverseRealVectorSHT = mb.InverseRealVectorSHT
     th.DiscreteContinuousConvS2 = mb.DiscreteContinuousConvS2
+    th.ResampleS2 = mb.ResampleS2
     fb = types.ModuleType("torch_harmonics.filter_basis")
     fb.get_filter_basis, fb.MorletFilterBasis = mbdisco.get_filter_basis, mbdisco.MorletFilterBasis
     th.filter_basis = fb
     # makani builds the distributed DISCO convolution at spatial model parallelism > 1: a clear NotImplementedError instead of an AttributeError
     mbd.DistributedDiscreteContinuousConvS2 = mbdisco.DistributedDiscreteContinuousConvS2
+    mbd.DistributedResampleS2 = mbres.DistributedResampleS2   # likewise for the decoder's resampling
     th.quadrature = mbq
     th.distributed = mbd
     th.__path__ = []  # mark as package so that submodule imports resolve through sys.modules

@@ -79,6 +79,12 @@ int disco_plan_destroy(b200sht_disco_plan* pl);
 long long disco_plan_query(const b200sht_disco_plan* pl, int what);
 int disco_forward(const b200sht_disco_plan* pl, const void* x, int dtype, int B, int C, float* X, cudaStream_t st);
 int disco_adjoint(const b200sht_disco_plan* pl, const float* dX, void* dx, int dtype, int B, int C, cudaStream_t st);
+int resample_plan_create(b200sht_resample_plan** out, int nlat_in, int nlon_in, int nlat_out, int nlon_out, int expand_poles, const int* lat_idx,
+                         const float* lat_w, const int* lon_left, const int* lon_right, const float* lon_w, cudaStream_t st);
+int resample_plan_destroy(b200sht_resample_plan* pl);
+long long resample_plan_query(const b200sht_resample_plan* pl, int what);
+int resample_forward(const b200sht_resample_plan* pl, const float* x, float* y, int planes, cudaStream_t st);
+int resample_adjoint(const b200sht_resample_plan* pl, const float* dy, float* dx, int planes, cudaStream_t st);
 
 }  // namespace b200sht
 
@@ -875,6 +881,24 @@ int b200sht_disco_forward(const b200sht_disco_plan* plan, const void* x, int dty
 
 int b200sht_disco_adjoint(const b200sht_disco_plan* plan, const float* dX, void* dx, int dtype, int B, int C, void* stream) {
   return disco_adjoint(plan, dX, dx, dtype, B, C, S(stream));
+}
+
+// ---- bilinear resampling on the sphere (resample.cu)
+int b200sht_resample_plan_create(b200sht_resample_plan** plan, int nlat_in, int nlon_in, int nlat_out, int nlon_out, int expand_poles, const int* lat_idx,
+                                 const float* lat_w, const int* lon_left, const int* lon_right, const float* lon_w, void* stream) {
+  return resample_plan_create(plan, nlat_in, nlon_in, nlat_out, nlon_out, expand_poles, lat_idx, lat_w, lon_left, lon_right, lon_w, S(stream));
+}
+
+int b200sht_resample_plan_destroy(b200sht_resample_plan* plan) { return resample_plan_destroy(plan); }
+
+int64_t b200sht_resample_plan_query(const b200sht_resample_plan* plan, int what) { return resample_plan_query(plan, what); }
+
+int b200sht_resample_forward(const b200sht_resample_plan* plan, const float* x, float* y, int planes, void* stream) {
+  return resample_forward(plan, x, y, planes, S(stream));
+}
+
+int b200sht_resample_adjoint(const b200sht_resample_plan* plan, const float* dy, float* dx, int planes, void* stream) {
+  return resample_adjoint(plan, dy, dx, planes, S(stream));
 }
 
 }  // extern "C"
