@@ -295,6 +295,9 @@ int b200sht_debug_dft_host(int N, int mmax, int direction, int scale_mode, float
 /* wait-time profile of the tensor-core DFT kernels (environment B200SHT_DFT_PROF=1): 16 counters of SM clocks, accumulated over all launches since the
  * last call and cleared by it (slots: see csrc/dft.cu).  All zeros when the profile is off.  Synchronises the device. */
 int b200sht_debug_dft_profile(uint64_t* counters16);
+/* wait-time profile of the tensor-core GEMM engine (a library built with -DB200SHT_UMMA_PROFILE): 16 counters of SM clocks, accumulated over all
+ * engine launches since the last call and cleared by it (slots: see csrc/umma.cu).  All zeros in the shipped build.  Synchronises the device. */
+int b200sht_debug_umma_profile(uint64_t* counters16);
 /* ------------------------------------------------------------------ pointwise tail of the SFNO block (SURVEY row N2) */
 /* Replaces torch.nn.InstanceNorm2d(num_features, eps, affine) (+ the nn.GELU that follows it) as built at makani/models/networks/sfnonet.py:618-620 and
  * applied at :385-406, and the bias + GELU of the 1x1-convolution stacks (makani/models/common/layers.py:537-760).  x, y, dy, dx: [B][C][hw] contiguous, float or

@@ -44,6 +44,7 @@ int dft_plan_init(Plan* pl);
 void dft_plan_destroy(Plan* pl);
 int dft_host(int N, int mmax, int direction, int mode, const float* rowscale, const float* in, float* out);
 int dft_profile_read(unsigned long long* out16);
+int umma_profile_read(unsigned long long* out16);
 int legendre_analysis_umma(const Plan* pl, const float* X, float* spec, int B, int C, cudaStream_t st, const float* X_lo = nullptr, int k_begin = 0,
                            int k_end = -1, int accumulate = 0, int last = 1);
 int dft_analysis(const Plan* pl, const void* x, int dtype, int B, int C, float* X, int mode, int round_tf32, cudaStream_t st, int k_begin = 0, int k_end = -1);
@@ -858,6 +859,11 @@ int b200sht_debug_set_lat_chunks_syn(int n) {
 int b200sht_debug_dft_profile(uint64_t* counters16) {
   B200_REQUIRE(counters16 != nullptr, "debug_dft_profile: null argument");
   return dft_profile_read(reinterpret_cast<unsigned long long*>(counters16));
+}
+
+int b200sht_debug_umma_profile(uint64_t* counters16) {
+  B200_REQUIRE(counters16 != nullptr, "debug_umma_profile: null argument");
+  return umma_profile_read(reinterpret_cast<unsigned long long*>(counters16));
 }
 
 int b200sht_debug_dft_host(int N, int mmax, int direction, int scale_mode, float row_scale, const float* in, float* out) {

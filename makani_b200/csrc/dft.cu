@@ -161,15 +161,6 @@ __device__ __forceinline__ void prof_wait(unsigned long long* prof, int slot, ui
   if (lead) atomicAdd(prof + slot, (unsigned long long)(clock64() - t0));
 }
 
-// bulk tensor stores from shared memory (one bulk async-group per output tile, issued and waited for by one thread)
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, uint32_t src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(tm), "r"(src), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
 // 3-D view (nlon, nlat, rows) of the synthesis output, box (ow, 8, 1), no swizzle
 static int make_tmap_out(CUtensorMap* tm, void* base, bool bf16, int nlon, int nlat, long long rows, int ow) {
   TmapKey key;

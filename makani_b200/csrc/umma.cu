@@ -3,7 +3,7 @@
 //
 //   one persistent engine (umma_kernel<Traits, NB, SPLIT>, one CTA per SM walking the tile list): warp 0 lane 0 = TMA producer, warps
 //   1..8 = consumers; consumer warp w owns rows 16 (w - 1) .. + 15 of the 128-row tile, issues mma.m16n8k8 (TF32) on them against every
-//   column of the tile and stores its accumulators itself.  The tile width (NB fragments of 8 columns) and the 3 x TF32 mode are template
+//   column of the tile and stores its accumulators itself (the TF32 synthesis stages them for bulk stores instead).  The tile width (NB fragments of 8 columns) and the 3 x TF32 mode are template
 //   parameters: the MMA loop is straight-line code without per-fragment predicates, and no instantiation spills registers.  A ring of `stages` operand stages guarded by full/empty mbarriers runs continuously
 //   across tiles, so the producer prefetches the next tile while the consumers finish the current one and write it out.
 //
@@ -36,6 +36,7 @@ constexpr int kMaxStages = 8;
 struct EngineParams {
   int stages;
   uint32_t stage_bytes, tx_bytes;
+  uint32_t out_bytes;      // output staging after the ring (bulk-store epilogue of SynTraits), 0 for the register epilogues
   int gx, gy, gz;          // logical tile grid (x fastest); CTAs walk it round-robin
   int split;               // 3 x TF32 (strict fp32 on the tensor cores): every stage also holds the residual tiles of both operands, `lo_off`
   uint32_t lo_off;         // bytes after the main tiles, and each MMA becomes hi.hi + hi.lo + lo.hi into the same accumulator
@@ -253,18 +254,38 @@ __device__ __forceinline__ void for_each_run(const float (&acc)[NA][4], F f) {
   }
 }
 
+// ----------------------------------------------------------------------------------------- wait-time profile
+// Built with -DB200SHT_UMMA_PROFILE (`python -m makani_b200.build --define B200SHT_UMMA_PROFILE --out libb200sht_umma_prof.so`, driven by
+// scripts/umma_waitprof.py): every role sums the SM clocks it spends per state into g_umma_prof, read back and cleared by
+// b200sht_debug_umma_profile().  Slots: 0 producer waits for a free stage (empty), 1 consumer warps wait for a loaded stage (full), 2 consumer
+// warps in the MMA loop (without the full waits), 3 consumer warps in the epilogue, 4 consumer-warp lifetime, 5 producer lifetime,
+// 6 tiles (consumer warps), 7 CTAs.  Consumer slots are sums over the 8 warps of every CTA.  The shipped build has none of it.
+#ifdef B200SHT_UMMA_PROFILE
+constexpr bool kUmmaProfile = true;
+#else
+constexpr bool kUmmaProfile = false;
+#endif
+__device__ unsigned long long g_umma_prof[16];
+__device__ __forceinline__ long long prof_clock() { return kUmmaProfile ? clock64() : 0; }
+
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(32 * kConsumerWarps) : "memory"); }   // warps 1..8 only
+
 // Persistent engine: one CTA per SM loops over tiles.  The operand ring (full/empty) runs continuously across tiles, so the
 // TMA producer prefetches the next tile while the consumer warps finish the current one.  NB: 8-column fragments per warp; SPLIT: 3 x TF32.
+// Traits with kStaged (the synthesis, not in 3 x TF32) stage the finished tile in shared memory after the ring and bulk-store it from there.
 template <class T, int NB, bool SPLIT>
 __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_constant__ typename T::Params p) {
+  constexpr bool kStaged = T::kStaged && !SPLIT;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* gbase = smem_raw + (base - raw);
   const int stages = p.stages;
   const uint32_t stage_bytes = p.stage_bytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(gbase + (size_t)stages * stage_bytes);
+  uint8_t* const out = gbase + (size_t)stages * stage_bytes;   // output staging (p.out_bytes, 1024-byte aligned)
+  uint64_t* full = reinterpret_cast<uint64_t*>(out + p.out_bytes);
   uint64_t* empty = full + kMaxStages;
+  const long long t_cta0 = prof_clock();
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
   pdl_trigger();   // the next kernel of the stream may be scheduled while this one runs (it waits for our completion before touching data)
@@ -279,6 +300,7 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_cons
 
   if (warp == 0) {
     if (lane == 0) {
+      unsigned long long w_empty = 0;
       int kbg = 0;   // k-block counter across tiles: position in the operand ring
       for (int ti = blockIdx.x; ti < ntiles; ti += gridDim.x) {
         typename T::Tile tile;
@@ -286,31 +308,58 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_cons
         const int nk = T::num_kblocks(p, tile);
         for (int kb = 0; kb < nk; ++kb, ++kbg) {
           const int s = kbg % stages, it = kbg / stages;
-          if (it > 0) mbar_wait(&empty[s], (it - 1) & 1);
+          if (it > 0) {
+            const long long t0 = prof_clock();
+            mbar_wait(&empty[s], (it - 1) & 1);
+            if constexpr (kUmmaProfile) w_empty += clock64() - t0;
+          }
           mbar_expect_tx(&full[s], p.tx_bytes);
           T::load(p, tile, kb, base + s * stage_bytes, &full[s]);
         }
+      }
+      if constexpr (kUmmaProfile) {
+        atomicAdd(&g_umma_prof[0], w_empty);
+        atomicAdd(&g_umma_prof[5], (unsigned long long)(clock64() - t_cta0));
+        atomicAdd(&g_umma_prof[7], 1ull);
       }
     }
     __syncwarp();
   } else {
     const int row0 = 16 * (warp - 1);
     int kbg = 0;
+    uint32_t piece = 0;   // staged epilogue: output pieces written so far (position in the double buffer)
+    unsigned long long w_full = 0, t_loop = 0, t_epi = 0, n_tiles = 0;
     for (int ti = blockIdx.x; ti < ntiles; ti += gridDim.x) {
       typename T::Tile tile;
       if (!T::make_tile(p, tile, ti % p.gx, (ti / p.gx) % p.gy, ti / (p.gx * p.gy))) continue;
+      const long long t0 = prof_clock();
       const int nk = T::num_kblocks(p, tile);
       float acc[NB * T::kPlanes][4];
 #pragma unroll
       for (int j = 0; j < NB * T::kPlanes; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
       for (int kb = 0; kb < nk; ++kb, ++kbg) {
         const int s = kbg % stages, it = kbg / stages;
+        const long long tw = prof_clock();
         mbar_wait(&full[s], it & 1);
+        if constexpr (kUmmaProfile) w_full += clock64() - tw;
         T::template mma<NB, SPLIT>(p, gbase + (size_t)s * stage_bytes, row0, acc);
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[s]);   // this warp's reads of the stage are done
       }
-      T::template epilogue<NB>(p, tile, row0, acc);
+      const long long t1 = prof_clock();
+      if constexpr (kStaged) T::template epilogue_staged<NB>(p, tile, row0, acc, out, piece);
+      else T::template epilogue<NB>(p, tile, row0, acc);
+      if constexpr (kUmmaProfile) { t_loop += t1 - t0; t_epi += clock64() - t1; ++n_tiles; }
+    }
+    // the bulk stores must be complete (not only have read shared memory) before the CTA exits: a dependent kernel's griddepcontrol.wait
+    // relies on grid completion for the visibility of this kernel's output
+    if constexpr (kStaged) if (warp == 1) bulk_wait0();
+    if constexpr (kUmmaProfile) if (lane == 0) {
+      atomicAdd(&g_umma_prof[1], w_full);
+      atomicAdd(&g_umma_prof[2], t_loop - w_full);
+      atomicAdd(&g_umma_prof[3], t_epi);
+      atomicAdd(&g_umma_prof[4], (unsigned long long)(clock64() - t_cta0));
+      atomicAdd(&g_umma_prof[6], n_tiles);
     }
   }
 }
@@ -327,6 +376,7 @@ struct AnaTraits {
     int acc_in, round_out;   // add to the spec values already stored (chunks after the first) / round the result to TF32 (last chunk)
   };
   static constexpr int kPlanes = 1;
+  static constexpr bool kStaged = false;   // register epilogue
   struct Tile { int m, l0, c0, pb0; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.m = bz;
@@ -379,12 +429,19 @@ struct SynTraits {
     alignas(64) CUtensorMap tmA;  // table (k, l, m)   box (32, 32, 1)   MN-major A (M = k)
     alignas(64) CUtensorMap tmB;  // spec  (n, m, l)   box (32, 1, 32)   MN-major B (N = n)
     alignas(64) CUtensorMap tmA_lo, tmB_lo;   // residuals of the table and of spec (split mode)
+    alignas(64) CUtensorMap tmZ;  // Z, bulk stores (k % 8, c, k / 8, pb, m) or tiled (k % 8, c, k / 8, plane 8 M2 + m, b)   box (8, 4, 16, 1, 1)
     float* Z;
     int L, M, nlat, kp, C, cp, PB, nblk, N, m0;
     int kc0, kc1;           // latitude range [kc0, kc1) of this launch (kc0 a multiple of 128): the tiles cover these rows only
     int tiled, M2, KT, B;   // tiled output for the tensor-core DFT (dft.cu): Z[r][k / 8][p][m / 8][m % 8][k % 8], orders padded to 8 * M2
   };
   static constexpr int kPlanes = 1;
+  // Bulk-store epilogue (TF32; the 3 x TF32 instantiations keep the register epilogue below: their doubled stages leave no room for it).
+  // The output of a tile is staged as boxes of 4 columns x 128 latitudes, 2 KB each, laid out [k / 8][column][k % 8] -- the order of the
+  // store map's box (8, 4, 16), which is the same in both layouts of Z.  Tiles of at most 20 fragments (160 columns) stage the whole
+  // tile at once; wider ones stage 32 columns at a time in two alternating 16 KB buffers.
+  static constexpr bool kStaged = true;
+  __host__ __device__ static constexpr uint32_t out_bytes(int nb) { return nb <= 20 ? 4096u * nb : 2u * 16384u; }
   struct Tile { int m, k0, n0, lbeg; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.m = bz;
@@ -446,6 +503,69 @@ struct SynTraits {
         }
       }
   }
+
+  // Columns 32 J .. + 31 of the warp's 16 rows into the 8 boxes at `buf`.  The lane holds latitudes k, k + 1 (k = row0 + 2 g) of columns
+  // 32 J + 8 q + 4 e + c (c = 0..3): box 8 J + 2 q + e, column c, one 8-byte store at [k / 8][c][k % 8].  Lane q writes column c = i ^ q
+  // in step i, so that the 16 lanes of a half-warp (g = 0..3 or 4..7: one k / 8) cover 16 different 8-byte bank slots.
+  template <int NB>
+  __device__ __forceinline__ static void stage_cols(const float (&acc)[NB][4], int J, int row0, uint8_t* buf) {
+    const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+    const int k = row0 + 2 * g;
+    uint8_t* const b0 = buf + (k >> 3) * 128 + (k & 7) * 4 + q * 4096;
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int c = i ^ q;
+        const float v0 = c == 0 ? acc[4 * J][e] : c == 1 ? acc[4 * J + 1][e] : c == 2 ? acc[4 * J + 2][e] : acc[4 * J + 3][e];
+        const float v1 = c == 0 ? acc[4 * J][2 + e] : c == 1 ? acc[4 * J + 1][2 + e] : c == 2 ? acc[4 * J + 2][2 + e] : acc[4 * J + 3][2 + e];
+        *reinterpret_cast<float2*>(b0 + e * 2048 + c * 32) = make_float2(v0, v1);
+      }
+  }
+  // Warp 1: bulk stores of the tile's boxes bt0 .. bt0 + nbx - 1 (staged 2 KB apart from `buf`), a few per lane, one bulk group per lane.
+  // Boxes of columns past the tile's last one or of channel padding (c0 >= C) are skipped; the map's extents clip the rest: channels at C,
+  // latitudes at kc1.  Latitude padding rows (nlat <= k < kp) and orders without degrees hold zero accumulators and are stored as zeros.
+  __device__ static void store_boxes(const Params& p, const Tile& t, int bt0, int nbx, uint32_t buf) {
+    for (int b = threadIdx.x & 31; b < nbx; b += 32) {
+      const int jp = t.n0 + 4 * (bt0 + b);
+      const int pb = jp / p.cp, c0 = jp - pb * p.cp;
+      if (pb >= p.PB || c0 >= p.C) continue;
+      if (!p.tiled) {
+        tma_store_5d(&p.tmZ, buf + b * 2048, 0, c0, t.k0 >> 3, pb, t.m);
+      } else {   // pb = plane * B + b
+        const int pl = pb / p.B;
+        tma_store_5d(&p.tmZ, buf + b * 2048, 0, c0, t.k0 >> 3, pl * 8 * p.M2 + t.m, pb - pl * p.B);
+      }
+    }
+    bulk_commit();
+  }
+  // All 8 consumer warps: wait until the buffer's previous stores have read it, stage, make the writes visible to the async proxy, and let
+  // warp 1 issue the stores.  Nobody waits for the stores themselves: the consumers go on to the next tile's MMAs.
+  template <int NB>
+  __device__ __forceinline__ static void epilogue_staged(const Params& p, const Tile& t, int row0, const float (&acc)[NB][4], uint8_t* out,
+                                                         uint32_t& piece) {
+    const bool issuer = (threadIdx.x >> 5) == 1;
+    if constexpr (NB <= 20) {
+      if (issuer) bulk_wait_read<0>();
+      consumer_sync();
+#pragma unroll
+      for (int J = 0; J < NB / 4; ++J) stage_cols<NB>(acc, J, row0, out + J * 16384);
+      fence_proxy_async();
+      consumer_sync();
+      if (issuer) store_boxes(p, t, 0, 2 * NB, smem_u32(out));
+    } else {
+#pragma unroll
+      for (int J = 0; J < NB / 4; ++J, ++piece) {
+        uint8_t* const buf = out + (piece & 1) * 16384;
+        if (issuer) bulk_wait_read<1>();   // the stores of the piece before last, which used this buffer
+        consumer_sync();
+        stage_cols<NB>(acc, J, row0, buf);
+        fence_proxy_async();
+        consumer_sync();
+        if (issuer) store_boxes(p, t, 8 * J, 8, smem_u32(buf));
+      }
+    }
+  }
 };
 
 // ====================================================================================================== mix
@@ -476,6 +596,7 @@ __device__ __forceinline__ void st_vec(float* dst, const float (&v)[V]) {   // d
 struct MixFwdTraits {
   using Params = MixParams;
   static constexpr int kPlanes = 2;
+  static constexpr bool kStaged = false;   // register epilogue
   struct Tile { int l, m0, g, o0, lg; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.l = bz;
@@ -543,6 +664,7 @@ struct MixDgradTraits {
   using Params = MixParams;   // tmX = gy (channels = Cout), out = gx; N tiles over i
   using Tile = MixFwdTraits::Tile;  // o0 is the first input channel i0 of the tile
   static constexpr int kPlanes = 2;
+  static constexpr bool kStaged = false;   // register epilogue
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) { return MixFwdTraits::make_tile(p, t, bx, by, bz); }
   __device__ static void prefetch(const Params& p) { prefetch_tmap(&p.tmX); prefetch_tmap(&p.tmW); }
   __device__ static int num_kblocks(const Params& p, const Tile&) { return (p.Cog + 31) / 32; }
@@ -567,6 +689,7 @@ struct MixDgradTraits {
 struct MixWgradTraits {
   using Params = MixParams;   // tmX = x (A, rows i), tmX2 = gy (B, cols o); K = spectral rows (m, b)
   static constexpr int kPlanes = 2;
+  static constexpr bool kStaged = false;   // register epilogue
   struct Tile { int lz, i0, g, o0; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.lz = bz;
@@ -682,16 +805,20 @@ int umma_plan_table_lo(const Plan* cpl) {
   return 0;
 }
 
-constexpr size_t kSmemMax = 232448 - 4096;  // 227 KB minus barriers / epilogue scratch / alignment slack
+constexpr size_t kSmemOptIn = 232448;                         // 227 KB: the most a CTA may use on an H100
+constexpr size_t kSmemFixed = 1024 /*align*/ + 2 * kMaxStages * 8;
+constexpr size_t kSmemMax = kSmemOptIn - 4096;  // ring-only kernels: 227 KB minus barriers / alignment slack
 
-static void pick_stages(EngineParams* e, uint32_t stage_bytes, int /*k-blocks per tile: the ring runs across tiles*/) {
+// out_bytes: output staging of the bulk-store epilogue; its ring gets exactly what is left of the 227 KB
+static void pick_stages(EngineParams* e, uint32_t stage_bytes, int /*k-blocks per tile: the ring runs across tiles*/, uint32_t out_bytes = 0) {
   e->stage_bytes = stage_bytes;
-  int s = (int)(kSmemMax / stage_bytes);   // persistent: one CTA per SM owns the whole shared memory
+  e->out_bytes = out_bytes;
+  int s = (int)((out_bytes ? kSmemOptIn - kSmemFixed - out_bytes : kSmemMax) / stage_bytes);   // persistent: one CTA per SM owns it all
   if (s > kMaxStages) s = kMaxStages;
   if (s < 2) s = 2;
   e->stages = s;
 }
-static size_t smem_bytes(const EngineParams& e) { return (size_t)e.stages * e.stage_bytes + 1024 /*align*/ + 2 * kMaxStages * 8; }
+static size_t smem_bytes(const EngineParams& e) { return (size_t)e.stages * e.stage_bytes + e.out_bytes + kSmemFixed; }
 
 static int sm_count() {   // of the current device (the launch device: _lib.call makes the tensor's device current)
   std::call_once(g_dev_once, init_dev_caches);
@@ -838,7 +965,21 @@ int legendre_synthesis_umma(const Plan* pl, const float* spec, float* Z, int B, 
     if (rc) return rc;
     p.lo_off = 16384 + 4096 * p.nblk;
   }
-  pick_stages(&p, (16384 + 4096 * p.nblk) * (p.split ? 2 : 1), ceil_div(pl->lmax, 32));
+  uint32_t out_bytes = 0;
+  if (!p.split) {   // store map of the bulk-store epilogue: boxes of 8 x 16 latitudes x 4 channels, clipped at channel C and latitude kc1
+    B200_REQUIRE(k_end % 8 == 0, "legendre_synthesis: latitude range end %d is not a multiple of 8", k_end);
+    const long long kp = pl->kp, M2 = p.M2, KT = p.KT;
+    long long d[5] = {8, C, k_end / 8, PB, pl->mmax}, s[5] = {1, kp, 8, C * kp, PB * C * kp};
+    if (tiled) {
+      const long long d2[5] = {8, C, k_end / 8, 16 * M2, B}, s2[5] = {1, KT * 128 * M2, 128 * M2, 8, C * KT * 128 * M2};
+      memcpy(d, d2, sizeof(d)); memcpy(s, s2, sizeof(s));
+    }
+    int bx[5] = {8, 4, 16, 1, 1};
+    int rc = make_tmap(&p.tmZ, Z, 5, d, s, bx, false);
+    if (rc) return rc;
+    out_bytes = SynTraits::out_bytes(nb);
+  }
+  pick_stages(&p, (16384 + 4096 * p.nblk) * (p.split ? 2 : 1), ceil_div(pl->lmax, 32), out_bytes);
   p.tx_bytes = (16384 + 4096 * p.nblk) * (p.split ? 2 : 1);
   dim3 grid(ceil_div(k_end - k_begin, 128), ceil_div(JP, p.N), tiled ? 8 * p.M2 : pl->mmax);
   return p.split ? SplitWidths::launch_nb<SynTraits, true>(p, nb, grid, st) : LegendreWidths::launch_nb<SynTraits, false>(p, nb, grid, st);
@@ -935,6 +1076,14 @@ int mix_wgrad_umma(const Plan* pl, int op, const float* x, const float* gy, floa
   p.tx_bytes = 32768u + 8192u * p.nblk;
   dim3 grid(ceil_div(p.Cig, 128), p.n_nt * G, p.shared_w ? 1 : p.L);
   return MixWidths::launch_nb<MixWgradTraits, false>(p, p.N / 8, grid, st);
+}
+
+int umma_profile_read(unsigned long long* out16) {   // the wait-time counters of a B200SHT_UMMA_PROFILE build (zeros otherwise); clears them
+  B200_CHECK_CUDA(cudaDeviceSynchronize());
+  B200_CHECK_CUDA(cudaMemcpyFromSymbol(out16, g_umma_prof, 16 * sizeof(unsigned long long)));
+  static const unsigned long long zeros[16] = {};
+  B200_CHECK_CUDA(cudaMemcpyToSymbol(g_umma_prof, zeros, sizeof(zeros)));
+  return 0;
 }
 
 int mix_cbias_grad(const float* gy, void* gcb, int L, int M, int B, int Co, int dense, cudaStream_t st);  // mix.cu

@@ -151,6 +151,23 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm,
 // generic-proxy shared-memory writes -> visible to the async proxy (TMA)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// bulk tensor stores from shared memory.  Bulk async-groups are per thread: the thread that commits a group is the one that waits for it.
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, uint32_t src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(tm), "r"(src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_5d(const CUtensorMap* tm, uint32_t src, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(tm), "r"(src), "r"(c0), "r"(c1),
+               "r"(c2), "r"(c3), "r"(c4)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// wait until at most N of this thread's groups still read shared memory (.read) / are still writing global memory
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_read0() { bulk_wait_read<0>(); }
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
 // ================================================================================================== host side
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -173,7 +190,7 @@ struct TmapKey {
   const void* base;
   long long dims[5], strides[5];
   int box[5];
-  int rank, kind;   // kind: 0 fp32 / 128-byte swizzle, 4 fp32 segments, 5 bf16 segments
+  int rank, kind;   // kind: 0 fp32 / 128-byte swizzle, 1 fp32 / no swizzle, 4 fp32 segments, 5 bf16 segments
 };
 struct TmapCache {
   static constexpr int kSlots = 128;
@@ -204,11 +221,13 @@ inline void tmap_store(const TmapKey& k, const CUtensorMap* tm, int slot) {
   c.used[slot] = true;
 }
 
-// fp32 tensor map, 128-byte swizzle.  dims[0] is the contiguous dimension; strides (in floats) for dims 1..rank-1.
-inline int make_tmap(CUtensorMap* tm, const void* base, int rank, const long long* dims, const long long* strides, const int* box) {
+// fp32 tensor map, 128-byte swizzle (swizzle = false: none, box rows land densely).  dims[0] is the contiguous dimension; strides (in
+// floats) for dims 1..rank-1, in any order.
+inline int make_tmap(CUtensorMap* tm, const void* base, int rank, const long long* dims, const long long* strides, const int* box,
+                     bool swizzle = true) {
   TmapKey key;
   memset(&key, 0, sizeof(key));
-  key.base = base; key.rank = rank; key.kind = 0;
+  key.base = base; key.rank = rank; key.kind = swizzle ? 0 : 1;
   for (int i = 0; i < rank; ++i) { key.dims[i] = dims[i]; key.strides[i] = i ? strides[i] : 1; key.box[i] = box[i]; }
   int slot = 0;
   if (tmap_lookup(key, tm, &slot)) return 0;
@@ -227,7 +246,7 @@ inline int make_tmap(CUtensorMap* tm, const void* base, int rank, const long lon
   }
   if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) { set_error("tensor map base is not 16-byte aligned"); return B200SHT_ERR_INVALID; }
   CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d), rank %d", (int)r, rank); return B200SHT_ERR_CUDA; }
   tmap_store(key, tm, slot);
