@@ -25,9 +25,8 @@ def install_torch_harmonics_shim(force=False):
         raise RuntimeError("a real torch_harmonics is already imported; pass force=True to replace it")
     import makani_b200 as mb
     from makani_b200 import disco as mbdisco
-    from makani_b200 import distributed as mbd
+    from makani_b200 import distributed as mbd   # with DistributedDiscreteContinuousConvS2 and DistributedResampleS2
     from makani_b200 import quadrature as mbq
-    from makani_b200 import resample as mbres
 
     th = types.ModuleType("torch_harmonics")
     th.__b200_shim__ = True
@@ -41,9 +40,6 @@ def install_torch_harmonics_shim(force=False):
     fb = types.ModuleType("torch_harmonics.filter_basis")
     fb.get_filter_basis, fb.MorletFilterBasis = mbdisco.get_filter_basis, mbdisco.MorletFilterBasis
     th.filter_basis = fb
-    # makani builds the distributed DISCO convolution at spatial model parallelism > 1: a clear NotImplementedError instead of an AttributeError
-    mbd.DistributedDiscreteContinuousConvS2 = mbdisco.DistributedDiscreteContinuousConvS2
-    mbd.DistributedResampleS2 = mbres.DistributedResampleS2   # likewise for the decoder's resampling
     th.quadrature = mbq
     th.distributed = mbd
     th.__path__ = []  # mark as package so that submodule imports resolve through sys.modules

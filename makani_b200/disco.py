@@ -311,9 +311,9 @@ class DiscreteContinuousConvS2(nn.Module):
         return _DiscoConv.apply(x.contiguous(), self.weight, self.bias, self.plan(x.device), self.groups)
 
 
-class DistributedDiscreteContinuousConvS2(nn.Module):
-    """Placeholder of `torch_harmonics.distributed.DistributedDiscreteContinuousConvS2`: makani builds it at spatial model parallelism > 1."""
-
-    def __init__(self, *args, **kwargs):
-        raise NotImplementedError("DistributedDiscreteContinuousConvS2 is not implemented yet (the distributed DISCO convolution is a follow-up); "
-                                  "run FCN3's DISCO layers with spatial model parallelism 1")
+def __getattr__(name):
+    # the distributed module lives in makani_b200/distributed/disco.py; the reference runners import it from here
+    if name == "DistributedDiscreteContinuousConvS2":
+        from .distributed.disco import DistributedDiscreteContinuousConvS2
+        return DistributedDiscreteContinuousConvS2
+    raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

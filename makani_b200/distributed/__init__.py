@@ -14,6 +14,9 @@ DistributedRealVectorSHT / DistributedInverseRealVectorSHT (torch_harmonics' dis
 and GradientCRPSLoss with spatial_distributed=True) run the same choreography on (B, C, 2, ., .) fields: the transposes split the vector
 channels, the longitude stages see the 2C component rows and the Legendre stage runs on a vector plan of this rank's orders
 (B200SHT_PLAN_VECTOR with an order offset, `b200sht_vector_*`).
+
+DistributedDiscreteContinuousConvS2 (distributed/disco.py: a latitude halo and window plans of psi_hat) and DistributedResampleS2
+(distributed/resample.py: whole spheres of a subset of planes) are FCN3's local operators under the same h x w grid.
 """
 import ctypes
 
@@ -482,3 +485,7 @@ class DistributedInverseRealVectorSHT(_DistributedBase):
         if self.comm_size_azimuth > 1:
             y = distributed_transpose_azimuth(y, (-1, 1), compute_split_shapes(num_chans, self.comm_size_azimuth))
         return y if x.dim() == 5 else y.reshape(*lead, 2, self.nlat_local, self.nlon_local)
+
+
+from .disco import DistributedDiscreteContinuousConvS2, set_disco_local_ops  # noqa: E402,F401
+from .resample import DistributedResampleS2, set_resample_local_ops  # noqa: E402,F401

@@ -38,7 +38,7 @@ def _all_to_all(recv, send, group):
     backend = dist.get_backend(group)
     if backend == "nccl" or backend == "mpi":
         return dist.all_to_all(recv, send, group=group)
-    # gloo: pairwise exchange
+    # gloo: pairwise exchange; empty chunks (the variable-size halo of the distributed DISCO convolution) are not sent
     rank = dist.get_rank(group=group)
     ranks = dist.get_process_group_ranks(group) if group is not None else list(range(dist.get_world_size()))
     recv[rank].copy_(send[rank])
@@ -46,8 +46,10 @@ def _all_to_all(recv, send, group):
     for j, peer in enumerate(ranks):
         if j == rank:
             continue
-        ops.append(dist.P2POp(dist.isend, send[j], peer, group))
-        ops.append(dist.P2POp(dist.irecv, recv[j], peer, group))
+        if send[j].numel():
+            ops.append(dist.P2POp(dist.isend, send[j], peer, group))
+        if recv[j].numel():
+            ops.append(dist.P2POp(dist.irecv, recv[j], peer, group))
     if ops:
         for req in dist.batch_isend_irecv(ops):
             req.wait()
