@@ -140,7 +140,8 @@ int b200sht_fft_analysis(const b200sht_plan* plan, const void* x, int dtype, int
  *                 Error unless b200sht_plan_query(plan, 8) == 1. */
 int b200sht_fft_synthesis(const b200sht_plan* plan, const float* latspec, void* y, int dtype, int B, int C,
                           const float* bias, int scale_mode, void* stream);
-/* Legendre analysis  spec[l][m][..] = sum_k P[m][l][k] latspec[m][..][k]   (l >= 32*floor(m/32)) */
+/* Legendre analysis  spec[l][m][..] = sum_k P[m][l][k] latspec[m][..][k]   (l >= 32*floor(m/32)).  At every precision only the rows
+ * k < nlat of latspec are read: its latitude padding [nlat, kp) may hold anything, NaN included. */
 int b200sht_legendre_analysis(const b200sht_plan* plan, const float* latspec, float* spec, int B, int C,
                               int precision, void* stream);
 /* Legendre synthesis latspec[m][..][k] = sum_l P[m][l][k] spec[l][m][..] */

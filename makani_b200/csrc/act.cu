@@ -9,7 +9,7 @@ __device__ __forceinline__ float dleaky(float x, float s) { return x > 0.f ? 1.f
 
 template <bool BWD>
 __global__ void complex_relu_kernel(int mode, const float* __restrict__ x, const float* __restrict__ bias, float slope, const float* __restrict__ gy,
-                                    float* __restrict__ out, float* __restrict__ gbias, int L, int M, int B, int C, int cp, int dense) {
+                                    float* __restrict__ out, int L, int M, int B, int C, int cp, int dense) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long total = (long long)L * M * B * cp;
   if (idx >= total) return;
@@ -51,7 +51,6 @@ __global__ void complex_relu_kernel(int mode, const float* __restrict__ x, const
         const float drr = 1.f + iz3 * xi * xi, dri = -iz3 * xr * xi, dii = 1.f + iz3 * xr * xr;
         o_r = gr * drr + gi * dri;
         o_i = gr * dri + gi * dii;
-        if (gbias) atomicAdd(gbias + c, (gr * xr + gi * xi) / za);
       } else { o_r = 0.f; o_i = 0.f; }
     } else {
       const float ang = atan2f(xi, xr) - bb;
@@ -63,11 +62,40 @@ __global__ void complex_relu_kernel(int mode, const float* __restrict__ x, const
   out[base + plane] = o_i;
 }
 
+// modulus bias gradient: gbias[c] = sum over the stored triangle and batch of (gr xr + gi xi) / |z| where |z| > 0 and |z| + bias[c] > 0.
+// One block per channel in a fixed order (per-thread strided sums, then a fixed tree): the same bits on every run.
+__global__ void complex_relu_bias_grad_kernel(const float* __restrict__ x, const float* __restrict__ bias, const float* __restrict__ gy,
+                                              float* __restrict__ gbias, int L, int M, int B, int cp, int dense) {
+  const int c = blockIdx.x;
+  const float bb = bias ? bias[c] : 0.f;
+  const size_t plane = (size_t)B * cp;
+  float s = 0.f;
+  for (int l = 0; l < L; ++l) {
+    const int nrows = mend_d(l, M, dense) * B;
+    for (int row = threadIdx.x; row < nrows; row += blockDim.x) {
+      const int m = row / B, b = row % B;
+      const size_t base = ((size_t)l * M + m) * 2 * plane + (size_t)b * cp + c;
+      const float xr = x[base], xi = x[base + plane];
+      const float za = sqrtf(xr * xr + xi * xi);
+      if (za > 0.f && za + bb > 0.f) s += (gy[base] * xr + gy[base + plane] * xi) / za;
+    }
+  }
+  __shared__ float part[32];
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float a = threadIdx.x < (blockDim.x >> 5) ? part[threadIdx.x] : 0.f;
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if (threadIdx.x == 0) gbias[c] = a;
+  }
+}
+
 int complex_relu_fwd(const Plan* pl, int mode, const float* x, const float* bias, float slope, float* y, int B, int C, cudaStream_t st) {
   B200_REQUIRE(mode >= 0 && mode <= 3, "complex_relu: unknown mode %d", mode);
   const int cp = round_up(C, 4);
   const long long total = (long long)pl->lmax * pl->mmax * B * cp;
-  complex_relu_kernel<false><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(mode, x, bias, slope, nullptr, y, nullptr, pl->lmax, pl->mmax, B, C, cp, pl->dense);
+  complex_relu_kernel<false><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(mode, x, bias, slope, nullptr, y, pl->lmax, pl->mmax, B, C, cp, pl->dense);
   B200_CHECK_LAUNCH();
   return 0;
 }
@@ -77,8 +105,13 @@ int complex_relu_bwd(const Plan* pl, int mode, const float* x, const float* bias
   B200_REQUIRE(mode >= 0 && mode <= 3, "complex_relu: unknown mode %d", mode);
   const int cp = round_up(C, 4);
   const long long total = (long long)pl->lmax * pl->mmax * B * cp;
-  if (gbias) B200_CHECK_CUDA(cudaMemsetAsync(gbias, 0, sizeof(float) * C, st));
-  complex_relu_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(mode, x, bias, slope, gy, gx, gbias, pl->lmax, pl->mmax, B, C, cp, pl->dense);
+  if (gbias && mode == 2) {  // before gx is written: gx may alias gy or x
+    complex_relu_bias_grad_kernel<<<C, 256, 0, st>>>(x, bias, gy, gbias, pl->lmax, pl->mmax, B, cp, pl->dense);
+    B200_CHECK_LAUNCH();
+  } else if (gbias) {
+    B200_CHECK_CUDA(cudaMemsetAsync(gbias, 0, sizeof(float) * C, st));
+  }
+  complex_relu_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(mode, x, bias, slope, gy, gx, pl->lmax, pl->mmax, B, C, cp, pl->dense);
   B200_CHECK_LAUNCH();
   return 0;
 }

@@ -166,8 +166,9 @@ constexpr int TS = 64;   // tile edge
 constexpr int TK = 16;   // k slab
 
 // spec[l][m][jp] = sum_k P[m][l][k] * X[m][j][k]      grid: (jp tiles, l tiles, m)
+// Only rows k < nlat are read: the latitude padding [nlat, kp) of X may hold anything, as for the tensor-core engine.
 __global__ void __launch_bounds__(256) legendre_analysis_simt_kernel(const float* __restrict__ P, const float* __restrict__ X,
-                                                                     float* __restrict__ spec, int L, int M, int kp, int B,
+                                                                     float* __restrict__ spec, int L, int M, int nlat, int kp, int B,
                                                                      int C, int cp, int m0) {
   __shared__ float As[TK][TS + 4];
   __shared__ float Bs[TK][TS + 4];
@@ -191,11 +192,20 @@ __global__ void __launch_bounds__(256) legendre_analysis_simt_kernel(const float
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
 
-  for (int k0 = 0; k0 < kp; k0 += TK) {
+  for (int k0 = 0; k0 < nlat; k0 += TK) {
     float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
-    if (k0 + kq < kp) {  // kp is a multiple of 8, kq of 4: a float4 is entirely in or out
-      if (arow) a = __ldg(reinterpret_cast<const float4*>(arow + k0 + kq));
-      if (brow) b = __ldg(reinterpret_cast<const float4*>(brow + k0 + kq));
+    const int k = k0 + kq;
+    if (k + 4 <= nlat) {  // a whole quad of latitudes in range (rows are 16-byte aligned: kp % 8 == 0)
+      if (arow) a = __ldg(reinterpret_cast<const float4*>(arow + k));
+      if (brow) b = __ldg(reinterpret_cast<const float4*>(brow + k));
+    } else if (k < nlat) {  // the quad holding the last latitude: the rows beyond nlat stay zero
+      float av[4] = {0.f, 0.f, 0.f, 0.f}, bv[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int q = 0; k + q < nlat; ++q) {
+        if (arow) av[q] = __ldg(arow + k + q);
+        if (brow) bv[q] = __ldg(brow + k + q);
+      }
+      a = make_float4(av[0], av[1], av[2], av[3]);
+      b = make_float4(bv[0], bv[1], bv[2], bv[3]);
     }
     __syncthreads();
     As[kq + 0][lrow] = a.x; As[kq + 1][lrow] = a.y; As[kq + 2][lrow] = a.z; As[kq + 3][lrow] = a.w;
@@ -286,7 +296,7 @@ int legendre_analysis_simt(const Plan* pl, const float* X, float* spec, int B, i
   const int cp = round_up(C, 4);
   const int JP = 2 * B * cp;
   dim3 grid(ceil_div(JP, TS), ceil_div(pl->lmax, TS), pl->mmax);
-  legendre_analysis_simt_kernel<<<grid, 256, 0, st>>>(pl->d_table, X, spec, pl->lmax, pl->mmax, pl->kp, B, C, cp, pl->m0);
+  legendre_analysis_simt_kernel<<<grid, 256, 0, st>>>(pl->d_table, X, spec, pl->lmax, pl->mmax, pl->nlat, pl->kp, B, C, cp, pl->m0);
   B200_CHECK_LAUNCH();
   return 0;
 }

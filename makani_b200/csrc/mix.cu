@@ -314,20 +314,27 @@ int mix_cbias_grad(const float* gy, void* gcb, int L, int M, int B, int Co, int 
 // OP_DIAGONAL      w native complex [G][Cig][Cog][L][M]
 // OP_SEP_DHCONV    w native complex [G][Cig][L]         (Co == Ci)
 // OP_SEP_DIAGONAL  w native complex [G][Cig][L][M]
-// one thread per (l, m, b, out channel); purely bandwidth bound (each weight is used once per batch element)
+// one thread per (l, m, b, padded out channel); purely bandwidth bound (each weight is used once per batch element).  The threads of the
+// channel padding [NOut, cp_out) write its exact zeros, as every other producer of a packed spectrum does.
 template <int OP, int MODE>  // MODE 0 forward, 1 dgrad
 __global__ void mix_permode_kernel(const float* __restrict__ xin, const float2* __restrict__ w, float* __restrict__ yout, const MixDims d) {
   const int NOut = MODE == 0 ? d.Cog * d.G : d.Cig * d.G;
-  const long long total = (long long)d.L * d.M * d.B * NOut;
+  const int cp_in = MODE == 0 ? d.cpi : d.cpo, cp_out = MODE == 0 ? d.cpo : d.cpi;
+  const long long total = (long long)d.L * d.M * d.B * cp_out;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const int m = (int)(idx % d.M);
   long long rest = idx / d.M;
   const int l = (int)(rest % d.L); rest /= d.L;
-  const int oc = (int)(rest % NOut);
-  const int b = (int)(rest / NOut);
+  const int oc = (int)(rest % cp_out);
+  const int b = (int)(rest / cp_out);
   if (m >= mend_d(l, d.M, d.dense)) return;
-  const int cp_in = MODE == 0 ? d.cpi : d.cpo, cp_out = MODE == 0 ? d.cpo : d.cpi;
+  float* yb = yout + ((size_t)l * d.M + m) * 2 * d.B * cp_out + (size_t)b * cp_out;
+  if (oc >= NOut) {
+    yb[oc] = 0.f;
+    yb[(size_t)d.B * cp_out + oc] = 0.f;
+    return;
+  }
   const float* xb = xin + ((size_t)l * d.M + m) * 2 * d.B * cp_in + (size_t)b * cp_in;
   const size_t xp = (size_t)d.B * cp_in;
   float vr = 0.f, vi = 0.f;
@@ -348,7 +355,6 @@ __global__ void mix_permode_kernel(const float* __restrict__ xin, const float2* 
     if (MODE == 0) { vr = xr * ww.x - xi * ww.y; vi = xr * ww.y + xi * ww.x; }
     else { vr = xr * ww.x + xi * ww.y; vi = xi * ww.x - xr * ww.y; }
   }
-  float* yb = yout + ((size_t)l * d.M + m) * 2 * d.B * cp_out + (size_t)b * cp_out;
   yb[oc] = vr;
   yb[(size_t)d.B * cp_out + oc] = vi;
 }
@@ -422,7 +428,7 @@ int mix_forward_simt(const Plan* pl, int op, const float* x, const void* w, cons
     B200_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "mix_forward: grid too large");
     mix_dense_kernel<0><<<grid, 256, 0, st>>>(x, static_cast<const float*>(w), static_cast<const float2*>(cbias), y, d);
   } else {
-    const long long total = (long long)d.L * d.M * B * Co;
+    const long long total = (long long)d.L * d.M * B * d.cpo;
     const unsigned nb = (unsigned)((total + 255) / 256);
     const float2* wn = static_cast<const float2*>(w);
     if (op == B200SHT_OP_DIAGONAL) mix_permode_kernel<B200SHT_OP_DIAGONAL, 0><<<nb, 256, 0, st>>>(x, wn, y, d);
@@ -460,7 +466,7 @@ int mix_backward_simt(const Plan* pl, int op, const float* x, const void* w, con
   } else {
     const float2* wn = static_cast<const float2*>(w);
     if (gx) {
-      const long long total = (long long)d.L * d.M * B * Ci;
+      const long long total = (long long)d.L * d.M * B * d.cpi;
       const unsigned nb = (unsigned)((total + 255) / 256);
       if (op == B200SHT_OP_DIAGONAL) mix_permode_kernel<B200SHT_OP_DIAGONAL, 1><<<nb, 256, 0, st>>>(gy, wn, gx, d);
       else if (op == B200SHT_OP_SEP_DHCONV) mix_permode_kernel<B200SHT_OP_SEP_DHCONV, 1><<<nb, 256, 0, st>>>(gy, wn, gx, d);

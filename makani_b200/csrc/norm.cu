@@ -4,13 +4,18 @@
 // instance norm (batch-norm kernels with one block per channel) needs 15.6 ms of a 77 ms model step for them.
 //
 //   instance norm (+ GELU), rows = (b, c), n = H * W contiguous elements per row, every row split over `splits` CTAs:
-//     forward : stats   partial (sum, sum of squares) of x - x[row start] per (row, split)      read x
+//     forward : stats   (sum, sum of squares) of x - x[row start] per (row, pair of splits)     read x
+//                       in fp64: x - pivot is exact, so a pivot far from the row mean (an outlier at x[row, 0]) costs no accuracy.  One CTA
+//                       of 2 x 256 threads per pair of splits: its two fp64 sums, as (hi, lo) float pairs, fill the workspace slots of two
+//                       splits; a row of one CTA writes its (mean, rstd) itself.
 //               apply   y = [gelu]((x - mean) * rstd * gamma[c] + beta[c])                       read x, write y
 //     backward: reduce  partial S1 = sum g, S2 = sum g * xhat   (g = dy, or dy * gelu'(z))      read x, dy
 //               apply   dx = rstd * gamma[c] * (g - S1 / n - xhat * S2 / n)                      read x, dy, write dx
 //     dgamma[c] = sum_b S2, dbeta[c] = sum_b S1 are formed by the caller from the per-row sums (tiny).
 //   bias + GELU: y = gelu(x + bias[c]);  dx = dy * gelu'(x + bias[c]), per-(row, split) partial sums of dx for dbias.
-// All arithmetic in fp32, activations float or bf16, 16-byte vector accesses when the row length allows it.
+// All other arithmetic in fp32, activations float or bf16, 16-byte vector accesses when the row length allows it.
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace b200sht {
@@ -64,50 +69,65 @@ struct NormArgs {
   const float* beta;   // [C] or null (0): instance-norm shift, or the bias of bias + GELU
   const float* stats;  // [rows][2] mean, rstd
   const float* sums;   // [rows][2] S1, S2 (backward apply)
-  float* partial;      // [rows][splits][2]
+  float* partial;      // [rows][splits][2]; forward statistics: [rows][splits][4], two fp64 sums each stored as a (hi, lo) float pair
+  float* stats_out;    // forward statistics of a one-CTA row: [rows][2] mean, rstd
   long long n;         // elements per row
-  long long chunk;     // elements per split (a multiple of 8)
+  long long chunk;     // elements per split (a multiple of 8); the last split runs to n
   int rows, C, splits, gelu;
+  float eps;
 };
 
-// two block-wide sums (blockDim.x == kNormThreads); result valid in thread 0
-__device__ __forceinline__ void block_sum2(float& a, float& b) {
-  __shared__ float sa[kNormThreads / 32], sb[kNormThreads / 32];
+// two block-wide sums (blockDim.x == NT); result valid in thread 0
+template <int NT, typename A>
+__device__ __forceinline__ void block_sum2(A& a, A& b) {
+  __shared__ A sa[NT / 32], sb[NT / 32];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); b += __shfl_xor_sync(0xffffffffu, b, o); }
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
   if (l == 0) { sa[w] = a; sb[w] = b; }
   __syncthreads();
   if (w == 0) {
-    a = l < kNormThreads / 32 ? sa[l] : 0.f;
-    b = l < kNormThreads / 32 ? sb[l] : 0.f;
+    a = l < NT / 32 ? sa[l] : A(0);
+    b = l < NT / 32 ? sb[l] : A(0);
 #pragma unroll
-    for (int o = 4; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); b += __shfl_xor_sync(0xffffffffu, b, o); }
+    for (int o = NT / 64; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); b += __shfl_xor_sync(0xffffffffu, b, o); }
   }
 }
 
+// (mean, rstd) of a row from the fp64 sums of x - pivot over its n elements
+__device__ __forceinline__ void store_stats(float* out, double pivot, double s0, double s1, long long n, float eps) {
+  const double md = s0 / (double)n;
+  double var = s1 / (double)n - md * md;
+  if (var < 0.0) var = 0.0;
+  out[0] = (float)(pivot + md);
+  out[1] = (float)(1.0 / sqrt(var + (double)eps));
+}
+
 // What a kernel does with one element.  MODE 0: forward statistics, 1: forward apply, 2: backward reduce, 3: backward apply,
-// 4: bias + GELU forward, 5: bias + GELU backward (also accumulates sum dx)
-template <typename T, int MODE, bool VEC>
-__global__ void __launch_bounds__(kNormThreads) norm_kernel(const NormArgs a) {
+// 4: bias + GELU forward, 5: bias + GELU backward (also accumulates sum dx).  NT threads per CTA.
+template <typename T, int MODE, bool VEC, int NT>
+__global__ void __launch_bounds__(NT) norm_kernel(const NormArgs a) {
   const int r = blockIdx.y, s = blockIdx.x;
-  const long long beg = (long long)s * a.chunk, end = beg + a.chunk < a.n ? beg + a.chunk : a.n;
+  const long long beg = (long long)s * a.chunk, end = (s == a.splits - 1 || beg + a.chunk > a.n) ? a.n : beg + a.chunk;
   const T* x = static_cast<const T*>(a.x) + (size_t)r * a.n;
   const T* dy = static_cast<const T*>(a.dy) + (size_t)r * a.n;
   T* out = static_cast<T*>(a.out) + (size_t)r * a.n;
   const int c = r % a.C;
   const float gamma = a.gamma ? a.gamma[c] : 1.f, beta = a.beta ? a.beta[c] : 0.f;
-  float mean = 0.f, rstd = 1.f, pivot = 0.f, m1 = 0.f, m2 = 0.f;
-  if (MODE == 0) pivot = ldf<T>(x, 0);
+  float mean = 0.f, rstd = 1.f, m1 = 0.f, m2 = 0.f;
+  double pivot = 0.0;
+  if (MODE == 0) pivot = (double)ldf<T>(x, 0);
   if (MODE == 1 || MODE == 2 || MODE == 3) { mean = a.stats[2 * r]; rstd = a.stats[2 * r + 1]; }
   if (MODE == 3) { m1 = a.sums[2 * r] / (float)a.n; m2 = a.sums[2 * r + 1] / (float)a.n; }
   const float gs = gamma * rstd;
-  float acc0 = 0.f, acc1 = 0.f;
+  using Acc = typename std::conditional<MODE == 0, double, float>::type;
+  Acc acc0 = 0, acc1 = 0, odd0 = 0, odd1 = 0;   // odd*: a second fp64 chain for the odd elements of a packet (half the dependent latency)
 
-  auto element = [&](float xv, float dv, float& ov) {
+  auto element = [&](float xv, float dv, float& ov, int j) {
     if (MODE == 0) {
-      const float d = xv - pivot;
-      acc0 += d; acc1 = fmaf(d, d, acc1);
+      const double d = (double)xv - pivot;
+      if (j & 1) { odd0 += d; odd1 = fma(d, d, odd1); }
+      else { acc0 += d; acc1 = fma(d, d, acc1); }
     } else if (MODE == 1) {
       const float z = fmaf((xv - mean) * rstd, gamma, beta);
       ov = a.gelu ? gelu_f(z) : z;
@@ -126,7 +146,7 @@ __global__ void __launch_bounds__(kNormThreads) norm_kernel(const NormArgs a) {
   constexpr bool kNeedDy = (MODE == 2 || MODE == 3 || MODE == 5), kWrites = (MODE == 1 || MODE == 3 || MODE == 4 || MODE == 5);
   if (VEC) {
     constexpr int kN = Pack<T>::kN;
-    constexpr long long kStride = (long long)kNormThreads * kN;
+    constexpr long long kStride = (long long)NT * kN;
     long long i = beg + (long long)threadIdx.x * kN;   // beg, n multiples of kN: whole packets
     // two packets per tensor in flight per thread (first measurement of the one-packet loop: 45-50 % of HBM, latency bound at 5 CTAs per SM)
     for (; i + kStride < end; i += 2 * kStride) {
@@ -137,13 +157,13 @@ __global__ void __launch_bounds__(kNormThreads) norm_kernel(const NormArgs a) {
 #pragma unroll
       for (int j = 0; j < kN; ++j) {
         float ov = 0.f;
-        element(px0.get(j), kNeedDy ? pd0.get(j) : 0.f, ov);
+        element(px0.get(j), kNeedDy ? pd0.get(j) : 0.f, ov, j);
         if (kWrites) po0.set(j, ov);
       }
 #pragma unroll
       for (int j = 0; j < kN; ++j) {
         float ov = 0.f;
-        element(px1.get(j), kNeedDy ? pd1.get(j) : 0.f, ov);
+        element(px1.get(j), kNeedDy ? pd1.get(j) : 0.f, ov, j);
         if (kWrites) po1.set(j, ov);
       }
       if (kWrites) { po0.store(out + i); po1.store(out + i + kStride); }
@@ -155,23 +175,32 @@ __global__ void __launch_bounds__(kNormThreads) norm_kernel(const NormArgs a) {
 #pragma unroll
       for (int j = 0; j < kN; ++j) {
         float ov = 0.f;
-        element(px.get(j), kNeedDy ? pd.get(j) : 0.f, ov);
+        element(px.get(j), kNeedDy ? pd.get(j) : 0.f, ov, j);
         if (kWrites) po.set(j, ov);
       }
       if (kWrites) po.store(out + i);
     }
   } else {
-    for (long long i = beg + threadIdx.x; i < end; i += kNormThreads) {
+    for (long long i = beg + threadIdx.x; i < end; i += NT) {
       float ov = 0.f;
-      element(ldf<T>(x, i), kNeedDy ? ldf<T>(dy, i) : 0.f, ov);
+      element(ldf<T>(x, i), kNeedDy ? ldf<T>(dy, i) : 0.f, ov, 0);
       if (kWrites) stf<T>(out, i, ov);
     }
   }
   if (MODE == 0 || MODE == 2 || MODE == 5) {
-    block_sum2(acc0, acc1);
+    acc0 += odd0; acc1 += odd1;
+    block_sum2<NT>(acc0, acc1);
     if (threadIdx.x == 0) {
-      float* p = a.partial + ((size_t)r * a.splits + s) * 2;
-      p[0] = acc0; p[1] = acc1;
+      if (MODE == 0 && a.splits == 1) {
+        store_stats(a.stats_out + 2 * r, pivot, (double)acc0, (double)acc1, a.n, a.eps);
+      } else if (MODE == 0) {
+        float* p = a.partial + ((size_t)r * a.splits + s) * 4;
+        p[0] = (float)acc0; p[1] = (float)(acc0 - (double)p[0]);
+        p[2] = (float)acc1; p[3] = (float)(acc1 - (double)p[2]);
+      } else {
+        float* p = a.partial + ((size_t)r * a.splits + s) * 2;
+        p[0] = (float)acc0; p[1] = (float)acc1;
+      }
     }
   }
 }
@@ -182,15 +211,15 @@ __global__ void norm_finalize_kernel(const float* __restrict__ partial, float* _
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= rows) return;
   double s0 = 0.0, s1 = 0.0;
-  for (int s = 0; s < splits; ++s) { s0 += partial[((size_t)r * splits + s) * 2]; s1 += partial[((size_t)r * splits + s) * 2 + 1]; }
   if (what == 0) {
-    const double pivot = (double)ldf<T>(static_cast<const T*>(x) + (size_t)r * n, 0);
-    const double md = s0 / (double)n;
-    double var = s1 / (double)n - md * md;
-    if (var < 0.0) var = 0.0;
-    out[2 * r] = (float)(pivot + md);
-    out[2 * r + 1] = (float)(1.0 / sqrt(var + (double)eps));
+    for (int s = 0; s < splits; ++s) {
+      const float* p = partial + ((size_t)r * splits + s) * 4;
+      s0 += (double)p[0] + (double)p[1];
+      s1 += (double)p[2] + (double)p[3];
+    }
+    store_stats(out + 2 * r, (double)ldf<T>(static_cast<const T*>(x) + (size_t)r * n, 0), s0, s1, n, eps);
   } else {
+    for (int s = 0; s < splits; ++s) { s0 += partial[((size_t)r * splits + s) * 2]; s1 += partial[((size_t)r * splits + s) * 2 + 1]; }
     out[2 * r] = (float)s0;
     out[2 * r + 1] = (float)s1;
   }
@@ -215,11 +244,12 @@ int norm_splits(int rows, long long n) {
 
 template <typename T, int MODE>
 static int launch_mode(const NormArgs& a, cudaStream_t st) {
+  constexpr int NT = MODE == 0 ? 2 * kNormThreads : kNormThreads;
   const dim3 grid(a.splits, a.rows);
   const bool vec = (a.n % Pack<T>::kN == 0) && ((reinterpret_cast<uintptr_t>(a.x) & 15) == 0) && (a.dy == nullptr || (reinterpret_cast<uintptr_t>(a.dy) & 15) == 0) &&
                    (a.out == nullptr || (reinterpret_cast<uintptr_t>(a.out) & 15) == 0);
-  if (vec) norm_kernel<T, MODE, true><<<grid, kNormThreads, 0, st>>>(a);
-  else norm_kernel<T, MODE, false><<<grid, kNormThreads, 0, st>>>(a);
+  if (vec) norm_kernel<T, MODE, true, NT><<<grid, NT, 0, st>>>(a);
+  else norm_kernel<T, MODE, false, NT><<<grid, NT, 0, st>>>(a);
   B200_CHECK_LAUNCH();
   return 0;
 }
@@ -252,8 +282,12 @@ int instance_norm_forward(const void* x, void* y, const float* gamma, const floa
   int rc = fill_args(&a, B, C, hw);
   if (rc) return rc;
   a.x = x; a.partial = ws;
-  rc = launch_dtype<0>(dtype, a, st);
-  if (!rc) rc = finalize(dtype, ws, stats, x, a.rows, a.splits, hw, eps, 0, st);
+  NormArgs sa = a;   // statistics: one CTA of 2 x 256 threads per pair of splits, the last one also takes an odd split
+  sa.splits = a.splits / 2 > 1 ? a.splits / 2 : 1;
+  sa.chunk = 2 * a.chunk;
+  sa.stats_out = stats; sa.eps = eps;
+  rc = launch_dtype<0>(dtype, sa, st);
+  if (!rc && sa.splits > 1) rc = finalize(dtype, ws, stats, x, a.rows, sa.splits, hw, eps, 0, st);
   a.out = y; a.gamma = gamma; a.beta = beta; a.stats = stats; a.gelu = gelu;
   if (!rc) rc = launch_dtype<1>(dtype, a, st);
   return rc;

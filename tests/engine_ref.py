@@ -31,6 +31,9 @@ FLT_MIN = 2.0 ** -126
 # 3 x TF32 (PREC_FP32X3): per term the omitted lo.lo product (<= 2^-21 |a||b|) and the TF32 rounding of the two residuals
 # (<= 2^-21 + 2^-22): 2^-20 |a||b| in all.  Derived, not calibrated.
 SPLIT_TERM = 2.0 ** -20
+# c for the fp32 CUDA-core kernels whose chains can be as short as one or two products (the SIMT Legendre stages at the last orders, the
+# per-mode mixes): the first-order worst case of a K-term fp32 FMA chain, |err| <= K 2^-24 sum |a||b|.  Derived, not calibrated.
+C_FMA = 1.0
 
 
 # ------------------------------------------------------------------------------------------------- TF32 conversions
@@ -253,3 +256,100 @@ def needed_c(got, ref, mag, K, r=0.0, extra=0.0, floor=0.0):
     den = (1.0 + r) * K * U32 * mag
     c = torch.where(den > 0, err.clamp_min(0) / den, torch.zeros_like(err))
     return float(c.max().item()) if c.numel() else 0.0
+
+
+# --------------------------------------------------------------------------------------------- per-mode channel mixes
+# Native complex weights of the per-mode operators (csrc/mix.cu, mix_permode_kernel):
+#   OP_DIAGONAL [G][Cig][Cog][L][M],   OP_SEP_DIAGONAL [G][Cig][L][M],   OP_SEP_DHCONV [G][Cig][L]   (separable: Ci == Co)
+# K counts real products per output element, as the mix references above: 2 per complex product.
+PERMODE_OPS = ("diagonal", "sep_diagonal", "sep_dhconv")
+
+
+def _permode_apply(op, z, w, G, Cig, Cog, conj_w, dgrad):
+    """sum over the input channel of z * w (or conj(w)) per (l, m), for z complex [L][M][B][Cin] and the native weight"""
+    L, M, B, _ = z.shape
+    wc = w.to(torch.complex128)
+    if conj_w:
+        wc = wc.conj()
+    if op == "diagonal":
+        zg = z.view(L, M, B, G, Cog if dgrad else Cig)
+        eq = "lmbgo,giolm->lmbgi" if dgrad else "lmbgi,giolm->lmbgo"
+        out, mag = _pair(eq, zg, wc)
+        return out.reshape(L, M, B, -1), mag.reshape(L, M, B, -1), 2 * (Cog if dgrad else Cig)
+    wf = wc.reshape(G * Cig, L, -1).permute(1, 2, 0)[:, :, None, :]      # [L][M or 1][1][C]
+    return z * wf, z.abs() * wf.abs(), 2
+
+
+def permode_forward_ref(op, x, w, G, Ci, Co, dense=False):
+    """y[l][m][b][g Cog + o] = sum_i x[l][m][b][g Cig + i] w(g, i, o, l, m) on the stored rows.  x packed spec [L][M][2][B][cpi], w native.
+    Returns (ref, mag, K): packed float64 [L][M][2][B][cpo] (zero in unstored rows and the padding)."""
+    L, M = x.shape[:2]
+    y, mag, K = _permode_apply(op, spec_to_complex(x, Ci, dense), w, G, Ci // G, Co // G, False, False)
+    cpo = (Co + 3) // 4 * 4
+    return complex_to_spec(y, cpo), complex_to_spec(mag, cpo), K
+
+
+def permode_dgrad_ref(op, gy, w, G, Ci, Co, dense=False):
+    """gx[l][m][b][g Cig + i] = sum_o gy[l][m][b][g Cog + o] conj(w(g, i, o, l, m)): the PyTorch complex gradient of permode_forward.
+    Returns (ref, mag, K) packed float64 [L][M][2][B][cpi]."""
+    gx, mag, K = _permode_apply(op, spec_to_complex(gy, Co, dense), w, G, Ci // G, Co // G, True, True)
+    cpi = (Ci + 3) // 4 * 4
+    return complex_to_spec(gx, cpi), complex_to_spec(mag, cpi), K
+
+
+def permode_wgrad_ref(op, x, gy, G, Ci, Co, dense=False):
+    """gw(g, i, o, l, m) = sum over b of conj(x[l][m][b][g Cig + i]) gy[l][m][b][g Cog + o] on the stored rows (OP_SEP_DHCONV: also
+    summed over the stored m of l).  Returns (ref, mag, K): complex128 / float64 in the native layout and K (OP_SEP_DHCONV: [L][1])."""
+    L, M, _, B, _ = x.shape
+    Cig, Cog = Ci // G, Co // G
+    xc = spec_to_complex(x, Ci, dense).conj()
+    gc = spec_to_complex(gy, Co, dense)
+    if op == "diagonal":
+        gw, mag = _pair("lmbgi,lmbgo->giolm", xc.view(L, M, B, G, Cig), gc.view(L, M, B, G, Cog))
+        return gw, mag, 2.0 * B
+    if op == "sep_diagonal":
+        gw, mag = _pair("lmbc,lmbc->clm", xc, gc)
+        return gw.reshape(G, Cig, L, M), mag.reshape(G, Cig, L, M), 2.0 * B
+    gw, mag = _pair("lmbc,lmbc->cl", xc, gc)
+    rows = stored_mask(L, M, 0, dense, device=x.device).sum(1).double() * B
+    return gw.reshape(G, Cig, L), mag.reshape(G, Cig, L), 2 * rows.view(L, 1)
+
+
+# -------------------------------------------------------------------------------------------------------- ComplexReLU
+RELU_MODES = ("real", "cartesian", "modulus", "halfplane")
+
+
+def complex_relu_ref(mode, x, bias, slope, gy, C, dense=False):
+    """ComplexReLU (oracle.complex_relu) of a packed spec x [L][M][2][B][cp] and its PyTorch complex gradient for the output gradient gy, by
+    autograd in complex128 on the exact fp32 inputs.  bias: float [C], a 1-element tensor (one bias for every channel) or None (0).
+    Modulus at z = 0 gives y = 0 and no gradient (the oracle's (|z| + b) z / |z| is 0 / 0 there).
+    Returns complex128 [L][M][B][C] y, gx and the bias gradient (shape of `bias`; None without one)."""
+    from oracle import makani_oracle as O
+
+    z = spec_to_complex(x, C, dense).requires_grad_(True)
+    g = spec_to_complex(gy, C, dense)
+    b = bias.double().requires_grad_(True) if bias is not None else None
+    bb = (b.reshape(-1) if b.numel() > 1 else b.reshape(())) if b is not None else 0.0
+    zero = (z.detach() == 0) if mode == "modulus" else torch.zeros(z.shape, dtype=torch.bool, device=z.device)
+    zs = torch.where(zero, torch.ones((), dtype=z.dtype), z)     # keep 0 / 0 out of the graph
+    y = torch.where(zero, torch.zeros((), dtype=z.dtype), O.complex_relu(zs, mode, bb, slope))
+    inputs = [z] + ([b] if b is not None and mode == "modulus" else [])
+    grads = torch.autograd.grad(y, inputs, grad_outputs=g)
+    gb = grads[1] if len(grads) > 1 else (torch.zeros_like(b) if b is not None else None)
+    return y.detach(), grads[0], gb
+
+
+# ------------------------------------------------------------------------------------------------------ instance norm
+def norm_stats_ref(x):
+    """fp64 mean and 1 / sqrt(var + eps) factor pieces of rows x [rows][n] (any float dtype): (mean, var) float64 [rows]"""
+    xd = x.double()
+    mean = xd.mean(1)
+    return mean, ((xd - mean[:, None]) ** 2).mean(1)
+
+
+def gelu_ref(z):
+    return 0.5 * z * (1.0 + torch.erf(z / 2.0 ** 0.5))
+
+
+def gelu_grad_ref(z):
+    return 0.5 * (1.0 + torch.erf(z / 2.0 ** 0.5)) + z * torch.exp(-0.5 * z * z) / (2.0 * torch.pi) ** 0.5

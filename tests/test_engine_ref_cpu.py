@@ -253,3 +253,83 @@ def test_bound_rejects_one_dropped_term():
     assert E.bound_ratio(E.tf32_rna(dropped), ref, mag, K, r=E.R_TF32) > 1.0
     exact0 = torch.zeros(3, dtype=torch.float64)
     assert E.bound_ratio(torch.tensor([0.0, 0.0, 1e-30]), exact0, exact0, K) == float("inf"), "exact zeros are exact"
+
+
+# ------------------------------------------------------------------------------------------------ per-mode mixes
+# op, L, M, B, G, Ci, Co, dense
+PERMODE_REF_CASES = [("diagonal", 9, 9, 2, 2, 4, 6, False), ("diagonal", 9, 9, 3, 1, 3, 5, True), ("sep_diagonal", 9, 9, 2, 2, 6, 6, False),
+                     ("sep_dhconv", 40, 35, 3, 1, 5, 5, False), ("sep_dhconv", 9, 9, 2, 2, 6, 6, True)]
+
+
+@pytest.mark.parametrize("op,L,M,B,G,Ci,Co,dense", PERMODE_REF_CASES)
+def test_permode_refs_match_oracle_contraction_and_autograd(op, L, M, B, G, Ci, Co, dense):
+    """forward against contractions.py's einsum (oracle.contract_dense) in the native weight layout, dgrad and wgrad against its autograd"""
+    g = torch.Generator().manual_seed(17)
+    Cig, Cog = Ci // G, Co // G
+    shape = {"diagonal": (G, Cig, Cog, L, M), "sep_diagonal": (G, Cig, L, M), "sep_dhconv": (G, Cig, L)}[op]
+    w = torch.randn(*shape, dtype=torch.complex128, generator=g)
+    cpi, cpo = (Ci + 3) // 4 * 4, (Co + 3) // 4 * 4
+    x = torch.randn(L, M, 2, B, cpi, dtype=torch.float64, generator=g)
+    gy = torch.randn(L, M, 2, B, cpo, dtype=torch.float64, generator=g)
+    keep = E.stored_mask(L, M, 0, dense)[:, :, None, None]
+    xo = E.spec_to_complex(x, Ci, dense).permute(2, 3, 0, 1).reshape(B, G, Cig, L, M).requires_grad_(True)
+    wo = w.clone().requires_grad_(True)
+    y = O.contract_dense(xo, wo, separable=op != "diagonal", operator_type="dhconv" if op == "sep_dhconv" else "diagonal")
+    y = torch.where(keep, y.reshape(B, Co, L, M).permute(2, 3, 0, 1), torch.zeros((), dtype=y.dtype))     # [L][M][B][Co]
+    ref, mag, K = E.permode_forward_ref(op, x, w, G, Ci, Co, dense)
+    assert K == (2 * Cig if op == "diagonal" else 2)
+    assert torch.allclose(E.spec_to_complex(ref, Co, dense), y.detach(), atol=1e-12)
+    assert (mag >= ref.abs() - 1e-12).all() and (ref[..., Co:] == 0).all()
+    gx, gw = torch.autograd.grad(y, [xo, wo], grad_outputs=E.spec_to_complex(gy, Co, dense))
+    ref, mag, K = E.permode_dgrad_ref(op, gy, w, G, Ci, Co, dense)
+    assert torch.allclose(E.spec_to_complex(ref, Ci, dense), gx.reshape(B, Ci, L, M).permute(2, 3, 0, 1), atol=1e-12)
+    assert (mag >= ref.abs() - 1e-12).all()
+    ref, mag, K = E.permode_wgrad_ref(op, x, gy, G, Ci, Co, dense)
+    assert ref.shape == w.shape and torch.allclose(ref, gw, atol=1e-12)
+    assert (mag >= ref.abs() - 1e-12).all()
+    if op == "sep_dhconv":
+        assert torch.equal(K.view(-1), 2 * B * E.stored_mask(L, M, 0, dense).sum(1).double())
+
+
+# ---------------------------------------------------------------------------------------------------- ComplexReLU
+@pytest.mark.parametrize("mode", E.RELU_MODES)
+@pytest.mark.parametrize("bias_kind", ["channel", "scalar", "none"])
+def test_complex_relu_ref_matches_finite_differences(mode, bias_kind):
+    """the autograd reference against central differences of the oracle's forward, away from its kinks; modulus at z = 0 gives 0 and no gradient"""
+    g = torch.Generator().manual_seed(5)
+    L, M, B, C, slope = 6, 5, 2, 3, 0.1
+    x = torch.randn(L, M, 2, B, 4, dtype=torch.float64, generator=g)
+    x[2, 1, :, 0, 1] = 0.0
+    gy = torch.randn(L, M, 2, B, 4, dtype=torch.float64, generator=g)
+    bias = {"channel": torch.randn(C, dtype=torch.float64, generator=g) * 0.5, "scalar": torch.tensor([0.3], dtype=torch.float64), "none": None}[bias_kind]
+    y, gx, gb = E.complex_relu_ref(mode, x, bias, slope, gy, C)
+    assert y[2, 1, 0, 1] == 0 and (gx[2, 1, 0, 1] == 0 or mode != "modulus")
+    z = E.spec_to_complex(x, C)
+    gc = E.spec_to_complex(gy, C)
+    bb = 0.0 if bias is None else (bias if bias.numel() > 1 else bias.reshape(()))
+
+    def loss(zz, b):
+        zero = (z == 0) & (mode == "modulus")
+        return (torch.where(zero, torch.zeros((), dtype=zz.dtype), O.complex_relu(zz, mode, b, slope)) * gc.conj()).real.sum()
+
+    h = 1e-6 * (z != 0)    # along every nonzero entry (z = 0 is a kink of every mode)
+    fd = (loss(z + h, bb) - loss(z - h, bb)) / 2e-6 + 1j * (loss(z + 1j * h, bb) - loss(z - 1j * h, bb)) / 2e-6
+    assert torch.allclose(gx[z != 0].sum(), fd.to(gx.dtype), rtol=1e-6, atol=1e-6)
+    if bias is not None and mode == "modulus":
+        fdb = torch.stack([(loss(z, bias + 1e-6 * e) - loss(z, bias - 1e-6 * e)) / 2e-6 for e in torch.eye(bias.numel(), dtype=torch.float64)])
+        assert torch.allclose(gb, fdb, rtol=1e-6, atol=1e-6)
+    elif bias is not None:
+        assert (gb == 0).all()
+
+
+# --------------------------------------------------------------------------------------------------- instance norm
+def test_norm_refs_match_torch():
+    g = torch.Generator().manual_seed(9)
+    x = torch.randn(3, 4, 50, dtype=torch.float64, generator=g) * 2 + 1
+    mean, var = E.norm_stats_ref(x.view(12, 50))
+    ref = torch.nn.functional.instance_norm(x, eps=1e-6)
+    assert torch.allclose(((x.view(12, 50) - mean[:, None]) / torch.sqrt(var[:, None] + 1e-6)).view(3, 4, 50), ref, atol=1e-12)
+    z = torch.linspace(-6, 6, 101, dtype=torch.float64, requires_grad=True)
+    assert torch.allclose(E.gelu_ref(z), torch.nn.functional.gelu(z), atol=1e-14)
+    (gz,) = torch.autograd.grad(torch.nn.functional.gelu(z).sum(), z)
+    assert torch.allclose(E.gelu_grad_ref(z.detach()), gz, atol=1e-14)

@@ -32,10 +32,10 @@ def untouched(t):
     return bool((t.contiguous().view(torch.int32) == SENTINEL).all())
 
 
-def check(case, what, got, ref, mag, K, r=0.0, extra=0.0, floor=0.0):
-    ratio = E.bound_ratio(got, ref, mag, K, r=r, extra=extra, floor=floor)
+def check(case, what, got, ref, mag, K, r=0.0, extra=0.0, floor=0.0, c=E.C_ACC):
+    ratio = E.bound_ratio(got, ref, mag, K, r=r, c=c, extra=extra, floor=floor)
     need = E.needed_c(got, ref, mag, K, r=r, extra=extra, floor=floor)
-    print(f"[engine] {case} {what}: worst ratio {ratio:.3e}, needs c >= {need:.3e} (c = {E.C_ACC})")
+    print(f"[engine] {case} {what}: worst ratio {ratio:.3e}, needs c >= {need:.3e} (c = {c})")
     if ratio > 1.0:
         g, f = (torch.view_as_real(got), torch.view_as_real(ref)) if torch.is_complex(got) else (got, ref)
         err = (g.double() - f).abs().flatten()
@@ -59,6 +59,8 @@ LEG_CASES = [
     ("ltiles128+1-kp136-PBc3", "legendre-gauss", 129, 256, 129, 129, 2, 73, None),
     ("B32-two-pbtiles-JP512", "equiangular", 91, 180, 91, 91, 32, 8, None),
     ("nct2-JP400", "legendre-gauss", 64, 128, 64, 65, 1, 200, None),
+    ("JP152-ragged-coltile-C73", "legendre-gauss", 64, 128, 64, 65, 1, 73, None),
+    ("L65-lstart32-ltile-tail", "equiangular", 65, 128, 65, 65, 3, 6, None),
     ("headline-23kblocks-tail17", "equiangular", 721, 1440, 240, 241, 1, 3, None),
     ("m0=23", "equiangular", 65, 128, 40, 45 - 23, 2, 5, 23),
     ("m0=32", "equiangular", 65, 128, 40, 45 - 32, 2, 5, 32),
@@ -72,7 +74,7 @@ def _plan(grid, nlat, nlon, L, M, m0):
     return Plan.create_ex(nlat, nlon, L, M, m0, 0, cost, w, True, DEV), m0
 
 
-def check_spec(case, what, sv, ref, mag, K, C, m0=0, dense=False, r=0.0, extra=0.0, zeros=True, floor=0.0):
+def check_spec(case, what, sv, ref, mag, K, C, m0=0, dense=False, r=0.0, extra=0.0, zeros=True, floor=0.0, c=E.C_ACC):
     """packed spec output [L][M][2][B][cp]: unstored entries untouched, stored ones in the bound (the padding channels and, with
     `zeros`, the l < m entries exact zeros)"""
     L, M = sv.shape[:2]
@@ -81,23 +83,28 @@ def check_spec(case, what, sv, ref, mag, K, C, m0=0, dense=False, r=0.0, extra=0
     assert (sv[st][..., C:] == 0).all(), f"{case} {what}: channel padding must hold exact zeros"
     if zeros:
         assert (sv[E.zero_mask(L, M, m0, dense, device=DEV)] == 0).all(), f"{case} {what}: l < m entries must be exact zeros"
-    check(case, what, sv[st], ref[st], mag[st], K, r=r, extra=extra, floor=floor)
+    check(case, what, sv[st], ref[st], mag[st], K, r=r, extra=extra, floor=floor, c=c)
 
 
-@pytest.mark.parametrize("prec", [TF32, X3], ids=["tf32", "fp32x3"])
+@pytest.mark.parametrize("prec", [TF32, X3, FP32], ids=["tf32", "fp32x3", "fp32"])
 @pytest.mark.parametrize("case,grid,nlat,nlon,L,M,B,C,m0", LEG_CASES, ids=[c[0] for c in LEG_CASES])
 def test_legendre_engine(case, grid, nlat, nlon, L, M, B, C, m0, prec):
+    """TF32 and 3 x TF32 on the tensor-core engine; FP32 on the CUDA-core kernels (64 x 64 output tiles, 16-deep k / l slabs), held to
+    the same bound with the fp32 table and operands as they are"""
     plan, m0 = _plan(grid, nlat, nlon, L, M, m0)
-    assert plan.umma_ok, "tensor-core path unavailable"
+    if prec != FP32:
+        assert plan.umma_ok, "tensor-core path unavailable"
     kp, cp = plan.kp, (C + 3) // 4 * 4
     split = prec == X3
+    tf32 = prec == TF32
     st = _stream(DEV)
     gen = torch.Generator(device=DEV).manual_seed(1234)
-    T = plan.table() if split else E.tf32_rna(plan.table())
-    rnd = (lambda *s: torch.randn(*s, device=DEV, generator=gen)) if split else (lambda *s: E.rand_tf32(*s, device=DEV, generator=gen))
-    tag = f"{case} {'fp32x3' if split else 'tf32'}"
+    T = E.tf32_rna(plan.table()) if tf32 else plan.table()
+    rnd = (lambda *s: E.rand_tf32(*s, device=DEV, generator=gen)) if tf32 else (lambda *s: torch.randn(*s, device=DEV, generator=gen))
+    tag = f"{case} {'fp32x3' if split else 'tf32' if tf32 else 'fp32'}"
     extra = E.SPLIT_TERM if split else 0.0
     kmul = 3 if split else 1   # hi.hi + hi.lo + lo.hi into one accumulator
+    c = E.C_ACC if prec != FP32 else E.C_FMA
 
     # analysis: latspec [M8][2][B][C][kp] with NaN in the latitude padding and the padding orders
     lat = torch.full((plan.latspec_elems(B, C),), float("nan"), device=DEV)
@@ -106,8 +113,8 @@ def test_legendre_engine(case, grid, nlat, nlon, L, M, B, C, m0, prec):
     spec = sentinel(plan.spec_elems(B, C))
     call("b200sht_legendre_analysis", plan.handle, _ptr(lat), _ptr(spec), B, C, prec, st)
     ref, mag = E.legendre_analysis_ref(T, X, nlat, cp, m0)
-    check_spec(tag, "analysis", spec.view(L, M, 2, B, cp), ref, mag, kmul * nlat, C, m0, r=0.0 if split else E.R_TF32, extra=extra,
-               floor=E.underflow_floor(kmul * nlat, X[..., :nlat]))
+    check_spec(tag, "analysis", spec.view(L, M, 2, B, cp), ref, mag, kmul * nlat, C, m0, r=E.R_TF32 if tf32 else 0.0, extra=extra,
+               floor=E.underflow_floor(kmul * nlat, X[..., :nlat]), c=c)
 
     # synthesis: spec with NaN in the unstored region, zeros where l < m and in the channel padding
     S = rnd(L, M, 2, B, cp)
@@ -122,8 +129,8 @@ def test_legendre_engine(case, grid, nlat, nlon, L, M, B, C, m0, prec):
     Zv = Z[:n].view(M, 2, B, C, kp)
     assert (Zv[..., nlat:] == 0).all(), f"{tag}: latitude padding rows must be exact zeros"
     floor = E.underflow_floor(kmul * L, S)
-    check(tag, "synthesis", Zv, ref, mag, kmul * K, extra=extra, floor=floor)
-    if not split and plan.dft_ok:
+    check(tag, "synthesis", Zv, ref, mag, kmul * K, extra=extra, floor=floor, c=c)
+    if tf32 and plan.dft_ok:
         Zt = sentinel(plan.latspec_elems(B, C))
         call("b200sht_legendre_synthesis_tiled", plan.handle, _ptr(S), _ptr(Zt), B, C, st)
         R = B * C

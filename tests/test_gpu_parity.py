@@ -367,7 +367,7 @@ def test_complex_relu_matches_reference_golden():
         assert torch.allclose(y, torch.from_numpy(g[f"relu_{mode}"]) * tri, atol=1e-6, rtol=1e-5), mode
 
 
-@pytest.mark.parametrize("op,act", [("diagonal", "real"), ("l-dependant", "cartesian"), ("diagonal", "modulus")])
+@pytest.mark.parametrize("op,act", [("diagonal", "real"), ("l-dependant", "cartesian"), ("diagonal", "modulus"), ("diagonal", "halfplane")])
 def test_spectral_attention_intended_semantics(op, act):
     torch.manual_seed(333)
     f = mb.RealSHT(32, 64, 16, 17, "legendre-gauss", precision="fp32")
@@ -380,7 +380,7 @@ def test_spectral_attention_intended_semantics(op, act):
     ws = [w.detach().cpu().to(torch.complex128).requires_grad_(True) for w in att.w]
     wo = att.wout.detach().cpu().to(torch.complex128).requires_grad_(True)
     bs = [b.detach().cpu().to(torch.complex128).requires_grad_(True) for b in att.b]
-    ab = [a.bias.detach().cpu().double() if isinstance(a.bias, torch.Tensor) else 0.0 for a in att.activations]
+    ab = [a.bias.detach().cpu().double().requires_grad_(True) if isinstance(a.bias, torch.Tensor) else 0.0 for a in att.activations]
     xr = x.double().requires_grad_(True)
     yr, _ = O.spectral_attention_forward(xr, ws, wo, of, oi, b_list=bs, act_mode=act, act_bias=ab, operator_type=op)
     close(y, yr, 1e-5, f"SpectralAttention[{op},{act}] y")
@@ -391,6 +391,9 @@ def test_spectral_attention_intended_semantics(op, act):
     close(att.wout.grad, wo.grad, 2e-5, "dwout")
     close(att.w[0].grad, ws[0].grad, 2e-5, "dw0")
     close(att.b[1].grad, bs[1].grad, 2e-5, "db1")
+    for k, (a, r) in enumerate(zip(att.activations, ab)):
+        if isinstance(a.bias, torch.Tensor):
+            close(a.bias.grad, r.grad if r.grad is not None else torch.zeros_like(r), 2e-5, f"activation {k} bias grad")
 
 
 # ----------------------------------------------------------------- size-independent properties at BASELINE sizes
