@@ -4,6 +4,7 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     RealSHT, InverseRealSHT                    <- torch_harmonics.{RealSHT, InverseRealSHT}
     RealVectorSHT, InverseRealVectorSHT        <- torch_harmonics.{RealVectorSHT, InverseRealVectorSHT} (makani's vort/div and gradient losses)
     DiscreteContinuousConvS2                   <- torch_harmonics.DiscreteContinuousConvS2 (FCN3's encoders, decoders and local blocks; morlet basis)
+    DiscreteContinuousConvTransposeS2          <- torch_harmonics.DiscreteContinuousConvTransposeS2 (learnable upsampling; morlet basis)
     ResampleS2                                 <- torch_harmonics.ResampleS2 (FCN3's and SNO's decoders; mode "bilinear")
     SpectralConv, SpectralAttention, ComplexReLU <- makani.models.common.*
     quadrature                                 <- torch_harmonics.quadrature
@@ -17,7 +18,7 @@ from ._lib import B200ShtError, load as load_library  # noqa: F401
 from . import quadrature  # noqa: F401
 from .sht import RealSHT, InverseRealSHT, get_plan, resolve_precision  # noqa: F401
 from .vector_sht import RealVectorSHT, InverseRealVectorSHT  # noqa: F401
-from .disco import DiscreteContinuousConvS2  # noqa: F401
+from .disco import DiscreteContinuousConvS2, DiscreteContinuousConvTransposeS2  # noqa: F401
 from .resample import ResampleS2  # noqa: F401
 from .spectral_convolution import SpectralConv, SpectralAttention, ComplexReLU, mix_packed  # noqa: F401
 from .host_pipeline import HostFeed  # noqa: F401

@@ -25,7 +25,7 @@ def install_torch_harmonics_shim(force=False):
         raise RuntimeError("a real torch_harmonics is already imported; pass force=True to replace it")
     import makani_b200 as mb
     from makani_b200 import disco as mbdisco
-    from makani_b200 import distributed as mbd   # with DistributedDiscreteContinuousConvS2 and DistributedResampleS2
+    from makani_b200 import distributed as mbd   # with the distributed DISCO convolutions and DistributedResampleS2
     from makani_b200 import quadrature as mbq
 
     th = types.ModuleType("torch_harmonics")
@@ -36,6 +36,7 @@ def install_torch_harmonics_shim(force=False):
     th.RealVectorSHT = mb.RealVectorSHT
     th.InverseRealVectorSHT = mb.InverseRealVectorSHT
     th.DiscreteContinuousConvS2 = mb.DiscreteContinuousConvS2
+    th.DiscreteContinuousConvTransposeS2 = mb.DiscreteContinuousConvTransposeS2
     th.ResampleS2 = mb.ResampleS2
     fb = types.ModuleType("torch_harmonics.filter_basis")
     fb.get_filter_basis, fb.MorletFilterBasis = mbdisco.get_filter_basis, mbdisco.MorletFilterBasis

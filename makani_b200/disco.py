@@ -10,6 +10,9 @@ section 5) and held by output latitude in CSR form.  The library's plan keeps it
 X = contraction(x) of shape (B, C_in, K, *out_shape) is a grouped GEMM on cuBLAS (torch.matmul; TF32 follows torch.backends.cuda.matmul.allow_tf32).
 The backward recomputes X for the weight gradient rather than keeping it (X is K times the activation) and returns dx = adjoint(W^T dy).
 
+DiscreteContinuousConvTransposeS2 (drop-in for `torch_harmonics.DiscreteContinuousConvTransposeS2`, same constructor) runs the same two kernels
+the other way round on a plan of the swapped geometry: its forward is the adjoint kernel after the GEMM, its backward the forward kernel.
+
 Only the "morlet" basis is implemented; "piecewise linear", "zernike", "harmonic" and the "nodal" norm mode raise NotImplementedError, and
 theta_cutoff=None raises ValueError (every makani call site passes it).
 """
@@ -73,8 +76,13 @@ def get_filter_basis(kernel_shape, basis_type):
 DiscoPsi = namedtuple("DiscoPsi", "row_ptr ker col val nlat_in nlon_in nlat_out nlon_out kernel_size")
 
 
-def precompute_psi(kernel_shape, basis_type, basis_norm_mode, in_shape, out_shape, grid_in, grid_out, theta_cutoff):
-    """psi_hat in fp64 as DiscoPsi.  Every grid point with r <= (1 + 1e-3) theta_cutoff is present for every k (zeros of the basis included)."""
+def precompute_psi(kernel_shape, basis_type, basis_norm_mode, in_shape, out_shape, grid_in, grid_out, theta_cutoff, transpose=False):
+    """psi_hat in fp64 as DiscoPsi.  Every grid point with r <= (1 + 1e-3) theta_cutoff is present for every k (zeros of the basis included).
+
+    transpose=True gives psi_T of DiscreteContinuousConvTransposeS2 on this (swapped) geometry: the same support and basis values, with
+    torch-harmonics' transpose normalisation.  Its sums run over the entries of each input row i, weighted by the quadrature of their centre
+    row t: v[k, i] = sum |psi| 2 pi w_out[t] / nlon_in, the support a[i] = sum 2 pi w_out[t] / nlon_in, and
+    psi_T = psi 2 pi w_out[t] / nlon_out / (d[k, i] + 1e-9)."""
     basis = get_filter_basis(kernel_shape, basis_type)
     if basis_norm_mode not in NORM_MODES:
         if basis_norm_mode == "nodal":
@@ -85,7 +93,7 @@ def precompute_psi(kernel_shape, basis_type, basis_norm_mode, in_shape, out_shap
         raise ValueError(f"nlon_in {nlon_in} must be a multiple of nlon_out {nlon_out}")
     K = basis.kernel_size
     cost_in, w_in = _grid_np(nlat_in, grid_in)
-    cost_out, _ = _grid_np(nlat_out, grid_out)
+    cost_out, w_out = _grid_np(nlat_out, grid_out)
     th_in, th_out = np.arccos(np.clip(cost_in, -1, 1)), np.arccos(np.clip(cost_out, -1, 1))
     phi = 2.0 * np.pi * np.arange(nlon_in) / nlon_in
     q = 2.0 * np.pi * w_in / nlon_in
@@ -106,22 +114,33 @@ def precompute_psi(kernel_shape, basis_type, basis_norm_mode, in_shape, out_shap
         ii_abs = rows[ii]
         per_t.append((ii_abs, jj, basis(r[ii, jj] / rc, bearing[ii, jj])))
 
-    v = np.stack([np.sum(np.abs(p) * q[i], axis=1) for i, _, p in per_t], axis=1)   # (K, nlat_out)
-    s = np.array([np.sum(q[i]) for i, _, _ in per_t])
+    if transpose:
+        qc = 2.0 * np.pi * w_out / nlon_in                                 # quadrature of the centre rows, in the sums of v and a
+        v, s = np.zeros((K, nlat_in)), np.zeros(nlat_in)                   # (K, nlat_in), (nlat_in,)
+        for t, (i, _, p) in enumerate(per_t):
+            v += np.stack([np.bincount(i, np.abs(pk), nlat_in) for pk in p]) * qc[t]
+            s += np.bincount(i, minlength=nlat_in) * qc[t]
+    else:
+        v = np.stack([np.sum(np.abs(p) * q[i], axis=1) for i, _, p in per_t], axis=1)   # (K, nlat_out)
+        s = np.array([np.sum(q[i]) for i, _, _ in per_t])
+    nrow = v.shape[1]
     if basis_norm_mode == "mean":
-        d = np.repeat(v.mean(axis=1, keepdims=True), nlat_out, axis=1)
+        d = np.repeat(v.mean(axis=1, keepdims=True), nrow, axis=1)
     elif basis_norm_mode == "individual":
         d = v
     elif basis_norm_mode == "support":
         d = np.repeat(s[None, :], K, axis=0)
     else:
-        d = np.ones((K, nlat_out))
+        d = np.ones((K, nrow))
 
     row_ptr = np.zeros(nlat_out + 1, dtype=np.int64)
     ker, col, val = [], [], []
     for t, (i, j, p) in enumerate(per_t):
         n = len(i)
-        vals = p * q[i][None, :] / (d[:, t : t + 1] + NORM_EPS)          # (K, n), points already in (i, j) order
+        if transpose:
+            vals = p * (2.0 * np.pi * w_out[t] / nlon_out) / (d[:, i] + NORM_EPS)
+        else:
+            vals = p * q[i][None, :] / (d[:, t : t + 1] + NORM_EPS)      # (K, n), points already in (i, j) order
         ker.append(np.tile(np.arange(K, dtype=np.int32), n))
         col.append(np.repeat((i * nlon_in + j).astype(np.int32), K))
         val.append(vals.T.reshape(-1))
@@ -185,12 +204,13 @@ class DiscoPlan:
 _psi_cache, _plan_cache, _cache_lock = {}, {}, threading.Lock()
 
 
-def _psi_key(kernel_shape, basis_type, basis_norm_mode, in_shape, out_shape, grid_in, grid_out, theta_cutoff):
-    return (tuple(kernel_shape), basis_type, basis_norm_mode, tuple(in_shape), tuple(out_shape), grid_in, grid_out, float(theta_cutoff))
+def _psi_key(kernel_shape, basis_type, basis_norm_mode, in_shape, out_shape, grid_in, grid_out, theta_cutoff, transpose=False):
+    key = (tuple(kernel_shape), basis_type, basis_norm_mode, tuple(in_shape), tuple(out_shape), grid_in, grid_out, float(theta_cutoff))
+    return key + (True,) if transpose else key
 
 
 def get_psi(*key):
-    """precompute_psi, cached per (kernel shape, basis, norm mode, geometry, cutoff)"""
+    """precompute_psi, cached per (kernel shape, basis, norm mode, geometry, cutoff[, transpose])"""
     with _cache_lock:
         if key not in _psi_cache:
             _psi_cache[key] = precompute_psi(*key)
@@ -253,16 +273,58 @@ class _DiscoConv(torch.autograd.Function):
         return dx, dw, db, None, None
 
 
-class DiscreteContinuousConvS2(nn.Module):
-    """Discrete-continuous convolution on the sphere (drop-in for torch_harmonics.DiscreteContinuousConvS2).
+def _transposed_mix(W, G):
+    """(C_out, C_in/G, K) -> (G, C_out/G * K, C_in/G): the channel mix of the transposed convolution, rows (o, k)"""
+    Wg = _grouped(W, G)
+    return Wg.view(G, Wg.shape[1], W.shape[1], W.shape[2]).transpose(2, 3).reshape(G, -1, W.shape[1])
 
-    weight (C_out, C_in / groups, K), initialised sqrt(1 / (C_in / groups) / K) randn; bias (C_out,) zeros.  psi_hat is not part of the state dict."""
+
+class _DiscoConvTranspose(torch.autograd.Function):
+    """y = adjoint(Y) (+ bias), Y = W_g^T-mix of x with K-fold rows (o, k).  Saves x and W only; the backward's gY = plan.forward(gy)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, plan, groups):
+        B, C_out = x.shape[0], weight.shape[0]
+        Y = torch.matmul(_transposed_mix(weight.to(torch.float32), groups),
+                         x.to(torch.float32).view(B, groups, -1, plan.nlat_out * plan.nlon_out))   # (B, G, C_out/G * K, HW_in)
+        y = plan.adjoint(Y.view(B, C_out, plan.K, plan.nlat_out, plan.nlon_out))
+        if bias is not None:
+            y = y + bias.to(torch.float32).view(1, -1, 1, 1)
+        ctx.save_for_backward(x, weight)
+        ctx.plan, ctx.groups, ctx.has_bias = plan, groups, bias is not None
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        x, weight = ctx.saved_tensors
+        plan, G = ctx.plan, ctx.groups
+        B, C, HW = x.shape[0], x.shape[1], plan.nlat_out * plan.nlon_out
+        gy = gy.to(torch.float32).contiguous()
+        dx = dw = db = None
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+            gY = plan.forward(gy).view(B, G, -1, HW)                                             # (B, G, C_out/G * K, HW_in)
+            Wt = _transposed_mix(weight.to(torch.float32), G)
+        if ctx.needs_input_grad[0]:
+            dx = torch.matmul(Wt.transpose(1, 2), gY).view(x.shape).to(x.dtype)
+        if ctx.needs_input_grad[1]:
+            dWt = torch.matmul(gY, x.to(torch.float32).view(B, G, -1, HW).transpose(2, 3)).sum(0)   # (G, C_out/G * K, C_in/G)
+            dw = dWt.view(G, -1, plan.K, C // G).transpose(2, 3).reshape(weight.shape).to(weight.dtype)
+        if ctx.has_bias and ctx.needs_input_grad[2]:
+            db = gy.sum(dim=(0, 2, 3))
+        return dx, dw, db, None, None
+
+
+class _DiscreteContinuousConv(nn.Module):
+    """The constructor, attributes, parameters and plan of both DISCO convolutions; `_transpose` selects the geometry of psi_hat."""
+
+    _transpose = False
 
     def __init__(self, in_channels, out_channels, in_shape, out_shape, kernel_shape, basis_type="piecewise linear", basis_norm_mode="mean",
                  groups=1, grid_in="equiangular", grid_out="equiangular", bias=True, theta_cutoff=None):
         super().__init__()
         if theta_cutoff is None:
-            raise ValueError("DiscreteContinuousConvS2 needs an explicit theta_cutoff (the default cutoff is not implemented)")
+            name = "DiscreteContinuousConvTransposeS2" if self._transpose else "DiscreteContinuousConvS2"
+            raise ValueError(f"{name} needs an explicit theta_cutoff (the default cutoff is not implemented)")
         if theta_cutoff <= 0:
             raise ValueError(f"theta_cutoff must be positive, got {theta_cutoff}")
         basis = get_filter_basis(kernel_shape, basis_type)
@@ -274,7 +336,9 @@ class DiscreteContinuousConvS2(nn.Module):
             raise ValueError(f"in_channels {in_channels} and out_channels {out_channels} must be divisible by groups {groups}")
         self.nlat_in, self.nlon_in = in_shape
         self.nlat_out, self.nlon_out = out_shape
-        if self.nlon_in % self.nlon_out:
+        if self._transpose and self.nlon_out % self.nlon_in:
+            raise ValueError(f"nlon_out {self.nlon_out} must be a multiple of nlon_in {self.nlon_in}")
+        if not self._transpose and self.nlon_in % self.nlon_out:
             raise ValueError(f"nlon_in {self.nlon_in} must be a multiple of nlon_out {self.nlon_out}")
         self.in_channels, self.out_channels = in_channels, out_channels
         self.kernel_shape, self.basis_type, self.basis_norm_mode = basis.kernel_shape, basis_type, basis_norm_mode
@@ -282,7 +346,10 @@ class DiscreteContinuousConvS2(nn.Module):
         self.kernel_size = basis.kernel_size
         self.groups = groups
         self.groupsize = in_channels // groups
-        self._key = _psi_key(self.kernel_shape, basis_type, basis_norm_mode, in_shape, out_shape, grid_in, grid_out, theta_cutoff)
+        if self._transpose:     # psi_T lives on the geometry of the forward convolution from the out grid to the in grid
+            self._key = _psi_key(self.kernel_shape, basis_type, basis_norm_mode, out_shape, in_shape, grid_out, grid_in, theta_cutoff, True)
+        else:
+            self._key = _psi_key(self.kernel_shape, basis_type, basis_norm_mode, in_shape, out_shape, grid_in, grid_out, theta_cutoff)
         psi = get_psi(*self._key)
         # psi_hat (CSR by output latitude) as non-persistent buffers: a state dict holds only weight / bias
         self.register_buffer("psi_row_ptr", torch.from_numpy(psi.row_ptr), persistent=False)
@@ -301,19 +368,43 @@ class DiscreteContinuousConvS2(nn.Module):
     def plan(self, device):
         return get_plan(self._key, device)
 
-    def forward(self, x):
+    def _check_input(self, x):
         if not x.is_cuda:
-            raise B200ShtError("DiscreteContinuousConvS2 runs on CUDA devices only; makani_b200 has no CPU fallback")
+            raise B200ShtError(f"{type(self).__name__} runs on CUDA devices only; makani_b200 has no CPU fallback")
         if x.dim() != 4 or x.shape[1] != self.in_channels or tuple(x.shape[2:]) != (self.nlat_in, self.nlon_in):
             raise ValueError(f"expected (B, {self.in_channels}, {self.nlat_in}, {self.nlon_in}), got {tuple(x.shape)}")
-        if x.dtype not in (torch.float32, torch.bfloat16):
-            x = x.to(torch.float32)
-        return _DiscoConv.apply(x.contiguous(), self.weight, self.bias, self.plan(x.device), self.groups)
+        return (x if x.dtype in (torch.float32, torch.bfloat16) else x.to(torch.float32)).contiguous()
+
+
+class DiscreteContinuousConvS2(_DiscreteContinuousConv):
+    """Discrete-continuous convolution on the sphere (drop-in for torch_harmonics.DiscreteContinuousConvS2).
+
+    weight (C_out, C_in / groups, K), initialised sqrt(1 / (C_in / groups) / K) randn; bias (C_out,) zeros.  psi_hat is not part of the state dict."""
+
+    def forward(self, x):
+        return _DiscoConv.apply(self._check_input(x), self.weight, self.bias, self.plan(x.device), self.groups)
+
+
+class DiscreteContinuousConvTransposeS2(_DiscreteContinuousConv):
+    """Transposed discrete-continuous convolution on the sphere (drop-in for torch_harmonics.DiscreteContinuousConvTransposeS2), for learnable
+    upsampling: x (B, C_in, *in_shape) -> float32 (B, C_out, *out_shape), nlon_out a multiple of nlon_in.
+
+        Y[b, o, k, t, p] = sum_c W[o, c, k] x[b, g(o) C_in / G + c, t, p]              (grouped GEMM on cuBLAS)
+        y[b, o, i, j']  = sum_{k, t, p} psi_T[k, t, i, (j' - s p) mod nlon_out] Y[b, o, k, t, p] (+ bias[o]),  s = nlon_out / nlon_in
+
+    psi_T is the filter tensor of the forward convolution from the out grid to the in grid with torch-harmonics' transpose normalisation
+    (`precompute_psi(..., transpose=True)`), so the contraction above is the adjoint kernel of that plan and the backward's gY is its forward
+    kernel.  Constructor, attributes and parameters as DiscreteContinuousConvS2; weight (C_out, C_in / groups, K)."""
+
+    _transpose = True
+
+    def forward(self, x):
+        return _DiscoConvTranspose.apply(self._check_input(x), self.weight, self.bias, self.plan(x.device), self.groups)
 
 
 def __getattr__(name):
     # the distributed module lives in makani_b200/distributed/disco.py; the reference runners import it from here
-    if name == "DistributedDiscreteContinuousConvS2":
-        from .distributed.disco import DistributedDiscreteContinuousConvS2
-        return DistributedDiscreteContinuousConvS2
+    if name in ("DistributedDiscreteContinuousConvS2", "DistributedDiscreteContinuousConvTransposeS2"):
+        from .distributed import disco
+        return getattr(disco, name)
     raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

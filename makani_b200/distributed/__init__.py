@@ -16,7 +16,8 @@ channels, the longitude stages see the 2C component rows and the Legendre stage 
 (B200SHT_PLAN_VECTOR with an order offset, `b200sht_vector_*`).
 
 DistributedDiscreteContinuousConvS2 (distributed/disco.py: a latitude halo and window plans of psi_hat) and DistributedResampleS2
-(distributed/resample.py: whole spheres of a subset of planes) are FCN3's local operators under the same h x w grid.
+(distributed/resample.py: whole spheres of a subset of planes) are FCN3's local operators under the same h x w grid;
+DistributedDiscreteContinuousConvTransposeS2 runs the DISCO stages the other way round.
 """
 import ctypes
 
@@ -487,5 +488,5 @@ class DistributedInverseRealVectorSHT(_DistributedBase):
         return y if x.dim() == 5 else y.reshape(*lead, 2, self.nlat_local, self.nlon_local)
 
 
-from .disco import DistributedDiscreteContinuousConvS2, set_disco_local_ops  # noqa: E402,F401
+from .disco import DistributedDiscreteContinuousConvS2, DistributedDiscreteContinuousConvTransposeS2, set_disco_local_ops  # noqa: E402,F401
 from .resample import DistributedResampleS2, set_resample_local_ops  # noqa: E402,F401

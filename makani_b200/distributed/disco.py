@@ -13,6 +13,9 @@ the forward kernel then sums every element of X over the same points in the same
 corresponding slice of the single-GPU X.  As the serial module, the backward recomputes X (kernel + one azimuth all-to-all) rather than
 keeping it; only the window of x is saved.  The per-rank stages are replaceable (`set_disco_local_ops`) so the choreography is unit-tested on
 CPU with gloo against the serial oracle.
+
+DistributedDiscreteContinuousConvTransposeS2 runs the same stages the other way round on the windows of its psi_T plan, whose output rows
+are the module's input latitudes: the backward chain above as its forward, the forward chain as its backward.
 """
 import threading
 from collections import namedtuple
@@ -21,7 +24,7 @@ import numpy as np
 import torch
 
 from .._lib import B200ShtError
-from ..disco import DiscoPlan, DiscoPsi, DiscreteContinuousConvS2, _grouped, get_psi
+from ..disco import DiscoPlan, DiscoPsi, DiscreteContinuousConvS2, DiscreteContinuousConvTransposeS2, _grouped, _transposed_mix, get_psi
 from .primitives import _all_to_all, _transpose, compute_split_shapes
 
 # output rows [t0, t1) of a rank, its input window [lo, hi) and the entries of those output rows (input rows re-indexed to i - lo)
@@ -165,12 +168,7 @@ class _DistDiscoConv(torch.autograd.Function):
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
             dX = torch.matmul(_grouped(weight.to(torch.float32), G).transpose(1, 2), gyg).view(B * C, K, m.nlat_out_local, m.nlon_out_local)
-            if m.comm_size_azimuth > 1:
-                dX = _a2a(dX, 0, 3, m.lon_out_shapes, m.azimuth_group)
-            g = halo_adjoint(m._ops.adjoint(dX).to(torch.float32), m._halo_send, m._halo_recv, m.nlat_in_local, m.polar_group)
-            if m.comm_size_azimuth > 1:
-                g = _a2a(g, 2, 0, compute_split_shapes(B * C, m.comm_size_azimuth), m.azimuth_group)
-            dx = g.view(B, C, m.nlat_in_local, m.nlon_in_local).to(ctx.x_dtype)
+            dx = m._pixels(m._window_adjoint(dX), B * C).view(B, C, m.nlat_in_local, m.nlon_in_local).to(ctx.x_dtype)
         if ctx.needs_input_grad[1]:
             X = m._pixels(m._ops.contract(xwin), B * C).view(B, G, -1, P)
             dw = torch.matmul(gyg, X.transpose(2, 3)).sum(0).reshape(weight.shape).to(weight.dtype)
@@ -179,20 +177,13 @@ class _DistDiscoConv(torch.autograd.Function):
         return dx, dw, db, None
 
 
-class DistributedDiscreteContinuousConvS2(DiscreteContinuousConvS2):
-    """DISCO convolution under h x w spatial model parallelism: the constructor, attributes, weight (C_out, C_in / groups, K) and bias of
-    DiscreteContinuousConvS2, not sharded (makani tags them is_shared_mp = ["spatial"] and all-reduces their gradients).  The groups are
-    makani_b200.distributed.polar_group() (latitudes) and azimuth_group() (longitudes), read at construction; a grid of one rank is refused."""
+class _SpatialGrid:
+    """The h x w process grid of both distributed DISCO convolutions: groups, split shapes, local shapes, the windows of the plan's output
+    rows and the halo over its input rows, and the two data movements around the window contraction.  The plan's output rows are the module's
+    output latitudes, and for the transposed convolution (`_transpose`) its input latitudes."""
 
-    def __init__(self, in_channels, out_channels, in_shape, out_shape, kernel_shape, basis_type="piecewise linear", basis_norm_mode="mean",
-                 groups=1, grid_in="equiangular", grid_out="equiangular", bias=True, theta_cutoff=None):
+    def _init_grid(self):
         from . import _rank, _size, azimuth_group, polar_group
-        if _size(polar_group()) * _size(azimuth_group()) == 1:
-            raise NotImplementedError("DistributedDiscreteContinuousConvS2 needs a process grid of more than one rank (the distributed DISCO "
-                                      "convolution splits latitudes over makani_b200.distributed.polar_group() and longitudes over "
-                                      "azimuth_group()); at spatial model parallelism 1 use DiscreteContinuousConvS2")
-        super().__init__(in_channels, out_channels, in_shape, out_shape, kernel_shape, basis_type, basis_norm_mode, groups, grid_in, grid_out,
-                         bias, theta_cutoff)
         self.polar_group, self.azimuth_group = polar_group(), azimuth_group()
         self.comm_size_polar, self.comm_rank_polar = _size(self.polar_group), _rank(self.polar_group)
         self.comm_size_azimuth, self.comm_rank_azimuth = _size(self.azimuth_group), _rank(self.azimuth_group)
@@ -200,29 +191,66 @@ class DistributedDiscreteContinuousConvS2(DiscreteContinuousConvS2):
         self.lat_in_shapes, self.lon_in_shapes = compute_split_shapes(self.nlat_in, h), compute_split_shapes(self.nlon_in, w)
         self.lat_out_shapes, self.lon_out_shapes = compute_split_shapes(self.nlat_out, h), compute_split_shapes(self.nlon_out, w)
         if min(self.lat_in_shapes + self.lat_out_shapes) < 1 or min(self.lon_in_shapes + self.lon_out_shapes) < 1:
-            raise ValueError(f"grids {in_shape} -> {out_shape} are too small for {h} x {w} ranks")
+            raise ValueError(f"grids {(self.nlat_in, self.nlon_in)} -> {(self.nlat_out, self.nlon_out)} are too small for {h} x {w} ranks")
         self.nlat_in_local, self.nlon_in_local = self.lat_in_shapes[self.comm_rank_polar], self.lon_in_shapes[self.comm_rank_azimuth]
         self.nlat_out_local, self.nlon_out_local = self.lat_out_shapes[self.comm_rank_polar], self.lon_out_shapes[self.comm_rank_azimuth]
-        self.windows = disco_windows(get_psi(*self._key), self.lat_out_shapes)
+        if self._transpose:
+            window_lat, halo_lat, self._window_lon, self._halo_lon = self.lat_in_shapes, self.lat_out_shapes, self.lon_in_shapes, self.lon_out_shapes
+        else:
+            window_lat, halo_lat, self._window_lon, self._halo_lon = self.lat_out_shapes, self.lat_in_shapes, self.lon_out_shapes, self.lon_in_shapes
+        self._halo_rows = halo_lat[self.comm_rank_polar]
+        self.windows = disco_windows(get_psi(*self._key), window_lat)
         self.window = self.windows[self.comm_rank_polar]
-        self._halo_send, self._halo_recv = halo_plan(self.windows, self.lat_in_shapes, self.comm_rank_polar)
+        self._halo_send, self._halo_recv = halo_plan(self.windows, halo_lat, self.comm_rank_polar)
         self._ops = _OPS_FACTORY(self)
 
     def extra_repr(self):
         return super().extra_repr() + f", h={self.comm_size_polar}, w={self.comm_size_azimuth}"
 
+    def _window_rows(self, r):
+        """r (B*C, local rows, local longitudes) on the plan's input grid -> (rows of B*C on this azimuth rank, hi - lo, all longitudes):
+        the rows of this rank's window"""
+        if self.comm_size_azimuth > 1:
+            r = _a2a(r, 0, 2, self._halo_lon, self.azimuth_group)
+        return halo_exchange(r, self._halo_send, self._halo_recv, self.polar_group)
+
+    def _window_adjoint(self, dX):
+        """dX (B*C, K, local rows, local longitudes) on the plan's output grid -> (rows of B*C on this azimuth rank, local rows, all
+        longitudes) on its input grid: the window adjoint, its rows returned to their owners and added in rank order"""
+        if self.comm_size_azimuth > 1:
+            dX = _a2a(dX, 0, 3, self._window_lon, self.azimuth_group)
+        return halo_adjoint(self._ops.adjoint(dX).to(torch.float32), self._halo_send, self._halo_recv, self._halo_rows, self.polar_group)
+
+    def _pixels(self, X, BC):
+        """X (rows of this azimuth rank, ..., all longitudes) -> (B*C, ..., the longitudes of this rank) fp32"""
+        X = X.to(torch.float32)
+        return _a2a(X, X.dim() - 1, 0, compute_split_shapes(BC, self.comm_size_azimuth), self.azimuth_group) if self.comm_size_azimuth > 1 else X
+
+
+def _refuse_one_rank(name, serial_name):
+    from . import _size, azimuth_group, polar_group
+    if _size(polar_group()) * _size(azimuth_group()) == 1:
+        raise NotImplementedError(f"{name} needs a process grid of more than one rank (the distributed DISCO "
+                                  "convolution splits latitudes over makani_b200.distributed.polar_group() and longitudes over "
+                                  f"azimuth_group()); at spatial model parallelism 1 use {serial_name}")
+
+
+class DistributedDiscreteContinuousConvS2(_SpatialGrid, DiscreteContinuousConvS2):
+    """DISCO convolution under h x w spatial model parallelism: the constructor, attributes, weight (C_out, C_in / groups, K) and bias of
+    DiscreteContinuousConvS2, not sharded (makani tags them is_shared_mp = ["spatial"] and all-reduces their gradients).  The groups are
+    makani_b200.distributed.polar_group() (latitudes) and azimuth_group() (longitudes), read at construction; a grid of one rank is refused."""
+
+    def __init__(self, in_channels, out_channels, in_shape, out_shape, kernel_shape, basis_type="piecewise linear", basis_norm_mode="mean",
+                 groups=1, grid_in="equiangular", grid_out="equiangular", bias=True, theta_cutoff=None):
+        _refuse_one_rank("DistributedDiscreteContinuousConvS2", "DiscreteContinuousConvS2")
+        super().__init__(in_channels, out_channels, in_shape, out_shape, kernel_shape, basis_type, basis_norm_mode, groups, grid_in, grid_out,
+                         bias, theta_cutoff)
+        self._init_grid()
+
     def _window_input(self, x):
         """x (B, C, nlat_in_local, nlon_in_local) -> (rows of B*C on this azimuth rank, hi - lo, nlon_in)"""
         B, C = x.shape[:2]
-        r = x.reshape(B * C, self.nlat_in_local, self.nlon_in_local)
-        if self.comm_size_azimuth > 1:
-            r = _a2a(r, 0, 2, self.lon_in_shapes, self.azimuth_group)
-        return halo_exchange(r, self._halo_send, self._halo_recv, self.polar_group)
-
-    def _pixels(self, X, BC):
-        """X (rows of this azimuth rank, K, nlat_out_local, nlon_out) -> (B*C, K, nlat_out_local, nlon_out_local) fp32"""
-        X = X.to(torch.float32)
-        return _a2a(X, 3, 0, compute_split_shapes(BC, self.comm_size_azimuth), self.azimuth_group) if self.comm_size_azimuth > 1 else X
+        return self._window_rows(x.reshape(B * C, self.nlat_in_local, self.nlon_in_local))
 
     def forward(self, x):
         want = (self.in_channels, self.nlat_in_local, self.nlon_in_local)
@@ -234,3 +262,68 @@ class DistributedDiscreteContinuousConvS2(DiscreteContinuousConvS2):
             x = x.to(torch.float32)
         return _DistDiscoConv.apply(x.contiguous(), self.weight, self.bias, self)
 
+
+class _DistDiscoConvTranspose(torch.autograd.Function):
+    """y = the window adjoint of Y (+ bias), Y = the K-fold channel mix of x on the local pixels.  Saves x and W only."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, m):
+        B, C_out, G = x.shape[0], weight.shape[0], m.groups
+        Y = torch.matmul(_transposed_mix(weight.to(torch.float32), G), x.to(torch.float32).view(B, G, -1, m.nlat_in_local * m.nlon_in_local))
+        g = m._window_adjoint(Y.view(B * C_out, m.kernel_size, m.nlat_in_local, m.nlon_in_local))
+        y = m._pixels(g, B * C_out).view(B, C_out, m.nlat_out_local, m.nlon_out_local)
+        if bias is not None:
+            y = y + bias.to(torch.float32).view(1, -1, 1, 1)
+        ctx.save_for_backward(x, weight)
+        ctx.m, ctx.has_bias = m, bias is not None
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        x, weight = ctx.saved_tensors
+        m, G = ctx.m, ctx.m.groups
+        B, C_out, P = x.shape[0], weight.shape[0], m.nlat_in_local * m.nlon_in_local
+        gy = gy.to(torch.float32).contiguous()
+        dx = dw = db = None
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+            gwin = m._window_rows(gy.view(B * C_out, m.nlat_out_local, m.nlon_out_local))
+            gY = m._pixels(m._ops.contract(gwin), B * C_out).view(B, G, -1, P)                   # (B, G, C_out/G * K, local pixels)
+            Wt = _transposed_mix(weight.to(torch.float32), G)
+        if ctx.needs_input_grad[0]:
+            dx = torch.matmul(Wt.transpose(1, 2), gY).view(x.shape).to(x.dtype)
+        if ctx.needs_input_grad[1]:
+            dWt = torch.matmul(gY, x.to(torch.float32).view(B, G, -1, P).transpose(2, 3)).sum(0)   # (G, C_out/G * K, C_in/G)
+            dw = dWt.view(G, -1, m.kernel_size, m.groupsize).transpose(2, 3).reshape(weight.shape).to(weight.dtype)
+        if ctx.has_bias and ctx.needs_input_grad[2]:
+            db = gy.sum(dim=(0, 2, 3))
+        return dx, dw, db, None
+
+
+class DistributedDiscreteContinuousConvTransposeS2(_SpatialGrid, DiscreteContinuousConvTransposeS2):
+    """Transposed DISCO convolution under h x w spatial model parallelism: the constructor, attributes, weight and bias of
+    DiscreteContinuousConvTransposeS2, not sharded; x local (B, C_in, lat_in_shapes[ih], lon_in_shapes[iw]) -> y local
+    (B, C_out, lat_out_shapes[ih], lon_out_shapes[iw]) float32.
+
+        forward : grouped GEMM on the local pixels -> [w-a2a lon <-> rows of B*C_out] -> window adjoint (windows of the in-grid rows)
+                  -> [h halo adjoint over the out-grid rows, fixed rank order] -> [w-a2a rows <-> lon] (+ bias)
+        backward: [w-a2a] -> [h halo] -> window contraction -> [w-a2a] -> GEMM^T (dx) and local partial sums (dW, dbias)
+
+    the backward chain of DistributedDiscreteContinuousConvS2 run as the forward, and its forward chain as the backward.  A grid of one rank is
+    refused."""
+
+    def __init__(self, in_channels, out_channels, in_shape, out_shape, kernel_shape, basis_type="piecewise linear", basis_norm_mode="mean",
+                 groups=1, grid_in="equiangular", grid_out="equiangular", bias=True, theta_cutoff=None):
+        _refuse_one_rank("DistributedDiscreteContinuousConvTransposeS2", "DiscreteContinuousConvTransposeS2")
+        super().__init__(in_channels, out_channels, in_shape, out_shape, kernel_shape, basis_type, basis_norm_mode, groups, grid_in, grid_out,
+                         bias, theta_cutoff)
+        self._init_grid()
+
+    def forward(self, x):
+        want = (self.in_channels, self.nlat_in_local, self.nlon_in_local)
+        if x.dim() != 4 or tuple(x.shape[1:]) != want:
+            raise ValueError(f"expected the local shard (B, {want[0]}, {want[1]}, {want[2]}), got {tuple(x.shape)}")
+        if x.shape[0] * self.out_channels < self.comm_size_azimuth:
+            raise ValueError(f"B * C_out = {x.shape[0] * self.out_channels} rows cannot be split over {self.comm_size_azimuth} azimuth ranks")
+        if x.dtype not in (torch.float32, torch.bfloat16):
+            x = x.to(torch.float32)
+        return _DistDiscoConvTranspose.apply(x.contiguous(), self.weight, self.bias, self)
