@@ -1,11 +1,12 @@
 // Tensor-core path (B200SHT_PREC_TF32): the Legendre contractions and the dense channel mix as TMA-fed TF32 GEMMs with fp32
 // accumulation.
 //
-//   one persistent engine (umma_kernel<Traits, NB, SPLIT>, one CTA per SM walking the tile list): warp 0 lane 0 = TMA producer, warps
-//   1..8 = consumers; consumer warp w owns rows 16 (w - 1) .. + 15 of the 128-row tile, issues mma.m16n8k8 (TF32) on them against every
-//   column of the tile and stores its accumulators itself (the TF32 synthesis stages them for bulk stores instead).  The tile width (NB fragments of 8 columns) and the 3 x TF32 mode are template
-//   parameters: the MMA loop is straight-line code without per-fragment predicates, and no instantiation spills registers.  A ring of `stages` operand stages guarded by full/empty mbarriers runs continuously
-//   across tiles, so the producer prefetches the next tile while the consumers finish the current one and write it out.
+//   one persistent engine (umma_kernel<Traits, NB, SPLIT>, one CTA per SM walking the tile list): warps 0..7 = consumers (two
+//   warpgroups of 64 rows), warp 8 lane 0 = TMA producer; consumer warp w owns rows 16 w .. + 15 of the 128-row tile and stores its
+//   accumulators itself (the TF32 synthesis stages them for bulk stores instead).  The tile width (NB fragments of 8 columns) and the
+//   3 x TF32 mode are template parameters: the MMA loop is straight-line code without per-fragment predicates, and no instantiation spills
+//   registers.  A ring of `stages` operand stages guarded by full/empty mbarriers runs continuously across tiles, so the producer
+//   prefetches the next tile while the consumers finish the current one and write it out.
 //
 //   five Traits supply the per-operation pieces (tile coordinates, TMA boxes, MMA list, epilogue):
 //     AnaTraits   spec[l][m][n]  = sum_k P[m][l][k] X[m][n][k]          A K-major,  B K-major     (RealSHT einsum "...km,mlk->...lm")
@@ -13,24 +14,28 @@
 //     MixFwd      y[row][o]      = sum_i x[row][i] w[i][o]   (complex)  A K-major,  B MN-major    (contractions.py:23 "bgixy,giox->bgoxy")
 //     MixDgrad    gx[row][i]     = sum_o gy[row][o] conj(w[i][o])       A K-major,  B K-major
 //     MixWgrad    gw[i][o]       = sum_row conj(x[row][i]) gy[row][o]   A MN-major, B MN-major
-//   complex products use planar operands: 4 real MMAs into two accumulators (real, imaginary), negated terms through a sign flip of
-//   a fragment.
+//   complex products use planar operands: 4 real MMAs into two accumulators (real, imaginary).
 //
-// All shared-memory operand tiles use the 128-byte swizzle; every TMA box is [rows][32 floats] so it lands as rows of 128 B.  Fragments
-// are read with 8- and 16-byte shared loads, conflict-free: within each 32-wide stage the K order, and for MN-major operands the row /
-// column order, is permuted so that each thread's operands are contiguous (layouts KK / MM / KM below); the epilogues undo the
-// permutation and store 8- or 16-byte vectors where the output is contiguous along the permuted index.  wgmma is
-// not used: it reads TF32 operands from shared memory only K-major, and synthesis (A and B), mix forward (B) and wgrad (A and B) have
-// MN-major operands; B cannot come from registers.  A register-sourced-A wgmma would serve the K-major analysis and dgrad GEMMs; it is
-// not built, and the H100 cost of this engine is recorded in DESIGN.md section 9.
+// Two MMA paths.  The TF32 GEMMs with two K-major operands (AnaTraits, MixDgradTraits; kKMajor) run on wgmma straight from the TMA
+// ring: each warpgroup issues wgmma.m64nNk8 on its 64 rows against the whole tile width from shared-memory descriptors, keeps one
+// stage's MMAs in flight and releases the stage before after wgmma.wait_group 1.  wgmma reads TF32 operands from shared memory only
+// K-major, so synthesis (A and B), mix forward (B) and wgrad (A and B) stay on mma.m16n8k8 (TF32) fed by per-warp fragment loads, and so
+// does the 3 x TF32 analysis (three products per fragment pair).  All shared-memory operand tiles use the 128-byte swizzle; every TMA box
+// is [rows][32 floats] so it lands as rows of 128 B, the K-major layout of the wgmma descriptors.  The mma.sync fragments are read with
+// 8- and 16-byte shared loads, conflict-free: within each 32-wide stage the K order, and for MN-major operands the row / column order, is
+// permuted so that each thread's operands are contiguous (layouts KK / MM / KM below); the epilogues undo the permutation and store 8- or
+// 16-byte vectors where the output is contiguous along the permuted index.  The H100 cost of this engine is recorded in DESIGN.md
+// section 9.
 #include "umma_common.cuh"
+#include "wgmma_tf32.cuh"
 #include <mutex>
 
 namespace b200sht {
 
 // ======================================================================================================= engine
-constexpr int kConsumerWarps = 8;                         // 8 x 16 rows = the 128-row tile
-constexpr int kUmmaThreads = 32 * (1 + kConsumerWarps);   // warp 0: TMA producer, warps 1..8: MMA + epilogue
+constexpr int kConsumerWarps = 8;                         // 8 x 16 rows = the 128-row tile, two warpgroups of 64 rows
+constexpr int kProducerWarp = kConsumerWarps;             // warps 0..7: MMA + epilogue, warp 8: TMA producer
+constexpr int kUmmaThreads = 32 * (1 + kConsumerWarps);
 constexpr int kMaxStages = 8;
 
 struct EngineParams {
@@ -49,7 +54,7 @@ struct EngineParams {
 // that is the same for both operands, and the rows / columns of a fragment may be any rows / columns of the tile as long as the epilogue
 // maps them back.  Three layouts, chosen per GEMM so that every fragment load is 8 or 16 bytes and bank-conflict-free under the 128-byte
 // swizzle (g = lane / 4, q = lane % 4; the MMA's K positions q, q + 4 of k8 step s are called (s, q, h = 0 / 1)):
-//   KK (both operands K-major: analysis, dgrad)   (s, q, h) -> K 8 q + 2 s + h: thread q owns K 8q .. 8q+7 of every row, two 16-byte loads
+//   KK (both operands K-major: 3 x TF32 analysis) (s, q, h) -> K 8 q + 2 s + h: thread q owns K 8q .. 8q+7 of every row, two 16-byte loads
 //        per row and stage (one per pair of k8 steps); rows / columns are the plain m16n8 ones.
 //   MM (both operands MN-major: synthesis, wgrad) (s, q, h) -> K 8 s + 2 q + h.  A: the warp's rows g, g + 8 are adjacent physical rows
 //        2g, 2g + 1 (one 8-byte load per K row); B: column g of fragments 4J .. 4J + 3 is physical column 32 J + 4 g .. + 3 (one 16-byte
@@ -109,40 +114,29 @@ __device__ __forceinline__ void sgn(const uint32_t (&a)[4], uint32_t (&o)[4]) { 
   for (int i = 0; i < 4; ++i) o[i] = S > 0 ? a[i] : a[i] ^ 0x80000000u;
 }
 
-template <int S>
-__device__ __forceinline__ void sgn2(const uint32_t (&b)[2], uint32_t (&o)[2]) {
-  o[0] = S > 0 ? b[0] : b[0] ^ 0x80000000u;
-  o[1] = S > 0 ? b[1] : b[1] ^ 0x80000000u;
-}
-
 // acc[j] += A(the warp's 16 rows) B(fragment j) over the 32 K of one stage.  SPLIT (3 x TF32): the residual tiles lie `lo` bytes after A and
-// B, and every product becomes hi.hi + hi.lo + lo.hi, issued per fragment so that no operand is loaded twice.
+// B, and every product becomes hi.hi + hi.lo + lo.hi, issued per fragment so that no operand is loaded twice.  KK serves the 3 x TF32
+// analysis only: the plain TF32 K-major GEMMs run on wgmma (AnaTraits::wgmma, MixDgradTraits::wgmma).
 template <Lay L, int NB, bool SPLIT>
 __device__ __forceinline__ void gemm_real(const uint8_t* a, const uint8_t* b, uint32_t lo, int row0, float (&acc)[NB][4]) {
   if constexpr (L == Lay::KK) {
-    // fragments per batch of B loads, so that consecutive MMAs go to different accumulators (fewer when the accumulators leave few registers)
-    constexpr int CH = (SPLIT || NB > 24) ? 1 : (NB % 4 == 0 && NB <= 20) ? 4 : 2;
-    static_assert(NB % CH == 0, "KK: NB must be even");
-#pragma unroll(NB > 24 ? 1 : 2)
+    static_assert(SPLIT, "KK on mma.sync: 3 x TF32 only");
+#pragma unroll 2
     for (int hh = 0; hh < 2; ++hh) {
       uint32_t fa[2][4], la[2][4];
       lda_kk(a, row0, hh, fa);
-      if (SPLIT) lda_kk(a + lo, row0, hh, la);
+      lda_kk(a + lo, row0, hh, la);
 #pragma unroll
-      for (int j0 = 0; j0 < NB; j0 += CH) {
-        uint32_t fb[CH][2][2], lb[CH][2][2];
+      for (int j = 0; j < NB; ++j) {
+        uint32_t fb[2][2], lb[2][2];
+        ldb_kk(b, j, hh, fb);
+        ldb_kk(b + lo, j, hh, lb);
 #pragma unroll
-        for (int c = 0; c < CH; ++c) {
-          ldb_kk(b, j0 + c, hh, fb[c]);
-          if (SPLIT) ldb_kk(b + lo, j0 + c, hh, lb[c]);
+        for (int t = 0; t < 2; ++t) {
+          mma_tf32(acc[j], fa[t], fb[t]);
+          mma_tf32(acc[j], fa[t], lb[t]);
+          mma_tf32(acc[j], la[t], fb[t]);
         }
-#pragma unroll
-        for (int t = 0; t < 2; ++t)
-#pragma unroll
-          for (int c = 0; c < CH; ++c) {
-            mma_tf32(acc[j0 + c], fa[t], fb[c][t]);
-            if (SPLIT) { mma_tf32(acc[j0 + c], fa[t], lb[c][t]); mma_tf32(acc[j0 + c], la[t], fb[c][t]); }
-          }
       }
     }
   } else {
@@ -167,59 +161,30 @@ __device__ __forceinline__ void gemm_real(const uint8_t* a, const uint8_t* b, ui
   }
 }
 // complex product of planar operands over one stage (S1..S3 = +-1):  re += ar br + S1 ai bi,  im += S2 ar bi + S3 ai br.  The signs go on
-// the A fragments (MN-major B: a B load holds four fragments) or on the B fragment (KK); the two B planes are consumed one after the
-// other, so only one is held at a time.
+// the A fragments (MN-major B: a B load holds four fragments); the two B planes are consumed one after the other, so only one is held at
+// a time.  MN-major B only (KM, MM): the K-major complex GEMM (dgrad) runs on wgmma.
 template <Lay L, int NB, int S1, int S2, int S3>
 __device__ __forceinline__ void gemm_cplx(const uint8_t* ar, const uint8_t* ai, const uint8_t* br, const uint8_t* bi, int row0, float (&acc)[2 * NB][4]) {
-  if constexpr (L == Lay::KK) {
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      uint32_t fr[2][4], fi[2][4];
-      lda_kk(ar, row0, hh, fr);
-      lda_kk(ai, row0, hh, fi);
-#pragma unroll
-      for (int j = 0; j < NB; ++j) {   // here the signs go on the B fragment (two registers per k8 step)
-        uint32_t g[2][2];
-        ldb_kk(br, j, hh, g);
-#pragma unroll
-        for (int t = 0; t < 2; ++t) {
-          uint32_t x[2];
-          sgn2<S3>(g[t], x);
-          mma_tf32(acc[j], fr[t], g[t]);
-          mma_tf32(acc[NB + j], fi[t], x);
-        }
-        ldb_kk(bi, j, hh, g);
-#pragma unroll
-        for (int t = 0; t < 2; ++t) {
-          uint32_t x[2], y[2];
-          sgn2<S1>(g[t], x);
-          sgn2<S2>(g[t], y);
-          mma_tf32(acc[j], fi[t], x);
-          mma_tf32(acc[NB + j], fr[t], y);
-        }
-      }
-    }
-  } else {
-    static_assert(NB % 4 == 0, "MN-major B: NB must be a multiple of 4");
+  static_assert(L != Lay::KK, "gemm_cplx: MN-major B only");
+  static_assert(NB % 4 == 0, "MN-major B: NB must be a multiple of 4");
 #pragma unroll 1   // one k8 step at a time: unrolled, the loads of the next steps are hoisted and the accumulators spill
-    for (int s = 0; s < 4; ++s) {
-      uint32_t fr[4], fi[4], x[4];
-      if (L == Lay::MM) { lda_mm(ar, row0, s, fr); lda_mm(ai, row0, s, fi); }
-      else { lda_km(ar, row0, s, fr); lda_km(ai, row0, s, fi); }
+  for (int s = 0; s < 4; ++s) {
+    uint32_t fr[4], fi[4], x[4];
+    if (L == Lay::MM) { lda_mm(ar, row0, s, fr); lda_mm(ai, row0, s, fi); }
+    else { lda_km(ar, row0, s, fr); lda_km(ai, row0, s, fi); }
 #pragma unroll
-      for (int J = 0; J < NB / 4; ++J) {
-        uint32_t g[4][2];
-        ldb_mn(br, J, s, g);
-        sgn<S3>(fi, x);
+    for (int J = 0; J < NB / 4; ++J) {
+      uint32_t g[4][2];
+      ldb_mn(br, J, s, g);
+      sgn<S3>(fi, x);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) { mma_tf32(acc[4 * J + c], fr, g[c]); mma_tf32(acc[NB + 4 * J + c], x, g[c]); }
-        ldb_mn(bi, J, s, g);
-        uint32_t y[4];
-        sgn<S1>(fi, x);
-        sgn<S2>(fr, y);
+      for (int c = 0; c < 4; ++c) { mma_tf32(acc[4 * J + c], fr, g[c]); mma_tf32(acc[NB + 4 * J + c], x, g[c]); }
+      ldb_mn(bi, J, s, g);
+      uint32_t y[4];
+      sgn<S1>(fi, x);
+      sgn<S2>(fr, y);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) { mma_tf32(acc[4 * J + c], x, g[c]); mma_tf32(acc[NB + 4 * J + c], y, g[c]); }
-      }
+      for (int c = 0; c < 4; ++c) { mma_tf32(acc[4 * J + c], x, g[c]); mma_tf32(acc[NB + 4 * J + c], y, g[c]); }
     }
   }
 }
@@ -259,7 +224,8 @@ __device__ __forceinline__ void for_each_run(const float (&acc)[NA][4], F f) {
 // scripts/umma_waitprof.py): every role sums the SM clocks it spends per state into g_umma_prof, read back and cleared by
 // b200sht_debug_umma_profile().  Slots: 0 producer waits for a free stage (empty), 1 consumer warps wait for a loaded stage (full), 2 consumer
 // warps in the MMA loop (without the full waits), 3 consumer warps in the epilogue, 4 consumer-warp lifetime, 5 producer lifetime,
-// 6 tiles (consumer warps), 7 CTAs.  Consumer slots are sums over the 8 warps of every CTA.  The shipped build has none of it.
+// 6 tiles (consumer warps), 7 CTAs.  Consumer slots are sums over the 8 warps of every CTA.  On the wgmma path the MMA loop is the issue
+// of the stage's wgmma and the wgmma.wait_group for the stage before.  The shipped build has none of it.
 #ifdef B200SHT_UMMA_PROFILE
 constexpr bool kUmmaProfile = true;
 #else
@@ -268,14 +234,16 @@ constexpr bool kUmmaProfile = false;
 __device__ unsigned long long g_umma_prof[16];
 __device__ __forceinline__ long long prof_clock() { return kUmmaProfile ? clock64() : 0; }
 
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(32 * kConsumerWarps) : "memory"); }   // warps 1..8 only
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(32 * kConsumerWarps) : "memory"); }   // warps 0..7 only
 
 // Persistent engine: one CTA per SM loops over tiles.  The operand ring (full/empty) runs continuously across tiles, so the
 // TMA producer prefetches the next tile while the consumer warps finish the current one.  NB: 8-column fragments per warp; SPLIT: 3 x TF32.
 // Traits with kStaged (the synthesis, not in 3 x TF32) stage the finished tile in shared memory after the ring and bulk-store it from there.
+// Traits with kKMajor (both operands K-major) run their TF32 instantiations on wgmma, one warpgroup per 64 rows.
 template <class T, int NB, bool SPLIT>
 __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_constant__ typename T::Params p) {
   constexpr bool kStaged = T::kStaged && !SPLIT;
+  constexpr bool kWgmma = T::kKMajor && !SPLIT;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -289,7 +257,7 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_cons
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
   pdl_trigger();   // the next kernel of the stream may be scheduled while this one runs (it waits for our completion before touching data)
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     for (int s = 0; s < stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumerWarps); }
     fence_barrier_init();
     T::prefetch(p);
@@ -298,7 +266,7 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_cons
   const int ntiles = p.gx * p.gy * p.gz;
   pdl_wait();      // prologue done (barriers, tensor-map prefetch): from here on this kernel reads what its predecessors wrote
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       unsigned long long w_empty = 0;
       int kbg = 0;   // k-block counter across tiles: position in the operand ring
@@ -310,7 +278,8 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_cons
           const int s = kbg % stages, it = kbg / stages;
           if (it > 0) {
             const long long t0 = prof_clock();
-            mbar_wait(&empty[s], (it - 1) & 1);
+            if constexpr (kWgmma) mbar_wait_nocall(&empty[s], (it - 1) & 1);   // no function call anywhere in a wgmma kernel
+            else mbar_wait(&empty[s], (it - 1) & 1);
             if constexpr (kUmmaProfile) w_empty += clock64() - t0;
           }
           mbar_expect_tx(&full[s], p.tx_bytes);
@@ -325,7 +294,7 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_cons
     }
     __syncwarp();
   } else {
-    const int row0 = 16 * (warp - 1);
+    const int row0 = 16 * warp;
     int kbg = 0;
     uint32_t piece = 0;   // staged epilogue: output pieces written so far (position in the double buffer)
     unsigned long long w_full = 0, t_loop = 0, t_epi = 0, n_tiles = 0;
@@ -333,18 +302,38 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_cons
       typename T::Tile tile;
       if (!T::make_tile(p, tile, ti % p.gx, (ti / p.gx) % p.gy, ti / (p.gx * p.gy))) continue;
       const long long t0 = prof_clock();
-      const int nk = T::num_kblocks(p, tile);
+      const int nk = T::num_kblocks(p, tile);   // >= 1 for the kKMajor Traits: their first wgmma (scale-d = 0) initializes acc
       float acc[NB * T::kPlanes][4];
+      if constexpr (kWgmma) {
+        // one stage's wgmma stay in flight: the stage before is released once wait_group 1 has retired its group
+        int prev = 0;
+        for (int kb = 0; kb < nk; ++kb, ++kbg) {
+          const int s = kbg % stages, it = kbg / stages;
+          const long long tw = prof_clock();
+          mbar_wait_nocall(&full[s], it & 1);
+          if constexpr (kUmmaProfile) w_full += clock64() - tw;
+          wgmma_fence();
+          T::template wgmma<NB>(p, base + s * stage_bytes, warp >> 2, kb > 0, acc);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);   // this warp's wgmma of the stage before have read it
+          prev = s;
+        }
+        wgmma_wait<0>();
+        wgmma_fence_operands(acc);
+        if (lane == 0) mbar_arrive(&empty[prev]);
+      } else {
 #pragma unroll
-      for (int j = 0; j < NB * T::kPlanes; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
-      for (int kb = 0; kb < nk; ++kb, ++kbg) {
-        const int s = kbg % stages, it = kbg / stages;
-        const long long tw = prof_clock();
-        mbar_wait(&full[s], it & 1);
-        if constexpr (kUmmaProfile) w_full += clock64() - tw;
-        T::template mma<NB, SPLIT>(p, gbase + (size_t)s * stage_bytes, row0, acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[s]);   // this warp's reads of the stage are done
+        for (int j = 0; j < NB * T::kPlanes; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+        for (int kb = 0; kb < nk; ++kb, ++kbg) {
+          const int s = kbg % stages, it = kbg / stages;
+          const long long tw = prof_clock();
+          mbar_wait(&full[s], it & 1);
+          if constexpr (kUmmaProfile) w_full += clock64() - tw;
+          T::template mma<NB, SPLIT>(p, gbase + (size_t)s * stage_bytes, row0, acc);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[s]);   // this warp's reads of the stage are done
+        }
       }
       const long long t1 = prof_clock();
       if constexpr (kStaged) T::template epilogue_staged<NB>(p, tile, row0, acc, out, piece);
@@ -353,7 +342,7 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_kernel(const __grid_cons
     }
     // the bulk stores must be complete (not only have read shared memory) before the CTA exits: a dependent kernel's griddepcontrol.wait
     // relies on grid completion for the visibility of this kernel's output
-    if constexpr (kStaged) if (warp == 1) bulk_wait0();
+    if constexpr (kStaged) if (warp == 0) bulk_wait0();
     if constexpr (kUmmaProfile) if (lane == 0) {
       atomicAdd(&g_umma_prof[1], w_full);
       atomicAdd(&g_umma_prof[2], t_loop - w_full);
@@ -377,6 +366,7 @@ struct AnaTraits {
   };
   static constexpr int kPlanes = 1;
   static constexpr bool kStaged = false;   // register epilogue
+  static constexpr bool kKMajor = true;    // TF32 on wgmma
   struct Tile { int m, l0, c0, pb0; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.m = bz;
@@ -396,9 +386,16 @@ struct AnaTraits {
       tma_load_4d(st + p.lo_off + 16384, &p.tmB_lo, bar, kb * 32, t.c0, t.pb0, t.m);
     }
   }
-  template <int NB, bool SPLIT>
+  template <int NB, bool SPLIT>   // 3 x TF32 only
   __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, float (&acc)[NB][4]) {
     gemm_real<Lay::KK, NB, SPLIT>(st, st + 16384, p.lo_off, row0, acc);
+  }
+  // warpgroup wg: rows 64 wg .. + 63 of the table tile (at st) against the N rows of X (at st + 16384); acc_on = 0: first stage of the tile
+  template <int NB>
+  __device__ __forceinline__ static void wgmma(const Params&, uint32_t st, int wg, bool acc_on, float (&acc)[NB][4]) {
+    const uint64_t da = wgmma_desc_kmajor(st + 8192 * wg), db = wgmma_desc_kmajor(st + 16384);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_tf32<8 * NB, 1, NB, 0>(acc, da + 2 * k, db + 2 * k, (k > 0 || acc_on) ? 1 : 0);
   }
   // column n = pbi * Cc + ci of the tile; Cc and cp are multiples of 4, so the column pair (n, n + 1) of a run is one float2 of spec
   template <int NB>
@@ -441,6 +438,7 @@ struct SynTraits {
   // store map's box (8, 4, 16), which is the same in both layouts of Z.  Tiles of at most 20 fragments (160 columns) stage the whole
   // tile at once; wider ones stage 32 columns at a time in two alternating 16 KB buffers.
   static constexpr bool kStaged = true;
+  static constexpr bool kKMajor = false;   // MN-major operands: mma.sync
   __host__ __device__ static constexpr uint32_t out_bytes(int nb) { return nb <= 20 ? 4096u * nb : 2u * 16384u; }
   struct Tile { int m, k0, n0, lbeg; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
@@ -522,7 +520,7 @@ struct SynTraits {
         *reinterpret_cast<float2*>(b0 + e * 2048 + c * 32) = make_float2(v0, v1);
       }
   }
-  // Warp 1: bulk stores of the tile's boxes bt0 .. bt0 + nbx - 1 (staged 2 KB apart from `buf`), a few per lane, one bulk group per lane.
+  // Warp 0: bulk stores of the tile's boxes bt0 .. bt0 + nbx - 1 (staged 2 KB apart from `buf`), a few per lane, one bulk group per lane.
   // Boxes of columns past the tile's last one or of channel padding (c0 >= C) are skipped; the map's extents clip the rest: channels at C,
   // latitudes at kc1.  Latitude padding rows (nlat <= k < kp) and orders without degrees hold zero accumulators and are stored as zeros.
   __device__ static void store_boxes(const Params& p, const Tile& t, int bt0, int nbx, uint32_t buf) {
@@ -540,11 +538,11 @@ struct SynTraits {
     bulk_commit();
   }
   // All 8 consumer warps: wait until the buffer's previous stores have read it, stage, make the writes visible to the async proxy, and let
-  // warp 1 issue the stores.  Nobody waits for the stores themselves: the consumers go on to the next tile's MMAs.
+  // warp 0 issue the stores.  Nobody waits for the stores themselves: the consumers go on to the next tile's MMAs.
   template <int NB>
   __device__ __forceinline__ static void epilogue_staged(const Params& p, const Tile& t, int row0, const float (&acc)[NB][4], uint8_t* out,
                                                          uint32_t& piece) {
-    const bool issuer = (threadIdx.x >> 5) == 1;
+    const bool issuer = (threadIdx.x >> 5) == 0;
     if constexpr (NB <= 20) {
       if (issuer) bulk_wait_read<0>();
       consumer_sync();
@@ -597,6 +595,7 @@ struct MixFwdTraits {
   using Params = MixParams;
   static constexpr int kPlanes = 2;
   static constexpr bool kStaged = false;   // register epilogue
+  static constexpr bool kKMajor = false;   // MN-major B: mma.sync
   struct Tile { int l, m0, g, o0, lg; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.l = bz;
@@ -665,6 +664,7 @@ struct MixDgradTraits {
   using Tile = MixFwdTraits::Tile;  // o0 is the first input channel i0 of the tile
   static constexpr int kPlanes = 2;
   static constexpr bool kStaged = false;   // register epilogue
+  static constexpr bool kKMajor = true;    // wgmma
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) { return MixFwdTraits::make_tile(p, t, bx, by, bz); }
   __device__ static void prefetch(const Params& p) { prefetch_tmap(&p.tmX); prefetch_tmap(&p.tmW); }
   __device__ static int num_kblocks(const Params& p, const Tile&) { return (p.Cog + 31) / 32; }
@@ -675,10 +675,20 @@ struct MixDgradTraits {
     tma_load_4d(st + p.offB_r, &p.tmW, bar, kb * 32, 0, t.o0, t.lg);   // box (32 o, 1, N i, 1): K-major rows i
     tma_load_4d(st + p.offB_i, &p.tmW, bar, kb * 32, 1, t.o0, t.lg);
   }
-  // gxr = gr wr + gi wi,  gxi = gi wr - gr wi
-  template <int NB, bool>
-  __device__ __forceinline__ static void mma(const Params& p, const uint8_t* st, int row0, float (&acc)[2 * NB][4]) {
-    gemm_cplx<Lay::KK, NB, 1, -1, 1>(st, st + p.offA_i, st + p.offB_r, st + p.offB_i, row0, acc);
+  // gxr = gr wr + gi wi,  gxi = gi wr - gr wi: four real wgmma per k8 step, the negated one through the instruction's B scale.  Warpgroup
+  // wg: rows 64 wg .. + 63 of both gy planes; acc_on = 0: first stage of the tile
+  template <int NB>
+  __device__ __forceinline__ static void wgmma(const Params& p, uint32_t st, int wg, bool acc_on, float (&acc)[2 * NB][4]) {
+    const uint64_t ar = wgmma_desc_kmajor(st + 8192 * wg), ai = wgmma_desc_kmajor(st + p.offA_i + 8192 * wg);
+    const uint64_t br = wgmma_desc_kmajor(st + p.offB_r), bi = wgmma_desc_kmajor(st + p.offB_i);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int sd = (k > 0 || acc_on) ? 1 : 0;
+      wgmma_tf32<8 * NB, 1, 2 * NB, 0>(acc, ar + 2 * k, br + 2 * k, sd);
+      wgmma_tf32<8 * NB, 1, 2 * NB, NB>(acc, ai + 2 * k, br + 2 * k, sd);
+      wgmma_tf32<8 * NB, 1, 2 * NB, 0>(acc, ai + 2 * k, bi + 2 * k, 1);
+      wgmma_tf32<8 * NB, -1, 2 * NB, NB>(acc, ar + 2 * k, bi + 2 * k, 1);
+    }
   }
   template <int NB>
   __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const float (&acc)[2 * NB][4]) {
@@ -690,6 +700,7 @@ struct MixWgradTraits {
   using Params = MixParams;   // tmX = x (A, rows i), tmX2 = gy (B, cols o); K = spectral rows (m, b)
   static constexpr int kPlanes = 2;
   static constexpr bool kStaged = false;   // register epilogue
+  static constexpr bool kKMajor = false;   // MN-major operands: mma.sync
   struct Tile { int lz, i0, g, o0; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.lz = bz;

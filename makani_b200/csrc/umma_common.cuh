@@ -59,6 +59,21 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// mbar_wait for a warp with wgmma in flight: a lost arrival traps without the printf, since a function call (vprintf) inside the wgmma
+// pipeline makes ptxas serialize every wgmma of the kernel
+__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  uint32_t spins = 0;
+  long long t0 = 0;
+  while (!mbar_try_wait_hint(bar, parity, 20000u)) {
+    if ((++spins & 255u) == 0) {
+      const long long t = clock64();
+      if (t0 == 0) t0 = t;
+      else if (t - t0 > 4000000000LL) __trap();
+    }
+  }
+}
+
 // wait of a warp that is not on the critical path (epilogue / MMA issuer of a CUDA-core-bound kernel): poll every `ns` nanoseconds
 // instead of waking on every arrival, so that the waiting warps leave the issue slots to the working ones
 __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity, uint32_t ns) {
@@ -101,8 +116,9 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) { asm volat
 // 1024-byte aligned).  Two layouts, both 32 floats wide:
 //   K-major:  row r (an M or N index) holds 32 consecutive K values
 //   MN-major: blocks of [32 K-rows][32 consecutive M / N values], 4096 bytes apart
-// Hopper's wgmma reads TF32 operands from shared memory only K-major; the m16n8k8 fragments below (used by dft.cu) are loaded element by
-// element, so both layouts feed the same instruction.  The GEMM engine of umma.cu loads permuted fragments with 8- and 16-byte loads instead.
+// Hopper's wgmma reads TF32 operands from shared memory only K-major: umma.cu runs its GEMMs with two K-major operands on it (descriptors
+// below), the others on mma.m16n8k8.  The m16n8k8 fragments below (used by dft.cu) are loaded element by element, so both layouts feed the
+// same instruction; the GEMM engine of umma.cu loads permuted fragments with 8- and 16-byte loads instead.
 __device__ __forceinline__ uint32_t swz128(uint32_t off) { return off ^ ((off >> 3) & 0x70u); }
 template <bool MN>
 __device__ __forceinline__ uint32_t ld_op(const uint8_t* tile, int r, int k) {
@@ -138,6 +154,28 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
   asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+
+// ------------------------------------------------------------------------------------------- warpgroup TF32 MMA (wgmma)
+// Shared-memory descriptor of a K-major operand tile as TMA lands it: rows of 32 floats (128 B) with the 128-byte swizzle, 8-row groups
+// 1024 B apart (stride byte offset), `saddr` in a 1024-byte-aligned swizzle pattern (base offset 0).  The leading byte offset is unused for
+// swizzled K-major tiles of one swizzle atom's width.  The k8 step s of the 32 K starts 32 s bytes into the rows: desc + 2 s.
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+}
+// orders the warpgroup's earlier register accesses of the accumulators before the wgmma that follow
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// wait until at most N of the warpgroup's committed wgmma groups are pending
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// pins accumulator registers after a wgmma_wait: their reads cannot be scheduled before it
+template <int NA>
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[NA][4]) {
+#pragma unroll
+  for (int j = 0; j < NA; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) asm volatile("" : "+f"(d[j][e])::"memory");
 }
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
