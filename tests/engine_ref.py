@@ -78,6 +78,15 @@ def zero_mask(L, M, m0=0, dense=False, device="cpu"):
     return stored_mask(L, M, m0, False, device) & (l < m0 + m)
 
 
+def vector_zero_mask(L, M, m0=0, device="cpu"):
+    """bool [2L][M]: stored entries of a stacked vector spec (rows D_l, then Q_l at L + l; include/b200sht.h) that hold exact zeros.  The
+    Legendre stages see 2L rows, stored from lstart(m0 + m) (stored_mask(2L, M, m0)), so the whole Q half is stored; D and Q are both
+    zero for l < m0 + m, which in the Q half reaches below lstart(m0 + m)."""
+    l = torch.arange(2 * L, device=device)[:, None] % L
+    m = torch.arange(M, device=device)[None, :]
+    return stored_mask(2 * L, M, m0, False, device) & (l < m0 + m)
+
+
 def to_tiled(Z, M2=None):
     """standard latspec [mmax][2][R][kp] -> the tiled layout [R][kp/8][2][M2][8][8] (orders zero-padded to 8 * M2) that
     b200sht_legendre_synthesis_tiled writes and b200sht_fft_synthesis(scale_mode | 2) reads (include/b200sht.h)"""

@@ -10,6 +10,7 @@ import torch
 
 import engine_ref as E
 from oracle import makani_oracle as O
+from oracle import makani_vector_oracle as V
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "contractions_golden.npz")
@@ -98,6 +99,31 @@ def test_stored_mask_follows_common_cuh():
         assert torch.equal(st, torch.tensor([[l >= 32 * ((m0 + m) // 32) for m in range(22)] for l in range(40)]))
         z = E.zero_mask(40, 22, m0)
         assert torch.equal(z, st & torch.tensor([[l < m0 + m for m in range(22)] for l in range(40)]))
+
+
+@pytest.mark.parametrize("L,M,m0", [(9, 10, 0), (40, 41, 0), (91, 40, 51), (40, 22, 23)])
+def test_vector_zero_mask_is_where_the_stacked_tables_vanish(L, M, m0):
+    """the stacked vector spec (rows D_l, then Q_l) as the Legendre stages store it: the 2L rows from lstart(m0 + m); exact zeros where
+    l < m0 + m in either half, which is exactly where the analysis of the stacked fp64 tables of the vector oracle vanishes (besides the
+    rows that are zero for every order: D_0, and Q of order 0)"""
+    z = E.vector_zero_mask(L, M, m0)
+    st = E.stored_mask(2 * L, M, m0)
+    want = torch.tensor([[2 * L > r >= E.lstart(m0 + m) and r % L < m0 + m for m in range(M)] for r in range(2 * L)])
+    assert torch.equal(z, want)
+    assert torch.equal(z[:L], E.zero_mask(L, M, m0)), "the D half follows the scalar convention"
+    assert st[L:].all(), "the whole Q half is stored"
+
+    nlat = 33
+    th, _ = O.precompute_latitudes(nlat, "equiangular")
+    D, Q = V.vector_legpoly(m0 + M, L, th)
+    T = torch.from_numpy(np.concatenate([D, Q], axis=1)[m0:])               # [M][2L][nlat]
+    X = torch.randn(M, 2, 1, 3, nlat, generator=torch.Generator().manual_seed(2), dtype=torch.float64)
+    ref, mag = E.legendre_analysis_ref(T, X, nlat, 4, m0)
+    assert (ref[z] == 0).all() and (mag[z] == 0).all()
+    r = torch.arange(2 * L)[:, None]
+    m = torch.arange(M)[None, :]
+    always0 = (r == 0) | ((r >= L) & (m0 + m == 0))
+    assert (mag[st & ~z & ~always0][..., :3] > 0).all()
 
 
 def test_to_tiled_index_map():

@@ -138,23 +138,10 @@ def test_legendre_synthesis_tiled_is_a_relayout(grid, nlat, nlon, lmax, mmax, B,
 import dft_ref as D
 import engine_ref as E
 from makani_b200.quadrature import _grid_np
-from test_gpu_engine import SENTINEL, sentinel, untouched
+from test_gpu_engine import SENTINEL, launched_kernels, sentinel, untouched
 
 F32, BF16 = torch.float32, torch.bfloat16
 SENT16 = 0x7FC1   # bf16 quiet NaN with a payload no kernel writes
-
-
-def _kernels(fn):
-    """names of the CUDA kernels `fn` launches (`fn` is repeated when the profiler recorded no kernel at all, which it
-    occasionally does for the first launches of a session: the calls profiled here are idempotent)"""
-    for _ in range(4):
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            fn()
-            torch.cuda.synchronize()
-        names = sorted({e.name for e in prof.events() if "kernel" in e.name})
-        if names:
-            return names
-    return names
 
 
 def _want_ana_kernel(nlon, dtype):
@@ -173,7 +160,7 @@ def _analysis(plan, x, B, C, mode, expect):
     mmax, kp, nlat = plan.mmax, plan.kp, plan.nlat
     lat = sentinel(plan.latspec_elems(B, C))
     st = mb.sht._stream(x.device)
-    names = _kernels(lambda: _lib.call("b200sht_fft_analysis", plan.handle, mb.sht._ptr(x), mb.sht._dtype_code(x.dtype), B, C, mb.sht._ptr(lat), mode | 2, st))
+    names = launched_kernels(lambda: _lib.call("b200sht_fft_analysis", plan.handle, mb.sht._ptr(x), mb.sht._dtype_code(x.dtype), B, C, mb.sht._ptr(lat), mode | 2, st))
     assert any(expect in n for n in names), f"expected {expect}, ran {names}"
     n = mmax * 2 * B * C * kp
     assert untouched(lat[n:]), "the padding orders [mmax, mmax8) must not be written"
@@ -288,7 +275,7 @@ def test_dft_analysis_routes_to_the_cuda_core_fft():
     x = torch.randn(2 * 33 * 72 + 1, device=DEV)
     for xv in (x[: 2 * 33 * 72], x[1:]):
         lat = sentinel(plan.latspec_elems(1, 2))
-        names = _kernels(lambda: _lib.call("b200sht_fft_analysis", plan.handle, mb.sht._ptr(xv), 0, 1, 2, mb.sht._ptr(lat), 1 | 2, st))
+        names = launched_kernels(lambda: _lib.call("b200sht_fft_analysis", plan.handle, mb.sht._ptr(xv), 0, 1, 2, mb.sht._ptr(lat), 1 | 2, st))
         assert any("fft_analysis_" in n for n in names) and not any("dft_analysis" in n for n in names), names
         X = lat[: 37 * 2 * 2 * plan.kp].view(37, 2, 2, plan.kp)
         assert _is_tf32(X)
