@@ -19,6 +19,7 @@
  *   b200sht_vsht_*_adjoint       <- autograd backward of the two vector transforms
  *   b200sht_disco_forward/adjoint<- the psi contraction of torch_harmonics.DiscreteContinuousConvS2 and its adjoint (fourcastnet3.py:117-252, :511-543)
  *   b200sht_resample_forward/adjoint <- torch_harmonics.ResampleS2(mode="bilinear") and its adjoint (fourcastnet3.py:356-358)
+ *   b200sht_attention_forward/backward <- the attention of torch_harmonics.NeighborhoodAttentionS2 (not constructed by makani)
  *
  * Conventions
  *   - every function returns 0 on success, a negative b200sht_status otherwise; b200sht_last_error() gives text.
@@ -347,6 +348,29 @@ int b200sht_disco_plan_destroy(b200sht_disco_plan* plan);
 int64_t b200sht_disco_plan_query(const b200sht_disco_plan* plan, int what);
 int b200sht_disco_forward(const b200sht_disco_plan* plan, const void* x, int dtype, int B, int C, float* X, void* stream);
 int b200sht_disco_adjoint(const b200sht_disco_plan* plan, const float* dX, void* dx, int dtype, int B, int C, void* stream);
+
+/* ------------------------------------------------------------------ neighbourhood attention on the sphere
+ * The attention of torch_harmonics.NeighborhoodAttentionS2 (makani_b200/attention.py, DESIGN.md section 4.9; element-wise parity with
+ * torch-harmonics is not pinned, its source is not available).  The neighbourhood is a DISCO plan with K = 1 whose value at (t, i, j) is the
+ * quadrature weight w_i = 2 pi w_in[i] / nlon_in and whose support S(t) is that of b200sht_disco_plan_create's psi (r <= (1 + 1e-3) theta_cutoff
+ * at longitude 0).  Within each (t, i) the support must be an arc of longitudes j in [-off, n - 1 - off] (mod nlon_in), n its point count and
+ * off = (n - 1) / 2, or the whole ring; makani_b200.attention builds and checks such plans.  With s = nlon_in / nlon_out and H heads:
+ *   N(t, p) = { (i, (j + s p) mod nlon_in) : (i, j) in S(t) },   l_n = scale <q_h(t, p), k_h(n)>
+ *   y_h(t, p) = sum_{n in N(t,p)} w_i exp(l_n) v_h(n) / sum_{n in N(t,p)} w_i exp(l_n),   lse_h(t, p) = log sum_{n in N(t,p)} w_i exp(l_n)
+ * Operands (fp32, device): q, dq [B][nlat_out nlon_out][heads ek], k, dk [B][nlat_in nlon_in][heads ek], v, dv [B][nlat_in nlon_in][heads ev],
+ *   y, dy [B][nlat_out nlon_out][heads ev], lse, D [B][heads][nlat_out nlon_out]: point-major, head h at channels [h e, (h + 1) e).
+ * b200sht_attention_forward: writes y and lse; online softmax per output point with a running max and sum in fp32.
+ * b200sht_attention_backward: given dy, writes dq, dk, dv and D = <dy_h, y_h> per output point (scratch the caller provides):
+ *   alpha_n = w_i exp(l_n - lse), dl_n = alpha_n (<dy_h, v_h(n)> - D), dq = scale sum_n dl_n k_h(n), dv_n = sum alpha dy, dk_n = scale sum dl q.
+ *   dk and dv are gathers by input point without atomics: results are bit-identical run to run.  The backward recomputes the forward's
+ *   logits bit for bit.
+ * Head dims ek, ev in 1 .. 64 (any value; multiples of 4 with 16-byte aligned operands take the vector path), otherwise B200SHT_ERR_UNSUPPORTED.
+ * B * heads at most 65535 per call. */
+int b200sht_attention_forward(const b200sht_disco_plan* plan, const float* q, const float* k, const float* v, float* y, float* lse, int B, int heads,
+                              int ek, int ev, float scale, void* stream);
+int b200sht_attention_backward(const b200sht_disco_plan* plan, const float* q, const float* k, const float* v, const float* y, const float* lse,
+                               const float* dy, float* dq, float* dk, float* dv, float* D, int B, int heads, int ek, int ev, float scale,
+                               void* stream);
 
 /* ------------------------------------------------------------------ bilinear resampling on the sphere
  * Replaces torch_harmonics.ResampleS2(mode="bilinear"), the upsampling of FCN3's DiscreteContinuousDecoder with upsample_sht=False

@@ -95,6 +95,9 @@ _SIGNATURES = {
     "b200sht_disco_plan_query": (c_int64, [_P, c_int]),
     "b200sht_disco_forward": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P]),
     "b200sht_disco_adjoint": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P]),
+    # neighbourhood attention on the sphere (on a K = 1 DISCO plan)
+    "b200sht_attention_forward": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, _P]),
+    "b200sht_attention_backward": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, _P]),
     # bilinear resampling on the sphere
     "b200sht_resample_plan_create": (c_int, [ctypes.POINTER(_P), c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     "b200sht_resample_plan_destroy": (c_int, [_P]),

@@ -80,6 +80,10 @@ int disco_plan_destroy(b200sht_disco_plan* pl);
 long long disco_plan_query(const b200sht_disco_plan* pl, int what);
 int disco_forward(const b200sht_disco_plan* pl, const void* x, int dtype, int B, int C, float* X, cudaStream_t st);
 int disco_adjoint(const b200sht_disco_plan* pl, const float* dX, void* dx, int dtype, int B, int C, cudaStream_t st);
+int attention_forward(const b200sht_disco_plan* pl, const float* q, const float* k, const float* v, float* y, float* lse, int B, int H, int EK,
+                      int EV, float scale, cudaStream_t st);
+int attention_backward(const b200sht_disco_plan* pl, const float* q, const float* k, const float* v, const float* y, const float* lse,
+                       const float* dy, float* dq, float* dk, float* dv, float* D, int B, int H, int EK, int EV, float scale, cudaStream_t st);
 int resample_plan_create(b200sht_resample_plan** out, int nlat_in, int nlon_in, int nlat_out, int nlon_out, int expand_poles, const int* lat_idx,
                          const float* lat_w, const int* lon_left, const int* lon_right, const float* lon_w, cudaStream_t st);
 int resample_plan_destroy(b200sht_resample_plan* pl);
@@ -887,6 +891,18 @@ int b200sht_disco_forward(const b200sht_disco_plan* plan, const void* x, int dty
 
 int b200sht_disco_adjoint(const b200sht_disco_plan* plan, const float* dX, void* dx, int dtype, int B, int C, void* stream) {
   return disco_adjoint(plan, dX, dx, dtype, B, C, S(stream));
+}
+
+// ---- neighbourhood attention on the sphere (attention.cu)
+int b200sht_attention_forward(const b200sht_disco_plan* plan, const float* q, const float* k, const float* v, float* y, float* lse, int B, int heads,
+                              int ek, int ev, float scale, void* stream) {
+  return attention_forward(plan, q, k, v, y, lse, B, heads, ek, ev, scale, S(stream));
+}
+
+int b200sht_attention_backward(const b200sht_disco_plan* plan, const float* q, const float* k, const float* v, const float* y, const float* lse,
+                               const float* dy, float* dq, float* dk, float* dv, float* D, int B, int heads, int ek, int ev, float scale,
+                               void* stream) {
+  return attention_backward(plan, q, k, v, y, lse, dy, dq, dk, dv, D, B, heads, ek, ev, scale, S(stream));
 }
 
 // ---- bilinear resampling on the sphere (resample.cu)

@@ -13,30 +13,10 @@
 // and i's points; a thread owns NJ input longitudes j' = res + pscale u and gathers, for each point (t, j) with j = res (mod pscale), the
 // K values dX[k, t, (u - j / pscale) mod nlon_out].  Every output element is summed by one thread in a fixed order: no atomics, and the
 // results are bit-identical run to run.
-#include "common.cuh"
+#include "disco_plan.cuh"
 #include <algorithm>
 #include <type_traits>
 #include <vector>
-
-namespace b200sht {
-
-struct DiscoPlan {
-  int nlat_in, nlon_in, nlat_out, nlon_out, K, Kp, pscale;
-  long long nnz, npts;
-  int* d_fwd_rowptr;   // [nlat_out][nlat_in + 1] first point of (t, row >= i)
-  int2* d_fwd_band;    // [nlat_out] rows [lo, hi) of the input band of t
-  int2* d_fwd_pos;     // [npts] (i, j)
-  float* d_fwd_val;    // [npts][Kp]
-  int* d_adj_rowptr;   // [nlat_in][nlat_out + 1] first point of (i, t' >= t)
-  int2* d_adj_band;    // [nlat_in] output rows [lo, hi) that reach i
-  int2* d_adj_pos;     // [npts] (t, j)
-  float* d_adj_val;    // [npts][Kp]
-  size_t bytes;
-};
-
-}  // namespace b200sht
-
-struct b200sht_disco_plan : public b200sht::DiscoPlan {};
 
 namespace b200sht {
 

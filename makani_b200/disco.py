@@ -76,6 +76,33 @@ def get_filter_basis(kernel_shape, basis_type):
 DiscoPsi = namedtuple("DiscoPsi", "row_ptr ker col val nlat_in nlon_in nlat_out nlon_out kernel_size")
 
 
+def support_search(in_shape, out_shape, grid_in, grid_out, theta_cutoff):
+    """The support of every output latitude t (its point at longitude 0): a list of (i, j, r, bearing) arrays, one entry per input point with
+    r <= (1 + CUTOFF_SLACK) theta_cutoff, in (i, j) order.  Shared by the DISCO filter tensor and the neighbourhood of NeighborhoodAttentionS2."""
+    (nlat_in, nlon_in), (nlat_out, nlon_out) = in_shape, out_shape
+    if nlon_in % nlon_out:
+        raise ValueError(f"nlon_in {nlon_in} must be a multiple of nlon_out {nlon_out}")
+    cost_in, _ = _grid_np(nlat_in, grid_in)
+    cost_out, _ = _grid_np(nlat_out, grid_out)
+    th_in, th_out = np.arccos(np.clip(cost_in, -1, 1)), np.arccos(np.clip(cost_out, -1, 1))
+    phi = 2.0 * np.pi * np.arange(nlon_in) / nlon_in
+    rc = (1.0 + CUTOFF_SLACK) * theta_cutoff
+    out = []
+    for t in range(nlat_out):
+        rows = np.nonzero(np.abs(th_in - th_out[t]) <= rc)[0]   # r >= |theta_i - theta_t|
+        ct, st = math.cos(th_out[t]), math.sin(th_out[t])
+        ci, si = np.cos(th_in[rows])[:, None], np.sin(th_in[rows])[:, None]
+        cp, sp = np.cos(phi)[None, :], np.sin(phi)[None, :]
+        # the input point in the frame of the output point: (xr, yr, zr) = R_y(-theta_t) (sin th cos ph, sin th sin ph, cos th).
+        # r = arccos(zr) evaluated as atan2(|(xr, yr)|, zr): the same angle, without arccos' loss of half the digits near r = 0
+        xr, yr, zr = ct * si * cp - ci * st, sp * si, ct * ci + st * si * cp
+        r = np.arctan2(np.hypot(xr, yr), zr)
+        bearing = np.mod(np.arctan2(yr, xr), 2.0 * np.pi)
+        ii, jj = np.nonzero(r <= rc)
+        out.append((rows[ii], jj, r[ii, jj], bearing[ii, jj]))
+    return out
+
+
 def precompute_psi(kernel_shape, basis_type, basis_norm_mode, in_shape, out_shape, grid_in, grid_out, theta_cutoff, transpose=False):
     """psi_hat in fp64 as DiscoPsi.  Every grid point with r <= (1 + 1e-3) theta_cutoff is present for every k (zeros of the basis included).
 
@@ -89,30 +116,13 @@ def precompute_psi(kernel_shape, basis_type, basis_norm_mode, in_shape, out_shap
             raise NotImplementedError("DISCO basis_norm_mode 'nodal' is not implemented")
         raise ValueError(f"unknown basis_norm_mode {basis_norm_mode!r}")
     (nlat_in, nlon_in), (nlat_out, nlon_out) = in_shape, out_shape
-    if nlon_in % nlon_out:
-        raise ValueError(f"nlon_in {nlon_in} must be a multiple of nlon_out {nlon_out}")
     K = basis.kernel_size
-    cost_in, w_in = _grid_np(nlat_in, grid_in)
-    cost_out, w_out = _grid_np(nlat_out, grid_out)
-    th_in, th_out = np.arccos(np.clip(cost_in, -1, 1)), np.arccos(np.clip(cost_out, -1, 1))
-    phi = 2.0 * np.pi * np.arange(nlon_in) / nlon_in
+    _, w_in = _grid_np(nlat_in, grid_in)
+    _, w_out = _grid_np(nlat_out, grid_out)
     q = 2.0 * np.pi * w_in / nlon_in
     rc = (1.0 + CUTOFF_SLACK) * theta_cutoff
-
-    per_t = []                                     # (i, j, psi (K, n)) of each output latitude
-    for t in range(nlat_out):
-        rows = np.nonzero(np.abs(th_in - th_out[t]) <= rc)[0]   # r >= |theta_i - theta_t|
-        ct, st = math.cos(th_out[t]), math.sin(th_out[t])
-        ci, si = np.cos(th_in[rows])[:, None], np.sin(th_in[rows])[:, None]
-        cp, sp = np.cos(phi)[None, :], np.sin(phi)[None, :]
-        # the input point in the frame of the output point: (xr, yr, zr) = R_y(-theta_t) (sin th cos ph, sin th sin ph, cos th).
-        # r = arccos(zr) evaluated as atan2(|(xr, yr)|, zr): the same angle, without arccos' loss of half the digits near r = 0
-        xr, yr, zr = ct * si * cp - ci * st, sp * si, ct * ci + st * si * cp
-        r = np.arctan2(np.hypot(xr, yr), zr)
-        bearing = np.mod(np.arctan2(yr, xr), 2.0 * np.pi)
-        ii, jj = np.nonzero(r <= rc)
-        ii_abs = rows[ii]
-        per_t.append((ii_abs, jj, basis(r[ii, jj] / rc, bearing[ii, jj])))
+    # (i, j, psi (K, n)) of each output latitude
+    per_t = [(i, j, basis(r / rc, bearing)) for i, j, r, bearing in support_search(in_shape, out_shape, grid_in, grid_out, theta_cutoff)]
 
     if transpose:
         qc = 2.0 * np.pi * w_out / nlon_in                                 # quadrature of the centre rows, in the sums of v and a
