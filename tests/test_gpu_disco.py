@@ -3,10 +3,13 @@ stores, determinism, the module against the fp64 oracle (fp32 and TF32 GEMMs), a
 
 Kernel bound: |out - ref| <= C_SUM n 2^-24 sum |psi| |in| per element, n = the number of terms of that element's sum (fp32 accumulation of n
 products; the classical bound of recursive summation has C = 1).  C_SUM = 0.25 was calibrated on an H100 80GB HBM3: the largest need over
-every case below was 0.033 (forward, bf16 input) and 0.015 (adjoint).  bf16 outputs add the bf16 unit roundoff, 2^-8 |ref|.
+every case below was 0.033 (forward, bf16 input) and 0.015 (adjoint); the rows added for KP = 8, 16, 24, 28, K = 72 and pscale 3 need at
+most 0.035 (forward, bf16 input, K = 72) and 0.0027 (adjoint), at a 700 W power limit.  bf16 outputs add the bf16 unit roundoff, 2^-8 |ref|.
+Every row asserts through the profiler, at fp32 input, which disco_forward_kernel<KP, NP> instantiations its forward launches (FWD_KERNELS).
 """
 import math
 import os
+import re
 import sys
 
 import numpy as np
@@ -15,6 +18,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 pytestmark = pytest.mark.gpu
 
@@ -22,11 +26,12 @@ from makani_b200 import _lib  # noqa: E402
 from makani_b200 import disco as D  # noqa: E402
 from makani_b200.sht import _ptr, _stream  # noqa: E402
 from oracle import makani_disco_oracle as O  # noqa: E402
+from test_gpu_engine import launched_kernels  # noqa: E402
 
 C_SUM = 0.25
 DEV = torch.device("cuda", 0)
 
-# (in_shape, out_shape, grid_in, grid_out, cutoff in input spacings): pscale 1 and 2, poles on equiangular output grids, nlon_out 45 (not a multiple
+# (in_shape, out_shape, grid_in, grid_out, cutoff in input spacings): pscale 1, 2 and 3, poles on equiangular output grids, nlon_out 45 (not a multiple
 # of any thread tile), nlon_in 90 (no 16-byte staging), a 13-row band over 11-row stages with > 256 points per pole latitude, and nlon 1040 (two
 # longitude tiles per CTA row, two adjoint passes over K = 20)
 GEOMS = {
@@ -35,9 +40,24 @@ GEOMS = {
     "eq21x90_eq21x45": ((21, 90), (21, 45), "equiangular", "equiangular", 2.5),
     "eq91x180_lg46x90": ((91, 180), (46, 90), "equiangular", "legendre-gauss", 6.0),
     "eq9x1040": ((9, 1040), (9, 1040), "equiangular", "equiangular", 1.5),
+    "lg24x96_eq25x32": ((24, 96), (25, 32), "legendre-gauss", "equiangular", 3.0),
 }
 CASES = [("eq33x64", (1, 1)), ("eq33x64", (3, 3)), ("eq33x96_lg17x48", (5, 4)), ("eq21x90_eq21x45", (3, 3)), ("eq91x180_lg46x90", (3, 3)),
-         ("eq91x180_lg46x90", (5, 4)), ("eq9x1040", (5, 4)), ("eq21x90_eq21x45", (6, 6))]
+         ("eq91x180_lg46x90", (5, 4)), ("eq9x1040", (5, 4)), ("eq21x90_eq21x45", (6, 6)),
+         ("eq33x64", (2, 4)), ("eq33x96_lg17x48", (4, 4)), ("eq21x90_eq21x45", (4, 6)), ("eq91x180_lg46x90", (4, 7)), ("eq33x64", (8, 9)),
+         ("lg24x96_eq25x32", (3, 3))]
+# the disco_forward_kernel<KP, NP> instantiations each kernel shape launches: K = kh * kw in launches of at most 32 kernel functions,
+# KP = ceil4 of a launch's count, NP = 4 up to KP = 16, else 2.  Together the cases run all eight forward widths.
+FWD_KERNELS = {
+    (1, 1): {(4, 4)}, (3, 3): {(12, 4)}, (5, 4): {(20, 2)}, (6, 6): {(32, 2), (4, 4)}, (2, 4): {(8, 4)}, (4, 4): {(16, 4)}, (4, 6): {(24, 2)},
+    (4, 7): {(28, 2)}, (8, 9): {(32, 2), (8, 4)},
+}
+# the profiler reports void b200sht::disco_forward_kernel<8, 4>(...); cu++filt prints (int)8, (int)4
+FWD_KERNEL = re.compile(r"disco_forward_kernel<(?:\(int\))?(\d+), (?:\(int\))?(\d+)>")
+
+
+def _fwd_kernels(names):
+    return {(int(m[1]), int(m[2])) for m in map(FWD_KERNEL.search, names) if m}
 
 
 def _psi(name, kernel_shape, norm="mean"):
@@ -95,6 +115,11 @@ def test_kernels_against_fp64(name, kernel_shape, dtype):
     n_f = int(np.diff(psi.row_ptr).max()) // K
     need_f = ((X.double() - ref).abs() / (n_f * 2.0**-24 * mag + 1e-300)).max().item()
     assert need_f <= C_SUM, f"forward needs C = {need_f:.3g}"
+    names = []
+    if dtype == torch.float32:   # the input dtype is a run-time argument of the same instantiations: profile each row once
+        want = FWD_KERNELS[kernel_shape]
+        names = launched_kernels(lambda: _forward_raw(plan, x, B, C), lambda n: _fwd_kernels(n) == want)
+        assert _fwd_kernels(names) == want, f"{name} {kernel_shape}: expected disco_forward_kernel {sorted(want)}, launched {names}"
     # adjoint
     dX = torch.randn(B, C, K, ho, wo, generator=g, device=DEV)
     buf, dx = _adjoint_raw(plan, dX, B, C, dtype)
@@ -108,7 +133,7 @@ def test_kernels_against_fp64(name, kernel_shape, dtype):
     need_a = ((dx.double() - ref).abs() - extra).clamp(min=0).div(n_a * 2.0**-24 * mag + 1e-300).max().item()
     assert need_a <= C_SUM, f"adjoint needs C = {need_a:.3g}"
     NEEDS[(name, kernel_shape, str(dtype))] = (need_f, need_a)
-    print(f"\nC needed: {name} {kernel_shape} {dtype}: forward {need_f:.3g} adjoint {need_a:.3g}")
+    print(f"\nC needed: {name} {kernel_shape} {dtype}: forward {need_f:.3g} adjoint {need_a:.3g}; forward ran {' '.join(sorted(names))}")
 
 
 @pytest.mark.parametrize("name,kernel_shape", [("eq91x180_lg46x90", (3, 3)), ("eq33x96_lg17x48", (5, 4))])
