@@ -9,7 +9,8 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     NeighborhoodAttentionS2                    <- torch_harmonics.NeighborhoodAttentionS2 (local attention on the DISCO neighbourhoods)
     SpectralConv, SpectralAttention, ComplexReLU <- makani.models.common.*
     quadrature                                 <- torch_harmonics.quadrature
-    distributed                                <- torch_harmonics.distributed (h x w spatial model parallelism)
+    distributed                                <- torch_harmonics.distributed (h x w spatial model parallelism; its
+                                                  DistributedNeighborhoodAttentionS2 is NeighborhoodAttentionS2 on a sharded grid)
     install_torch_harmonics_shim()             <- makes `import torch_harmonics` resolve to this package
     HostFeed                                   <- double-buffered host->device input staging (the data loader's prefetch queue)
     sfno.SphericalFourierNeuralOperatorNet     <- makani.models.networks.sfnonet (same constructor / parameters / state dict)

@@ -135,6 +135,15 @@ def _project_points(x, weight, bias):
     return torch.baddbmm(bias.to(torch.float32).view(1, 1, -1).expand(B, xt.shape[1], -1), xt, wt)
 
 
+def _project_out(y, weight, bias):
+    """the output projection of the point-major y (B, HW, C_v) -> (B, C_out, HW) fp32, one GEMM"""
+    B, C = y.shape[0], y.shape[2]
+    wp = weight.to(torch.float32).reshape(weight.shape[0], C).expand(B, -1, -1)
+    if bias is None:
+        return torch.bmm(wp, y.transpose(1, 2))
+    return torch.baddbmm(bias.to(torch.float32).view(1, -1, 1).expand(B, -1, y.shape[1]), wp, y.transpose(1, 2))
+
+
 class NeighborhoodAttentionS2(nn.Module):
     """Neighbourhood attention on the sphere (drop-in for torch_harmonics.NeighborhoodAttentionS2).
 
@@ -217,9 +226,4 @@ class NeighborhoodAttentionS2(nn.Module):
         k = _project_points(key, self.k_weights, self.k_bias)
         v = _project_points(value, self.v_weights, self.v_bias)
         y = _NeighborhoodAttention.apply(q, k, v, self.plan(query.device), self.num_heads, self.scale)   # (B, HW_out, C_v)
-        wp = self.proj_weights.to(torch.float32).reshape(self.out_channels, self.out_channels).expand(B, -1, -1)
-        if self.proj_bias is None:
-            out = torch.bmm(wp, y.transpose(1, 2))
-        else:
-            out = torch.baddbmm(self.proj_bias.to(torch.float32).view(1, -1, 1).expand(B, -1, y.shape[1]), wp, y.transpose(1, 2))
-        return out.view(B, self.out_channels, self.nlat_out, self.nlon_out)
+        return _project_out(y, self.proj_weights, self.proj_bias).view(B, self.out_channels, self.nlat_out, self.nlon_out)

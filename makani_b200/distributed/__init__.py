@@ -17,7 +17,8 @@ channels, the longitude stages see the 2C component rows and the Legendre stage 
 
 DistributedDiscreteContinuousConvS2 (distributed/disco.py: a latitude halo and window plans of psi_hat) and DistributedResampleS2
 (distributed/resample.py: whole spheres of a subset of planes) are FCN3's local operators under the same h x w grid;
-DistributedDiscreteContinuousConvTransposeS2 runs the DISCO stages the other way round.
+DistributedDiscreteContinuousConvTransposeS2 runs the DISCO stages the other way round, and DistributedNeighborhoodAttentionS2
+(distributed/attention.py) runs the attention kernels on window plans of the neighbourhood, over the same halo.
 """
 import ctypes
 
@@ -490,3 +491,4 @@ class DistributedInverseRealVectorSHT(_DistributedBase):
 
 from .disco import DistributedDiscreteContinuousConvS2, DistributedDiscreteContinuousConvTransposeS2, set_disco_local_ops  # noqa: E402,F401
 from .resample import DistributedResampleS2, set_resample_local_ops  # noqa: E402,F401
+from .attention import DistributedNeighborhoodAttentionS2, set_attention_local_ops  # noqa: E402,F401

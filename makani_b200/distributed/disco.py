@@ -94,6 +94,20 @@ def _a2a(x, dim0, dim1, dim1_split_sizes, group):
 _window_plans, _window_lock = {}, threading.Lock()
 
 
+def window_plan(plan_class, key, window, device, what):
+    """plan_class(window.psi, device), cached per plan class, global key, window and device"""
+    if device.type != "cuda":
+        raise B200ShtError(f"{what} runs on CUDA devices only (got {device}); makani_b200 has no CPU fallback")
+    k = (plan_class,) + tuple(key) + (window.t0, window.t1, device.index if device.index is not None else torch.cuda.current_device())
+    with _window_lock:
+        p = _window_plans.get(k)
+    if p is None:
+        p = plan_class(window.psi, device)
+        with _window_lock:
+            p = _window_plans.setdefault(k, p)
+    return p
+
+
 class CudaDiscoLocalOps:
     """The window contraction and its adjoint on the kernels of csrc/disco.cu, on a plan of `layer.window` (cached per key, window, device).
     `layer` has `_key` (the psi_hat key of makani_b200.disco) and `window` (a DiscoWindow)."""
@@ -102,17 +116,7 @@ class CudaDiscoLocalOps:
         self.key, self.window = layer._key, layer.window
 
     def _plan(self, device):
-        if device.type != "cuda":
-            raise B200ShtError(f"the DISCO convolution runs on CUDA devices only (got {device}); makani_b200 has no CPU fallback")
-        w = self.window
-        k = self.key + (w.t0, w.t1, device.index if device.index is not None else torch.cuda.current_device())
-        with _window_lock:
-            p = _window_plans.get(k)
-        if p is None:
-            p = DiscoPlan(w.psi, device)
-            with _window_lock:
-                p = _window_plans.setdefault(k, p)
-        return p
+        return window_plan(DiscoPlan, self.key, self.window, device, "the DISCO convolution")
 
     def contract(self, xwin):
         """xwin (R, hi - lo, nlon_in) fp32 / bf16 -> X (R, K, t1 - t0, nlon_out) fp32"""
@@ -178,11 +182,12 @@ class _DistDiscoConv(torch.autograd.Function):
 
 
 class _SpatialGrid:
-    """The h x w process grid of both distributed DISCO convolutions: groups, split shapes, local shapes, the windows of the plan's output
-    rows and the halo over its input rows, and the two data movements around the window contraction.  The plan's output rows are the module's
-    output latitudes, and for the transposed convolution (`_transpose`) its input latitudes."""
+    """The h x w process grid of the distributed DISCO convolutions and the distributed neighbourhood attention: groups, split shapes, local
+    shapes, the windows of a global DiscoPsi's output rows and the halo over its input rows, and the data movements around the per-rank
+    stage.  The plan's output rows are the module's output latitudes, and for the transposed convolution (`_transpose`) its input latitudes."""
 
-    def _init_grid(self):
+    def _init_grid(self, psi, ops_factory):
+        """psi: the global DiscoPsi whose output rows are windowed; ops_factory(self) -> the per-rank stage (self._ops)"""
         from . import _rank, _size, azimuth_group, polar_group
         self.polar_group, self.azimuth_group = polar_group(), azimuth_group()
         self.comm_size_polar, self.comm_rank_polar = _size(self.polar_group), _rank(self.polar_group)
@@ -199,20 +204,28 @@ class _SpatialGrid:
         else:
             window_lat, halo_lat, self._window_lon, self._halo_lon = self.lat_out_shapes, self.lat_in_shapes, self.lon_out_shapes, self.lon_in_shapes
         self._halo_rows = halo_lat[self.comm_rank_polar]
-        self.windows = disco_windows(get_psi(*self._key), window_lat)
+        self.windows = disco_windows(psi, window_lat)
         self.window = self.windows[self.comm_rank_polar]
         self._halo_send, self._halo_recv = halo_plan(self.windows, halo_lat, self.comm_rank_polar)
-        self._ops = _OPS_FACTORY(self)
+        self._ops = ops_factory(self)
 
     def extra_repr(self):
         return super().extra_repr() + f", h={self.comm_size_polar}, w={self.comm_size_azimuth}"
 
     def _window_rows(self, r):
-        """r (B*C, local rows, local longitudes) on the plan's input grid -> (rows of B*C on this azimuth rank, hi - lo, all longitudes):
-        the rows of this rank's window"""
+        """r (B*C, local rows, local longitudes, ...) on the plan's input grid -> (rows of B*C on this azimuth rank, hi - lo, all longitudes,
+        ...): the rows of this rank's window"""
         if self.comm_size_azimuth > 1:
             r = _a2a(r, 0, 2, self._halo_lon, self.azimuth_group)
-        return halo_exchange(r, self._halo_send, self._halo_recv, self.polar_group)
+        g = halo_exchange(r.reshape(r.shape[0], r.shape[1], -1), self._halo_send, self._halo_recv, self.polar_group)
+        return g.view(g.shape[0], g.shape[1], *r.shape[2:])
+
+    def _window_rows_adjoint(self, g, BC):
+        """the adjoint of _window_rows: g (rows of B*C on this azimuth rank, hi - lo, all longitudes, ...) -> (B*C, local rows, local
+        longitudes, ...), the window rows returned to their owners and added in rank order"""
+        d = halo_adjoint(g.reshape(g.shape[0], g.shape[1], -1), self._halo_send, self._halo_recv, self._halo_rows, self.polar_group)
+        d = d.view(g.shape[0], self._halo_rows, *g.shape[2:])
+        return _a2a(d, 2, 0, compute_split_shapes(BC, self.comm_size_azimuth), self.azimuth_group) if self.comm_size_azimuth > 1 else d
 
     def _window_adjoint(self, dX):
         """dX (B*C, K, local rows, local longitudes) on the plan's output grid -> (rows of B*C on this azimuth rank, local rows, all
@@ -227,11 +240,11 @@ class _SpatialGrid:
         return _a2a(X, X.dim() - 1, 0, compute_split_shapes(BC, self.comm_size_azimuth), self.azimuth_group) if self.comm_size_azimuth > 1 else X
 
 
-def _refuse_one_rank(name, serial_name):
+def _refuse_one_rank(name, serial_name, what="the distributed DISCO convolution"):
     from . import _size, azimuth_group, polar_group
     if _size(polar_group()) * _size(azimuth_group()) == 1:
-        raise NotImplementedError(f"{name} needs a process grid of more than one rank (the distributed DISCO "
-                                  "convolution splits latitudes over makani_b200.distributed.polar_group() and longitudes over "
+        raise NotImplementedError(f"{name} needs a process grid of more than one rank ({what} "
+                                  "splits latitudes over makani_b200.distributed.polar_group() and longitudes over "
                                   f"azimuth_group()); at spatial model parallelism 1 use {serial_name}")
 
 
@@ -245,7 +258,7 @@ class DistributedDiscreteContinuousConvS2(_SpatialGrid, DiscreteContinuousConvS2
         _refuse_one_rank("DistributedDiscreteContinuousConvS2", "DiscreteContinuousConvS2")
         super().__init__(in_channels, out_channels, in_shape, out_shape, kernel_shape, basis_type, basis_norm_mode, groups, grid_in, grid_out,
                          bias, theta_cutoff)
-        self._init_grid()
+        self._init_grid(get_psi(*self._key), _OPS_FACTORY)
 
     def _window_input(self, x):
         """x (B, C, nlat_in_local, nlon_in_local) -> (rows of B*C on this azimuth rank, hi - lo, nlon_in)"""
@@ -316,7 +329,7 @@ class DistributedDiscreteContinuousConvTransposeS2(_SpatialGrid, DiscreteContinu
         _refuse_one_rank("DistributedDiscreteContinuousConvTransposeS2", "DiscreteContinuousConvTransposeS2")
         super().__init__(in_channels, out_channels, in_shape, out_shape, kernel_shape, basis_type, basis_norm_mode, groups, grid_in, grid_out,
                          bias, theta_cutoff)
-        self._init_grid()
+        self._init_grid(get_psi(*self._key), _OPS_FACTORY)
 
     def forward(self, x):
         want = (self.in_channels, self.nlat_in_local, self.nlon_in_local)
