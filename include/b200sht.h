@@ -404,16 +404,6 @@ int b200sht_resample_adjoint(const b200sht_resample_plan* plan, const float* dy,
 /* Programmatic dependent launch between the tensor-core kernels of a call sequence (prologue of kernel i+1 under the tail of kernel i; environment
  * B200SHT_PDL sets the initial value, default on).  Returns the previous setting.  Results do not depend on it. */
 int b200sht_debug_set_pdl(int on);
-/* Latitude chunks of the fused (longitude analysis -> Legendre analysis) pair inside b200sht_sht_forward / _inverse_adjoint and the
- * SpectralConv entry points at B200SHT_PREC_TF32: n > 1 forces n chunks, 1 switches chunking off, 0 restores the default (by size; the
- * environment variable B200SHT_LAT_CHUNKS sets the initial value).  Returns the previous setting.  Results are identical up to the
- * summation order of the Legendre sums. */
-int b200sht_debug_set_lat_chunks(int n);
-/* Latitude chunks of the (Legendre synthesis -> longitude synthesis) pair inside b200sht_sht_inverse / _forward_adjoint and the SpectralConv
- * entry points at B200SHT_PREC_TF32 on plans with the tensor-core DFT: n > 1 forces n chunks of whole 128-row tiles, 0 or 1 leaves the pair
- * unchunked (the default; the environment variable B200SHT_LAT_CHUNKS_SYN sets the initial value).  Returns the previous setting.  Every
- * output row is computed the same way either way, so the results are bit-identical. */
-int b200sht_debug_set_lat_chunks_syn(int n);
 /* radices chosen for length N; returns the number of stages or a negative status */
 int b200sht_debug_fft_plan(int N, int* radices, int max_radices);
 /* table [mmax][lmax][nlat] (fp32) from cos(colatitude) cost[nlat] */

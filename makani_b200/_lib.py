@@ -109,8 +109,6 @@ _SIGNATURES = {
     "b200sht_debug_dft_host": (c_int, [c_int, c_int, c_int, c_int, c_float, _P, _P]),
     "b200sht_debug_dft_profile": (c_int, [_P]),
     "b200sht_debug_umma_profile": (c_int, [_P]),
-    "b200sht_debug_set_lat_chunks": (c_int, [c_int]),
-    "b200sht_debug_set_lat_chunks_syn": (c_int, [c_int]),
     "b200sht_debug_set_pdl": (c_int, [c_int]),
     "b200sht_debug_fft_plan": (c_int, [c_int, _P, c_int]),
     "b200sht_debug_table_host": (c_int, [c_int, c_int, c_int, _P, c_int, _P]),

@@ -45,12 +45,8 @@ void dft_plan_destroy(Plan* pl);
 int dft_host(int N, int mmax, int direction, int mode, const float* rowscale, const float* in, float* out);
 int dft_profile_read(unsigned long long* out16);
 int umma_profile_read(unsigned long long* out16);
-int legendre_analysis_umma(const Plan* pl, const float* X, float* spec, int B, int C, cudaStream_t st, const float* X_lo = nullptr, int k_begin = 0,
-                           int k_end = -1, int accumulate = 0, int last = 1);
-int dft_analysis(const Plan* pl, const void* x, int dtype, int B, int C, float* X, int mode, int round_tf32, cudaStream_t st, int k_begin = 0, int k_end = -1);
-int legendre_synthesis_umma(const Plan* pl, const float* spec, float* Z, int B, int C, int tiled, cudaStream_t st, const float* spec_lo = nullptr,
-                            int k_begin = 0, int k_end = -1);
-int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int C, const float* bias, int mode, cudaStream_t st, int k_begin = 0, int k_end = -1);
+int legendre_analysis_umma(const Plan* pl, const float* X, float* spec, int B, int C, cudaStream_t st, const float* X_lo = nullptr);
+int legendre_synthesis_umma(const Plan* pl, const float* spec, float* Z, int B, int C, int tiled, cudaStream_t st, const float* spec_lo = nullptr);
 int umma_plan_table_lo(const Plan* pl);
 int tf32_residual(const float* src, float* dst, size_t n, cudaStream_t st);
 bool dft_usable(const Plan* pl);
@@ -327,50 +323,10 @@ int b200sht_legendre_synthesis_tiled(const b200sht_plan* pl, const float* spec, 
   return legendre_synthesis_tiled_any(pl, spec, latspec, B, C, stream);
 }
 
-// Longitude analysis + Legendre analysis.  At TF32 with the tensor-core DFT the pair can run in latitude chunks: the DFT writes the latspec
-// rows of one chunk (tens of MB) and the Legendre kernel reduces over exactly those rows right away -- reading them from L2 (50 MB on
-// an H100) instead of HBM -- and adds its partial sums to the coefficients of the earlier chunks (unrounded fp32; the last chunk rounds to TF32).
-// The Legendre table is sliced along latitude, so no byte of it is read twice.  B200SHT_LAT_CHUNKS = n forces n chunks (1 = off);
-// default: chunks of at most kLatChunkBytes of latspec when the whole tensor exceeds it.
-constexpr size_t kLatChunkBytes = 16u << 20;   // a third of the H100's 50 MB L2: the chunk and its slice of the table stay resident
-constexpr bool kLatChunkByDefault = false;      // off until a measurement on the H100 shows a gain
-static int& lat_chunks_forced() {
-  static int forced = [] { const char* e = getenv("B200SHT_LAT_CHUNKS"); return e ? atoi(e) : 0; }();
-  return forced;
-}
-// the synthesis pair (Legendre synthesis -> longitude synthesis) can be chunked the same way (B200SHT_LAT_CHUNKS_SYN = n; off by default):
-// its consumer, the DFT kernel, is not HBM-bound, so the gain is the latency of L2 hits only.  b200sht_debug_set_lat_chunks_syn changes it.
-static int& lat_chunks_syn() {
-  static int n = [] { const char* e = getenv("B200SHT_LAT_CHUNKS_SYN"); return e ? atoi(e) : 0; }();
-  return n;
-}
-static int lat_chunks(const b200sht_plan* pl, int B, int C) {
-  int n = lat_chunks_forced();
-  if (n <= 0 && !kLatChunkByDefault) return 1;
-  if (n <= 0) {
-    const size_t bytes = (size_t)pl->mmax * 2 * B * C * pl->kp * sizeof(float);
-    n = (int)((bytes + kLatChunkBytes - 1) / kLatChunkBytes);
-  }
-  const int maxn = pl->nlat / 64;   // at least two 32-row K-blocks per chunk
-  if (n > maxn) n = maxn;
-  return n < 1 ? 1 : n;
-}
 // Legendre synthesis + longitude synthesis: through the tiled latspec layout and the tensor-core DFT when the plan supports it at TF32
 static int synthesis_pair(const b200sht_plan* pl, const float* spec, float* lat, void* y, int dtype, int B, int C, const float* bias, int mode,
                           int precision, void* stream) {
   if (precision == B200SHT_PREC_TF32 && pl->umma_ok && dft_usable(pl)) {
-    const int n = lat_chunks_syn();
-    if (n > 1 && pl->kp > 128 && (reinterpret_cast<uintptr_t>(lat) & 127) == 0) {
-      B200_REQUIRE(B > 0 && C > 0 && (long long)B * C <= 65535, "synthesis: B*C=%lld out of range", (long long)B * C);
-      const int rows = round_up(ceil_div(pl->kp, n), 128);
-      int rc = 0;
-      for (int k0 = 0; k0 < pl->kp && !rc; k0 += rows) {
-        const int k1 = k0 + rows < pl->kp ? k0 + rows : -1;
-        rc = legendre_synthesis_umma(pl, spec, lat, B, C, 1, S(stream), nullptr, k0, k1);
-        if (!rc) rc = dft_synthesis(pl, lat, y, dtype, B, C, bias, mode & 1, S(stream), k0, k1);
-      }
-      return rc;
-    }
     int rc = legendre_synthesis_tiled_any(pl, spec, lat, B, C, stream);
     if (!rc) rc = b200sht_fft_synthesis(pl, lat, y, dtype, B, C, bias, mode | 2, stream);
     return rc;
@@ -380,23 +336,10 @@ static int synthesis_pair(const b200sht_plan* pl, const float* spec, float* lat,
   return rc;
 }
 
+// Longitude analysis + Legendre analysis
 static int analysis_pair(const b200sht_plan* pl, const void* x, int dtype, int B, int C, float* lat, float* spec, int mode, int precision, void* stream) {
-  const bool dft = precision == B200SHT_PREC_TF32 && pl->umma_ok && !pl->no_table && dft_usable(pl) && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
-                   (dtype == B200SHT_BF16 || pl->nlon % 32 == 0);
-  const int n = dft ? lat_chunks(pl, B, C) : 1;
-  if (n <= 1) {
-    int rc = b200sht_fft_analysis(pl, x, dtype, B, C, lat, mode | (precision == B200SHT_PREC_TF32 ? 2 : 0), stream);
-    if (!rc) rc = legendre_analysis_any(pl, lat, spec, B, C, precision, stream);
-    return rc;
-  }
-  B200_REQUIRE(B > 0 && C > 0 && (long long)B * C <= 65535, "analysis: B*C=%lld out of range", (long long)B * C);
-  const int rows = round_up(ceil_div(pl->nlat, n), 32);
-  int rc = 0;
-  for (int k0 = 0, i = 0; k0 < pl->nlat && !rc; k0 += rows, ++i) {
-    const bool last = k0 + rows >= pl->nlat;
-    rc = dft_analysis(pl, x, dtype, B, C, lat, mode & 1, 1, S(stream), k0, last ? -1 : k0 + rows);
-    if (!rc) rc = legendre_analysis_umma(pl, lat, spec, B, C, S(stream), nullptr, k0, last ? -1 : k0 + rows, i > 0, last);
-  }
+  int rc = b200sht_fft_analysis(pl, x, dtype, B, C, lat, mode | (precision == B200SHT_PREC_TF32 ? 2 : 0), stream);
+  if (!rc) rc = legendre_analysis_any(pl, lat, spec, B, C, precision, stream);
   return rc;
 }
 
@@ -845,18 +788,6 @@ int b200sht_bias_gelu_backward(const void* x, const float* bias, const void* dy,
 int b200sht_debug_set_pdl(int on) {
   const int old = b200sht::pdl_flag();
   b200sht::pdl_flag() = on;
-  return old;
-}
-
-int b200sht_debug_set_lat_chunks(int n) {
-  const int old = lat_chunks_forced();
-  lat_chunks_forced() = n;
-  return old;
-}
-
-int b200sht_debug_set_lat_chunks_syn(int n) {
-  const int old = lat_chunks_syn();
-  lat_chunks_syn() = n;
   return old;
 }
 

@@ -248,8 +248,7 @@ struct DftSynParams {
   const float* rowscale;
   const float* bias;
   unsigned long long* prof;
-  int R, C, nlat, nlon, kp, mmax, N2, half, M2, mode, ntiles, ktiles, has_nyq, ow;
-  int kt0, kt_all;   // latitude range of this launch: first 8-row tile, tiles per image in the whole tensor (ktiles = tiles per image in the range)
+  int R, C, nlat, nlon, kp, mmax, N2, half, M2, mode, ntiles, ktiles, has_nyq, ow;   // ktiles: 8-row tiles per image
 };
 
 // shared memory: [A: 16 blocks x (cos 8 rows | sin 8 rows), 32 KB][B ring: kDftSynStages x 16 KB][output: 2 x 8 rows x nlon]
@@ -321,11 +320,10 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
         if (it > 0) prof_wait(prof, 8, &empty[s], (it - 1) & 1, true);
         mbar_expect_tx(&full[s], 16384);
         const uint32_t st = sB + s * 16384;
-        const int ta = (ti / p.ktiles) * p.kt_all + p.kt0 + ti % p.ktiles;   // tile index in the whole tensor
-        tma_load_5d(st, &p.tmZ, &full[s], 0, 0, 0, 0, ta);           // re, classes 0..3
-        tma_load_5d(st + 4096, &p.tmZ, &full[s], 0, 1, 0, 0, ta);    // re, classes 4..7
-        tma_load_5d(st + 8192, &p.tmZ, &full[s], 0, 0, 0, 1, ta);    // im
-        tma_load_5d(st + 12288, &p.tmZ, &full[s], 0, 1, 0, 1, ta);
+        tma_load_5d(st, &p.tmZ, &full[s], 0, 0, 0, 0, ti);           // re, classes 0..3
+        tma_load_5d(st + 4096, &p.tmZ, &full[s], 0, 1, 0, 0, ti);    // re, classes 4..7
+        tma_load_5d(st + 8192, &p.tmZ, &full[s], 0, 0, 0, 1, ti);    // im
+        tma_load_5d(st + 12288, &p.tmZ, &full[s], 0, 1, 0, 1, ti);
       }
     }
     __syncwarp();
@@ -335,7 +333,7 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
       for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
         const int b = n & 1;
         prof_wait(prof, 11, &staged[b], (n >> 1) & 1, true);
-        const int r = ti / p.ktiles, k0 = (p.kt0 + ti - r * p.ktiles) * 8;
+        const int r = ti / p.ktiles, k0 = (ti - r * p.ktiles) * 8;
         if (k0 < p.nlat)   // tiles of the padding rows kp > nlat: nothing to store (rows k >= nlat of a partial tile are clipped by TMA)
           for (int bx = 0; bx * ow < nlon; ++bx) tma_store_3d(&p.tmY, sO + b * obytes + bx * 8 * ow * (uint32_t)sizeof(T), bx * ow, k0, r);
         bulk_commit();
@@ -356,8 +354,7 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
       const int n = task / nblk, blk = task - n * nblk;   // tile n of this CTA, 8-column block blk
       const int ti = blockIdx.x + n * gridDim.x;
       if (ti >= p.ntiles) break;
-      const int r = ti / p.ktiles, k0 = (p.kt0 + ti - r * p.ktiles) * 8;
-      const int ta = r * p.kt_all + p.kt0 + (ti - r * p.ktiles);   // tile index in the whole tensor
+      const int r = ti / p.ktiles, k0 = (ti - r * p.ktiles) * 8;
       const int ka = k0 + 2 * kpi;
       const int s = n % kDftSynStages, it = n / kDftSynStages;
       // per-row output factors:  out = x * sc + off(parity of the longitude)
@@ -367,7 +364,7 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
         rsa = rs.x; rsb = rs.y;
       } else {
         // tiled latspec: element (m, plane, r, k) at ((tile * 2 + plane) * M2 + m / 8) * 64 + (m % 8) * 8 + k % 8, tile = r * ktiles + k / 8
-        const float* zt = p.Z + (size_t)ta * 2 * p.M2 * 64 + 2 * kpi;
+        const float* zt = p.Z + (size_t)ti * 2 * p.M2 * 64 + 2 * kpi;
         const float2 z0 = *reinterpret_cast<const float2*>(zt);
         z0a = z0.x; z0b = z0.y;
         if (p.has_nyq) {
@@ -462,8 +459,7 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
   if (kDftProfile && p.prof && threadIdx.x < 16) atomicAdd(p.prof + threadIdx.x, prof_s[threadIdx.x]);
 }
 
-// k_begin / k_end: latitude range [k_begin, k_end) to produce (k_begin a multiple of 8; k_end < 0: all rows) -- the other rows of y are not touched
-int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int C, const float* bias, int mode, cudaStream_t st, int k_begin, int k_end) {
+int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int C, const float* bias, int mode, cudaStream_t st) {
   const DftTables* t = static_cast<const DftTables*>(pl->dft_state);
   B200_REQUIRE(t != nullptr, "dft_synthesis: plan has no DFT tables");
   const int R = B * C;
@@ -472,10 +468,7 @@ int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int
   p.Z = Z; p.tw = t->tw; p.rowscale = pl->d_rowscale; p.bias = bias; p.prof = dft_prof_buffer();
   p.R = R; p.C = C; p.nlat = pl->nlat; p.nlon = pl->nlon; p.kp = pl->kp; p.mmax = pl->mmax;
   p.N2 = t->N2; p.half = t->half; p.mode = mode;
-  if (k_end < 0 || k_end > pl->kp) k_end = pl->kp;
-  B200_REQUIRE(k_begin >= 0 && k_begin % 8 == 0 && k_begin < k_end, "dft_synthesis: bad latitude range [%d, %d)", k_begin, k_end);
-  p.kt_all = pl->kp / 8; p.kt0 = k_begin / 8;
-  p.ktiles = (k_end - k_begin + 7) / 8; p.ntiles = R * p.ktiles;
+  p.ktiles = pl->kp / 8; p.ntiles = R * p.ktiles;
   p.has_nyq = (pl->mmax == pl->nlon / 2 + 1) ? 1 : 0;
   p.M2 = t->M2;
   {
@@ -556,8 +549,7 @@ struct DftAnaParams {
   const float2* tw;
   const float* rowscale;
   unsigned long long* prof;
-  int R, nlat, nlon, kp, mmax, N2, half, M2, nkb, mode, round_tf32, ntiles, ktiles, nraw, gs;
-  int kt0;   // first 16-row tile of the latitude range this launch transforms (ktiles = tiles in the range; latitude-chunked analysis, capi.cu)
+  int R, nlat, nlon, kp, mmax, N2, half, M2, nkb, mode, ntiles, ktiles, nraw, gs;   // ktiles: 16-row tiles per image
 };
 
 // warps: 0..7 MMA + epilogue (rows 16 w .. + 15 of the tile = class w), 8 loader (TMA: the resident B, then the samples), 9..15 producers.
@@ -643,7 +635,7 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
       }
       int n = 0;
       for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
-        const int r = ti / p.ktiles, row0 = r * p.nlat + (p.kt0 + ti - r * p.ktiles) * 16;
+        const int r = ti / p.ktiles, row0 = r * p.nlat + (ti - r * p.ktiles) * 16;
         for (int kb = 0; kb < nkb; ++kb) {
           const int g = n * nkb + kb, rs = g % p.nraw, it = g / p.nraw;
           if (it > 0) prof_wait(prof, 2, &raw_empty[rs], (it - 1) & 1, true);
@@ -669,13 +661,11 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
     // 16-byte loads per operand row, conflict-free under the 128-byte swizzle -- and step t of the four m16n8k8 steps contracts the columns
     // 8 q + 2 t (fragment column q) and 8 q + 2 t + 1 (fragment column q + 4) of both operands.
     const size_t plane = (size_t)p.R * p.kp;
-    const float tcomp = p.round_tf32 ? kTruncComp : 1.f;
-    const uint32_t tmask = p.round_tf32 ? 0xffffe000u : 0xffffffffu;
     const int c = warp, gq = lane >> 2, q = lane & 3;
     mbar_wait(b_full, 0);
     int n = 0;
     for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
-      const int r = ti / p.ktiles, k0 = (p.kt0 + ti - r * p.ktiles) * 16;
+      const int r = ti / p.ktiles, k0 = (ti - r * p.ktiles) * 16;
       float xr[4][4], xi[4][4];
 #pragma unroll
       for (int j = 0; j < 4; ++j)
@@ -735,14 +725,14 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
           for (int e = 0; e < 2; ++e) {
             const int m = c + 8 * (8 * j + 2 * q + e);
             if (m >= p.mmax) continue;
-            // round_tf32: the output is a TF32 value -- the bias-compensated truncation (see B200_DFT_TF32_MODE above) folded into the
-            // scale factor, then the 13 low bits cleared (one LOP3 instead of the 3 instructions of cvt.rna).  The TF32 Legendre GEMM
-            // ignores those bits anyway; readers of the fp32 value (the bias gradient, latspec_unpack) then see an unbiased TF32 value
-            // instead of one scaled by 1 + 2^-10 / 3.
-            const float sc = ((p.mode == 0) ? rs : ((m == 0 || 2 * m == p.nlon) ? 1.f : 2.f)) * tcomp;
+            // The output is a TF32 value -- the bias-compensated truncation (see B200_DFT_TF32_MODE above) folded into the scale factor,
+            // then the 13 low bits cleared (one LOP3 instead of the 3 instructions of cvt.rna).  The TF32 Legendre GEMM ignores those bits
+            // anyway; readers of the fp32 value (the bias gradient, latspec_unpack) then see an unbiased TF32 value instead of one scaled
+            // by 1 + 2^-10 / 3.
+            const float sc = ((p.mode == 0) ? rs : ((m == 0 || 2 * m == p.nlon) ? 1.f : 2.f)) * kTruncComp;
             float* dst = xb + (size_t)m * 2 * plane;
-            dst[0] = __uint_as_float(__float_as_uint(xr[j][2 * h + e] * sc) & tmask);
-            dst[plane] = __uint_as_float(__float_as_uint(xi[j][2 * h + e] * sc) & tmask);
+            dst[0] = __uint_as_float(__float_as_uint(xr[j][2 * h + e] * sc) & 0xffffe000u);
+            dst[plane] = __uint_as_float(__float_as_uint(xi[j][2 * h + e] * sc) & 0xffffe000u);
           }
       }
     }
@@ -760,7 +750,7 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
     const T* const rawS = reinterpret_cast<const T*>(gR);
     int n = 0;
     for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
-      const int r = ti / p.ktiles, kt16 = (p.kt0 + ti - r * p.ktiles) * 16;
+      const int r = ti / p.ktiles, kt16 = (ti - r * p.ktiles) * 16;
       for (int item = pw; item < 8 * nkb; item += nprod) {
         const int kb = item >> 3, q = item & 7;
         const int k0 = kt16 + 2 * q;
@@ -850,8 +840,7 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
   if (kDftProfile && p.prof && threadIdx.x < 16) atomicAdd(p.prof + threadIdx.x, prof_s[threadIdx.x]);
 }
 
-// k_begin / k_end: latitude range [k_begin, k_end) to transform (k_begin a multiple of 16; k_end < 0: up to kp) -- the other rows of X are not touched
-int dft_analysis(const Plan* pl, const void* x, int dtype, int B, int C, float* X, int mode, int round_tf32, cudaStream_t st, int k_begin, int k_end) {
+int dft_analysis(const Plan* pl, const void* x, int dtype, int B, int C, float* X, int mode, cudaStream_t st) {
   const DftTables* t = static_cast<const DftTables*>(pl->dft_state);
   B200_REQUIRE(t != nullptr, "dft_analysis: plan has no DFT tables");
   const int R = B * C;
@@ -859,11 +848,8 @@ int dft_analysis(const Plan* pl, const void* x, int dtype, int B, int C, float* 
   memset(&p, 0, sizeof(p));
   p.X = X; p.tw = t->tw; p.rowscale = pl->d_rowscale; p.prof = dft_prof_buffer();
   p.R = R; p.nlat = pl->nlat; p.nlon = pl->nlon; p.kp = pl->kp; p.mmax = pl->mmax;
-  p.N2 = t->N2; p.half = t->half; p.M2 = t->M2; p.nkb = t->nkb; p.mode = mode; p.round_tf32 = round_tf32;
-  if (k_end < 0 || k_end > pl->kp) k_end = pl->kp;
-  B200_REQUIRE(k_begin >= 0 && k_begin % 16 == 0 && k_begin < k_end, "dft_analysis: bad latitude range [%d, %d)", k_begin, k_end);
-  p.kt0 = k_begin / 16;
-  p.ktiles = (k_end - k_begin + 15) / 16; p.ntiles = R * p.ktiles;
+  p.N2 = t->N2; p.half = t->half; p.M2 = t->M2; p.nkb = t->nkb; p.mode = mode;
+  p.ktiles = (pl->kp + 15) / 16; p.ntiles = R * p.ktiles;
   const bool bf16 = (dtype == B200SHT_BF16);
   p.nraw = bf16 ? 3 : 2;   // raw stages of 20 / 34 KB
   {

@@ -845,15 +845,15 @@ static int run_fft_dir(const Plan* pl, int dir, const void* in, void* out, const
 
 // tensor-core DFT (dft.cu): used when the caller runs the TF32 precision (scale_mode bit 1) and the grid is in its range
 bool dft_usable(const Plan* pl);
-int dft_analysis(const Plan* pl, const void* x, int dtype, int B, int C, float* X, int mode, int round_tf32, cudaStream_t st, int k_begin = 0, int k_end = -1);
-int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int C, const float* bias, int mode, cudaStream_t st, int k_begin = 0, int k_end = -1);
+int dft_analysis(const Plan* pl, const void* x, int dtype, int B, int C, float* X, int mode, cudaStream_t st);
+int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int C, const float* bias, int mode, cudaStream_t st);
 
 int fft_analysis(const Plan* pl, const void* x, int dtype, int B, int C, float* X, int scale_mode, cudaStream_t st) {
   B200_REQUIRE(B > 0 && C > 0 && (long long)B * C <= 65535, "fft_analysis: B*C=%lld out of range", (long long)B * C);
   B200_REQUIRE(dtype == B200SHT_F32 || dtype == B200SHT_BF16, "fft_analysis: unknown dtype %d", dtype);
   // tensor-core DFT: TMA reads the samples, so the input must be 16-byte aligned (and nlon % 32 == 0 for fp32 input); otherwise the CUDA-core FFT
   if ((scale_mode & 2) && dft_usable(pl) && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (dtype == B200SHT_BF16 || pl->nlon % 32 == 0))
-    return dft_analysis(pl, x, dtype, B, C, X, scale_mode & 1, 1, st);
+    return dft_analysis(pl, x, dtype, B, C, X, scale_mode & 1, st);
   FftParams prm = make_params(pl, B, C, scale_mode, nullptr);
   if (dtype == B200SHT_F32) return run_fft_dir<float>(pl, 0, x, X, prm, st);
   if (dtype == B200SHT_BF16) return run_fft_dir<__nv_bfloat16>(pl, 0, x, X, prm, st);

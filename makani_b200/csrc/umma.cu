@@ -361,8 +361,7 @@ struct AnaTraits {
     alignas(64) CUtensorMap tmA_lo, tmB_lo;   // residuals of the table and of X (split mode)
     float* spec;
     int L, M, nlat, C, cp, PB, Cc, PBc, n_ct, N, m0;
-    int kb0, nkb;        // latitude range of this launch in 32-row K-blocks (latitude-chunked analysis: partial sums over a chunk of rows)
-    int acc_in, round_out;   // add to the spec values already stored (chunks after the first) / round the result to TF32 (last chunk)
+    int nkb;             // 32-row K-blocks over the latitudes
   };
   static constexpr int kPlanes = 1;
   static constexpr bool kStaged = false;   // register epilogue
@@ -378,7 +377,6 @@ struct AnaTraits {
   __device__ static void prefetch(const Params& p) { prefetch_tmap(&p.tmA); prefetch_tmap(&p.tmB); }
   __device__ static int num_kblocks(const Params& p, const Tile&) { return p.nkb; }
   __device__ static void load(const Params& p, const Tile& t, int kb, uint32_t st, uint64_t* bar) {
-    kb += p.kb0;
     tma_load_3d(st, &p.tmA, bar, kb * 32, t.l0, t.m);
     tma_load_4d(st + 16384, &p.tmB, bar, kb * 32, t.c0, t.pb0, t.m);
     if (p.split) {
@@ -411,10 +409,8 @@ struct AnaTraits {
       if (pb >= p.PB || c >= p.cp) return;
       float2* dst = reinterpret_cast<float2*>(p.spec + ((size_t)l * p.M + t.m) * JP + (size_t)pb * p.cp + c);
       float2 o = make_float2(v[0], v[1]);
-      if (p.acc_in) { const float2 d = *dst; o.x += d.x; o.y += d.y; }   // partial sums of the earlier latitude chunks (unrounded fp32)
-      // strict fp32 (split) and the partial sums of a chunked analysis stay as accumulated; otherwise the consumers are TF32 MMAs: round
-      // to nearest here
-      if (p.round_out) { o.x = tf32_rn(o.x); o.y = tf32_rn(o.y); }
+      // strict fp32 (split) stays as accumulated; otherwise the consumers are TF32 MMAs: round to nearest here
+      if (!p.split) { o.x = tf32_rn(o.x); o.y = tf32_rn(o.y); }
       *dst = o;
     });
   }
@@ -429,7 +425,6 @@ struct SynTraits {
     alignas(64) CUtensorMap tmZ;  // Z, bulk stores (k % 8, c, k / 8, pb, m) or tiled (k % 8, c, k / 8, plane 8 M2 + m, b)   box (8, 4, 16, 1, 1)
     float* Z;
     int L, M, nlat, kp, C, cp, PB, nblk, N, m0;
-    int kc0, kc1;           // latitude range [kc0, kc1) of this launch (kc0 a multiple of 128): the tiles cover these rows only
     int tiled, M2, KT, B;   // tiled output for the tensor-core DFT (dft.cu): Z[r][k / 8][p][m / 8][m % 8][k % 8], orders padded to 8 * M2
   };
   static constexpr int kPlanes = 1;
@@ -443,7 +438,7 @@ struct SynTraits {
   struct Tile { int m, k0, n0, lbeg; };
   __device__ static bool make_tile(const Params& p, Tile& t, int bx, int by, int bz) {
     t.m = bz;
-    t.k0 = p.kc0 + 128 * bx;
+    t.k0 = 128 * bx;
     t.n0 = p.N * by;
     t.lbeg = lstart(p.m0 + t.m);
     return true;
@@ -473,8 +468,8 @@ struct SynTraits {
   __device__ __forceinline__ static void epilogue(const Params& p, const Tile& t, int row0, const float (&acc)[NB][4]) {
     const int JP = p.PB * p.cp;
     const int k = t.k0 + frag_row<Lay::MM>(row0, 0);
-    if (k >= p.kc1) return;
-    const bool pair = k + 1 < p.kc1;
+    if (k >= p.kp) return;
+    const bool pair = k + 1 < p.kp;
     const int q = threadIdx.x & 3;
 #pragma unroll
     for (int J = 0; J < NB / 4; ++J)
@@ -522,7 +517,7 @@ struct SynTraits {
   }
   // Warp 0: bulk stores of the tile's boxes bt0 .. bt0 + nbx - 1 (staged 2 KB apart from `buf`), a few per lane, one bulk group per lane.
   // Boxes of columns past the tile's last one or of channel padding (c0 >= C) are skipped; the map's extents clip the rest: channels at C,
-  // latitudes at kc1.  Latitude padding rows (nlat <= k < kp) and orders without degrees hold zero accumulators and are stored as zeros.
+  // latitudes at kp.  Latitude padding rows (nlat <= k < kp) and orders without degrees hold zero accumulators and are stored as zeros.
   __device__ static void store_boxes(const Params& p, const Tile& t, int bt0, int nbx, uint32_t buf) {
     for (int b = threadIdx.x & 31; b < nbx; b += 32) {
       const int jp = t.n0 + 4 * (bt0 + b);
@@ -884,18 +879,10 @@ using SplitWidths = Widths<8, 16>;   // 3 x TF32 (precision fp32x3): residual fr
 using MixWidths = Widths<4, 8, 12>;  // complex: 2 x 96 accumulator columns
 
 // ---------------------------------------------------------------------------------------------- Legendre
-// k_begin / k_end: latitude range [k_begin, k_end) to reduce over (k_begin a multiple of 32; k_end < 0: all rows); accumulate: add to the spec
-// values stored by the launches of the earlier ranges; last: this is the final range (TF32 rounding of the result happens here)
-int legendre_analysis_umma(const Plan* pl, const float* X, float* spec, int B, int C, cudaStream_t st, const float* X_lo, int k_begin, int k_end,
-                           int accumulate, int last) {
+int legendre_analysis_umma(const Plan* pl, const float* X, float* spec, int B, int C, cudaStream_t st, const float* X_lo) {
   AnaTraits::Params p;
   memset(&p, 0, sizeof(p));
-  if (k_end < 0 || k_end > pl->nlat) k_end = pl->nlat;
-  B200_REQUIRE(k_begin >= 0 && k_begin % 32 == 0 && k_begin < k_end, "legendre_analysis: bad latitude range [%d, %d)", k_begin, k_end);
-  p.kb0 = k_begin / 32;
-  p.nkb = ceil_div(k_end - k_begin, 32);
-  p.acc_in = accumulate;
-  p.round_out = (last && X_lo == nullptr) ? 1 : 0;
+  p.nkb = ceil_div(pl->nlat, 32);
   const int cp = round_up(C, 4), PB = 2 * B;
   p.spec = spec; p.L = pl->lmax; p.M = pl->mmax; p.nlat = pl->nlat; p.C = C; p.cp = cp; p.PB = PB; p.m0 = pl->m0;
   const int maxc = X_lo ? 128 : 256;   // columns per tile (SplitWidths / LegendreWidths)
@@ -936,14 +923,9 @@ int legendre_analysis_umma(const Plan* pl, const float* X, float* spec, int B, i
   return p.split ? SplitWidths::launch_nb<AnaTraits, true>(p, nb, grid, st) : LegendreWidths::launch_nb<AnaTraits, false>(p, nb, grid, st);
 }
 
-// k_begin / k_end: latitude range [k_begin, k_end) to produce (k_begin a multiple of 128; k_end < 0: up to kp)
-int legendre_synthesis_umma(const Plan* pl, const float* spec, float* Z, int B, int C, int tiled, cudaStream_t st, const float* spec_lo, int k_begin,
-                            int k_end) {
+int legendre_synthesis_umma(const Plan* pl, const float* spec, float* Z, int B, int C, int tiled, cudaStream_t st, const float* spec_lo) {
   SynTraits::Params p;
   memset(&p, 0, sizeof(p));
-  if (k_end < 0 || k_end > pl->kp) k_end = pl->kp;
-  B200_REQUIRE(k_begin >= 0 && k_begin % 128 == 0 && k_begin < k_end, "legendre_synthesis: bad latitude range [%d, %d)", k_begin, k_end);
-  p.kc0 = k_begin; p.kc1 = k_end;
   const int cp = round_up(C, 4), PB = 2 * B, JP = PB * cp;
   p.Z = Z; p.L = pl->lmax; p.M = pl->mmax; p.nlat = pl->nlat; p.kp = pl->kp; p.C = C; p.cp = cp; p.PB = PB; p.m0 = pl->m0;
   p.tiled = tiled; p.M2 = (pl->mmax + 7) / 8; p.KT = pl->kp / 8; p.B = B;
@@ -977,12 +959,11 @@ int legendre_synthesis_umma(const Plan* pl, const float* spec, float* Z, int B, 
     p.lo_off = 16384 + 4096 * p.nblk;
   }
   uint32_t out_bytes = 0;
-  if (!p.split) {   // store map of the bulk-store epilogue: boxes of 8 x 16 latitudes x 4 channels, clipped at channel C and latitude kc1
-    B200_REQUIRE(k_end % 8 == 0, "legendre_synthesis: latitude range end %d is not a multiple of 8", k_end);
+  if (!p.split) {   // store map of the bulk-store epilogue: boxes of 8 x 16 latitudes x 4 channels, clipped at channel C and latitude kp
     const long long kp = pl->kp, M2 = p.M2, KT = p.KT;
-    long long d[5] = {8, C, k_end / 8, PB, pl->mmax}, s[5] = {1, kp, 8, C * kp, PB * C * kp};
+    long long d[5] = {8, C, KT, PB, pl->mmax}, s[5] = {1, kp, 8, C * kp, PB * C * kp};
     if (tiled) {
-      const long long d2[5] = {8, C, k_end / 8, 16 * M2, B}, s2[5] = {1, KT * 128 * M2, 128 * M2, 8, C * KT * 128 * M2};
+      const long long d2[5] = {8, C, KT, 16 * M2, B}, s2[5] = {1, KT * 128 * M2, 128 * M2, 8, C * KT * 128 * M2};
       memcpy(d, d2, sizeof(d)); memcpy(s, s2, sizeof(s));
     }
     int bx[5] = {8, 4, 16, 1, 1};
@@ -992,7 +973,7 @@ int legendre_synthesis_umma(const Plan* pl, const float* spec, float* Z, int B, 
   }
   pick_stages(&p, (16384 + 4096 * p.nblk) * (p.split ? 2 : 1), ceil_div(pl->lmax, 32), out_bytes);
   p.tx_bytes = (16384 + 4096 * p.nblk) * (p.split ? 2 : 1);
-  dim3 grid(ceil_div(k_end - k_begin, 128), ceil_div(JP, p.N), tiled ? 8 * p.M2 : pl->mmax);
+  dim3 grid(ceil_div(pl->kp, 128), ceil_div(JP, p.N), tiled ? 8 * p.M2 : pl->mmax);
   return p.split ? SplitWidths::launch_nb<SynTraits, true>(p, nb, grid, st) : LegendreWidths::launch_nb<SynTraits, false>(p, nb, grid, st);
 }
 

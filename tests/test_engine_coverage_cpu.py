@@ -9,7 +9,7 @@ last case off a width, fails this test until a case runs the new instantiation."
 import os
 import re
 
-from test_gpu_engine import CHUNK_GRIDS, LEG_CASES, MIX_CASES, TF32, VEC_CASES, X3, leg_engine_kernels, mix_engine_kernels
+from test_gpu_engine import FORWARD_GRIDS, LEG_CASES, MIX_CASES, TF32, VEC_CASES, X3, leg_engine_kernels, mix_engine_kernels
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 UMMA_CU = os.path.join(ROOT, "makani_b200", "csrc", "umma.cu")
@@ -42,7 +42,7 @@ def test_every_built_instantiation_runs_under_the_bound():
 
 
 def test_the_other_engine_tables_name_built_instantiations():
-    """the chunked and vector Legendre cases assert their instantiations too: they must name kernels the engine builds"""
-    named = {("AnaTraits", c[-1], False) for c in CHUNK_GRIDS}
+    """the SHT forward and vector Legendre cases assert their instantiations too: they must name kernels the engine builds"""
+    named = {("AnaTraits", c[-1], False) for c in FORWARD_GRIDS}
     named |= {k for c in VEC_CASES for s in leg_engine_kernels(c[-1], TF32) for k in s}
     assert named <= built_instantiations(), sorted(named - built_instantiations())

@@ -368,7 +368,7 @@ def test_mix_shapes_outside_the_tensor_cores(case, L, M, B, G, Ci, Co):
     _run_mix(f"fallback-{case}", L, M, B, G, Ci, Co, False, "dhconv", None)
 
 
-# ------------------------------------------------------------------------------------------------ latitude ranges
+# ------------------------------------------------------------------------------------------------ SHT forward
 def _workspace(plan, B, C):
     nbytes = int(_lib.load().b200sht_sht_workspace_bytes(plan.handle, B, C))
     return sentinel(nbytes // 4)
@@ -376,20 +376,17 @@ def _workspace(plan, B, C):
 
 # id, grid, nlat, nlon, lmax, mmax, B, C, dtype (the tensor-core DFT takes fp32 rows when nlon % 32 == 0, bf16 otherwise), tile width NB
 # of the TF32 Legendre analysis (umma_kernel<AnaTraits, NB, false>)
-CHUNK_GRIDS = [
+FORWARD_GRIDS = [
     ("181x360-bf16", "legendre-gauss", 181, 360, 181, 181, 1, 4, torch.bfloat16, 4),
     ("721x1440", "equiangular", 721, 1440, 240, 241, 1, 3, torch.float32, 4),
     ("721x1440-cols128-C64", "equiangular", 721, 1440, 240, 241, 1, 64, torch.float32, 16),
 ]
 
 
-@pytest.mark.parametrize("n", [2, 3, 5])
-@pytest.mark.parametrize("case,grid,nlat,nlon,L,M,B,C,dtype,nb", CHUNK_GRIDS, ids=[c[0] for c in CHUNK_GRIDS])
-def test_chunked_analysis(case, grid, nlat, nlon, L, M, B, C, dtype, nb, n):
-    """b200sht_sht_forward with the (longitude analysis -> Legendre analysis) pair in n latitude chunks (at most nlat / 64): partial sums
-    per chunk, TF32 rounding on the last.  Operands: the latspec the longitude stage left in the workspace (the same rows as one plain
-    b200sht_fft_analysis) and the TF32 table."""
-    lib = _lib.load()
+@pytest.mark.parametrize("case,grid,nlat,nlon,L,M,B,C,dtype,nb", FORWARD_GRIDS, ids=[c[0] for c in FORWARD_GRIDS])
+def test_sht_forward_analysis(case, grid, nlat, nlon, L, M, B, C, dtype, nb):
+    """b200sht_sht_forward at TF32: the (longitude analysis -> Legendre analysis) pair through the workspace.  Operands: the latspec the
+    longitude stage left in the workspace (the same rows as one plain b200sht_fft_analysis) and the TF32 table."""
     plan = mb.get_plan(nlat, nlon, L, M, grid, True, DEV)
     assert plan.umma_ok and plan.dft_ok
     kp, cp = plan.kp, (C + 3) // 4 * 4
@@ -402,47 +399,15 @@ def test_chunked_analysis(case, grid, nlat, nlon, L, M, B, C, dtype, nb, n):
     call("b200sht_fft_analysis", plan.handle, _ptr(x), code, B, C, _ptr(lat0), 0 | 2, st)
     ws = _workspace(plan, B, C)
     coeffs = torch.empty(B, C, L, M, dtype=torch.complex64, device=DEV)
-    old = lib.b200sht_debug_set_lat_chunks(n)
-    try:
-        # the chunks after the first add to the spectrum the earlier ones stored: the profiled launch gets buffers of its own
-        ws_p, coeffs_p = _workspace(plan, B, C), torch.empty_like(coeffs)
-        assert_engine_ran(f"{case} chunks={n}", "analysis", lambda: call("b200sht_sht_forward", plan.handle, _ptr(x), code, B, C, _ptr(coeffs_p), _ptr(ws_p),
-                                                                         TF32, st), {("AnaTraits", nb, False)})
-        call("b200sht_sht_forward", plan.handle, _ptr(x), code, B, C, _ptr(coeffs), _ptr(ws), TF32, st)
-    finally:
-        lib.b200sht_debug_set_lat_chunks(old)
+    assert_engine_ran(case, "analysis", lambda: call("b200sht_sht_forward", plan.handle, _ptr(x), code, B, C, _ptr(coeffs), _ptr(ws), TF32, st),
+                      {("AnaTraits", nb, False)})
     X = ws[:nl].view(M, 2, B, C, kp)
     X0 = lat0[:nl].view(M, 2, B, C, kp)
-    assert torch.equal(X[..., :nlat].view(torch.int32), X0[..., :nlat].view(torch.int32)), "chunked latspec rows != plain fft_analysis"
+    assert torch.equal(X[..., :nlat].view(torch.int32), X0[..., :nlat].view(torch.int32)), "latspec rows != plain fft_analysis"
     spec_off = (4 * plan.latspec_elems(B, C) + 255) // 256 * 256 // 4
     sv = ws[spec_off : spec_off + plan.spec_elems(B, C)].view(L, M, 2, B, cp)
     ref, mag = E.legendre_analysis_ref(E.tf32_rna(plan.table()), E.tf32_trunc(X), nlat, cp)
-    check_spec(f"{case} chunks={n}", "analysis", sv, ref, mag, nlat, C, r=E.R_TF32, floor=E.underflow_floor(nlat, X[..., :nlat]))
+    check_spec(case, "analysis", sv, ref, mag, nlat, C, r=E.R_TF32, floor=E.underflow_floor(nlat, X[..., :nlat]))
     tri = torch.tril(torch.ones(L, M, dtype=torch.bool, device=DEV))
     want = torch.where(tri, torch.complex(sv[:, :, 0, :, :C], sv[:, :, 1, :, :C]).permute(2, 3, 0, 1), 0)
     assert torch.equal(coeffs, want), "coefficients != the packed spectrum in the workspace"
-
-
-@pytest.mark.parametrize("case,grid,nlat,nlon,L,M,B,C,dtype,nb", CHUNK_GRIDS, ids=[c[0] for c in CHUNK_GRIDS])
-def test_chunked_synthesis_is_bit_identical(case, grid, nlat, nlon, L, M, B, C, dtype, nb):
-    """b200sht_sht_inverse / _forward_adjoint with the (Legendre synthesis -> longitude synthesis) pair in 2 or 3 chunks of whole
-    128-row tiles compute every output row exactly as the unchunked call"""
-    lib = _lib.load()
-    plan = mb.get_plan(nlat, nlon, L, M, grid, True, DEV)
-    assert plan.dft_ok and plan.kp > 128
-    st = _stream(DEV)
-    torch.manual_seed(98)
-    c = torch.randn(B, C, L, M, dtype=torch.complex64, device=DEV)
-    for fn in ("b200sht_sht_inverse", "b200sht_sht_forward_adjoint"):
-        ys = []
-        for n in (1, 2, 3):
-            y = torch.full((B, C, nlat, nlon), float("nan"), device=DEV)
-            old = lib.b200sht_debug_set_lat_chunks_syn(n)
-            try:
-                call(fn, plan.handle, _ptr(c), _ptr(y), _lib.F32, B, C, _ptr(_workspace(plan, B, C)), TF32, st)
-            finally:
-                lib.b200sht_debug_set_lat_chunks_syn(old)
-            assert torch.isfinite(y).all()
-            ys.append(y)
-        for n, y in zip((2, 3), ys[1:]):
-            assert torch.equal(y, ys[0]), f"{fn}: {n} latitude chunks changed the result"

@@ -206,7 +206,7 @@ CONV_CASES = [
 ]
 
 
-def _run_conv_case(case, precision, rtol, act_dtype=torch.float32, return_outputs=False):
+def _run_conv_case(case, precision, rtol, act_dtype=torch.float32):
     (nlat_i, nlon_i, grid_i, nlat_o, nlon_o, grid_o, lmax, mmax, B, Cin, Cout, G, op, sep, bias) = case
     torch.manual_seed(333)
     f = mb.RealSHT(nlat_i, nlon_i, lmax, mmax, grid_i, precision=precision)
@@ -244,8 +244,6 @@ def _run_conv_case(case, precision, rtol, act_dtype=torch.float32, return_output
     rel["dweight"] = close(conv.weight.grad, w64.grad, rtol, tag + " dweight")
     if bias:
         rel["dbias"] = close(conv.bias.grad, b64.grad, rtol, tag + " dbias")
-    if return_outputs:   # (relative L2 errors against the oracle, the CUDA tensors themselves)
-        return rel, {"y": y.detach().float().cpu(), "dx": xd.grad.detach().float().cpu(), "dweight": torch.view_as_real(conv.weight.grad.detach()).cpu()}
     return rel
 
 

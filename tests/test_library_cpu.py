@@ -152,9 +152,9 @@ def test_spectral_conv_constructor_contract():
     assert (t.lmax, t.mmax, t.grid) == (64, 65, "equiangular")
 
 
-def test_mix_tensor_core_shape_query_and_switches():
+def test_mix_tensor_core_shape_query_and_pdl_switch():
     """pure host logic of the C ABI: which shapes the tcgen05 mix serves (the caller then packs the weight for that precision), workspace sizes of the
-    pointwise kernels, and the run-time switches return their previous value"""
+    pointwise kernels, and the run-time PDL switch returns its previous value"""
     lib = _lib.load()
     q = lib.b200sht_mix_uses_tensor_cores
     assert q(_lib.OP_DHCONV, 1, 1, 73, 73, _lib.PREC_TF32) == 1
@@ -171,8 +171,6 @@ def test_mix_tensor_core_shape_query_and_switches():
     assert w(0, 5, 63) < 0
     old = lib.b200sht_debug_set_pdl(0)
     assert lib.b200sht_debug_set_pdl(old) == 0
-    old = lib.b200sht_debug_set_lat_chunks(3)
-    assert lib.b200sht_debug_set_lat_chunks(old) == 3
 
 
 def test_pointwise_modules_on_cpu_are_the_torch_operators():
