@@ -136,6 +136,7 @@ int b200sht_fft_analysis(const b200sht_plan* plan, const void* x, int dtype, int
 /* Longitude synthesis: truncated half spectrum -> real rows (+ optional per-channel bias, cast to dtype).
  * scale_mode 0: irfft(norm="forward") semantics (imaginary part of m=0 / Nyquist ignored)
  * scale_mode 1: adjoint of the scale_mode-0 analysis (row_scale = quad_w[k] 2 pi/nlon, modes m>0 halved)
+ * In scale_mode 0 / 1 `latspec` must be 8-byte aligned (B200SHT_ERR_INVALID otherwise); `y` needs only the alignment of its dtype.
  * scale_mode | 2: `latspec` is in the TILED layout written by b200sht_legendre_synthesis_tiled and the transform runs on the tensor
  *                 cores (TF32; radix-8 butterflies on the CUDA cores x a [mmax/8 x nlon/16] DFT matrix as a TF32 GEMM, csrc/dft.cu).
  *                 Error unless b200sht_plan_query(plan, 8) == 1. */

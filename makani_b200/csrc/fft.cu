@@ -869,6 +869,8 @@ int fft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int
     B200_REQUIRE((reinterpret_cast<uintptr_t>(Z) & 127) == 0, "fft_synthesis: the tiled latspec must be 128-byte aligned");
     return dft_synthesis(pl, Z, y, dtype, B, C, bias, scale_mode & 1, st);
   }
+  // the run-time kernels read the latspec as float2 pairs of rows (fill_spectrum), the compile-time ones as float4 when it is 16-byte aligned
+  B200_REQUIRE((reinterpret_cast<uintptr_t>(Z) & 7) == 0, "fft_synthesis: the latspec must be 8-byte aligned");
   FftParams prm = make_params(pl, B, C, scale_mode, bias);
   if (dtype == B200SHT_F32) return run_fft_dir<float>(pl, 1, Z, y, prm, st);
   if (dtype == B200SHT_BF16) return run_fft_dir<__nv_bfloat16>(pl, 1, Z, y, prm, st);

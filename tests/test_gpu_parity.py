@@ -94,40 +94,6 @@ def test_fft_stages(nlat, nlon, mmax, C, dtype):
         assert abs(lhs - rhs) <= 1e-5 * max(abs(lhs), abs(rhs), 1.0), (lhs, rhs)
 
 
-def _ct_nlons():
-    from test_fft_layout import ct_plans
-
-    return sorted(2 * p[3] * p[4] * p[5] for p in ct_plans())
-
-
-@pytest.mark.parametrize("nlon", _ct_nlons())
-@pytest.mark.parametrize("full", [False, True], ids=["truncated", "all-modes"])
-def test_fft_every_compile_time_plan(nlon, full):
-    """every entry of CT_PLANS (fft.cu), truncated (2 mmax <= H: the synthesis skips the zero partner spectrum) and with all
-    nlon/2 + 1 orders, ragged latitude count: analysis against rfft, synthesis against irfft."""
-    torch.manual_seed(333)
-    nlat, B, C = 13, 1, 3
-    mmax = nlon // 2 + 1 if full else max(2, nlon // 6)
-    plan = mb.get_plan(nlat, nlon, 8, mmax, "legendre-gauss", True, torch.device(DEV))
-    x = torch.randn(B, C, nlat, nlon, device=DEV)
-    lat = torch.full((plan.latspec_elems(B, C),), float("nan"), device=DEV)
-    st = mb.sht._stream(x.device)
-    _lib.call("b200sht_fft_analysis", plan.handle, mb.sht._ptr(x), 0, B, C, mb.sht._ptr(lat), 1, st)
-    X = lat[: mmax * 2 * B * C * plan.kp].view(mmax, 2, B * C, plan.kp)
-    got = torch.complex(X[:, 0, :, :nlat], X[:, 1, :, :nlat]).permute(1, 2, 0).reshape(B, C, nlat, mmax)
-    ref = torch.fft.rfft(x.double().cpu(), dim=-1)[..., :mmax]
-    ms = torch.full((mmax,), 2.0, dtype=torch.float64)
-    ms[0] = 1
-    if full:
-        ms[-1] = 1
-    close(got, ref * ms, 3e-6, f"fft_analysis nlon={nlon} mmax={mmax}")
-    Z = torch.randn(mmax, 2, B * C, plan.kp, device=DEV)
-    y = torch.empty(B, C, nlat, nlon, device=DEV)
-    _lib.call("b200sht_fft_synthesis", plan.handle, mb.sht._ptr(Z), mb.sht._ptr(y), 0, B, C, mb.sht._VP(0), 0, st)
-    Zc = torch.complex(Z[:, 0, :, :nlat], Z[:, 1, :, :nlat]).permute(1, 2, 0).reshape(B, C, nlat, mmax).to(torch.complex128).cpu()
-    close(y, torch.fft.irfft(Zc, n=nlon, dim=-1, norm="forward"), 3e-6, f"fft_synthesis nlon={nlon} mmax={mmax}")
-
-
 # --------------------------------------------------------------------------------- RealSHT / InverseRealSHT
 SHT_CASES = [
     ("equiangular", 64, 128, None, None, 1, 8),       # BASELINE configs[0]
