@@ -317,6 +317,33 @@ int b200sht_bias_gelu_forward(const void* x, const float* bias, void* y, int dty
 int b200sht_bias_gelu_backward(const void* x, const float* bias, const void* dy, void* dx, float* row_sums, float* workspace, int dtype, int B, int C, int64_t hw,
                                void* stream);
 
+/* ------------------------------------------------------------------ quadrature-weighted instance norm on the sphere (SURVEY row N2)
+ * Replaces makani's GeometricInstanceNormS2 (makani/models/common/layer_norm.py:30-152) and DistributedGeometricInstanceNormS2
+ * (makani/mpu/layer_norm.py:173-253), staged so that the distributed class can gather the per-rank statistics between the stages; the serial class
+ * calls the same stages with R = 1 and D = 1.  A row (b, c) of x is an H x W plane (the local shard), q: float [H] the latitude weights of its rows,
+ * constant along longitude.  x, y, dy, dx: [B][C][H][W] contiguous, float or bf16 (dtype); gamma / beta: float [C] (null: 1 / 0); B*C <= 65535.
+ *   mu = (1/D) sum q x,  var = (1/D) sum q (x - mu)^2,  r = (var + eps)^-1/2,  xhat = (x - mu) r,  y = [gelu](gamma xhat + beta)
+ *   dx = gamma r (g - (q/D) (S1 + xhat S2 - corr S2)),  S1 = sum g, S2 = sum g xhat over the whole field (g = dy, or dy gelu'(z) when gelu != 0)
+ * partials: double [B*C][3] per row (sum q, mean, M2), the fp64 Welford triple of this shard; sums: double [B*C][2] per row (S1, S2) of this shard;
+ * stats: float [B*C][3] (mu, r, corr = r mu (D - S) / D, S the combined weight).  fp64 buffers and the workspace must be 8-byte aligned;
+ * workspace: b200sht_geometric_norm_workspace_floats floats. */
+int64_t b200sht_geometric_norm_workspace_floats(int B, int C, int64_t hw);
+/* the fp64 triple (sum q, mean, M2) of every row of this shard, sums taken about the pivot x[row, 0] */
+int b200sht_geometric_norm_partials(const void* x, const float* q, double* partials, float* workspace, int dtype, int B, int C, int H, int W, void* stream);
+/* partials: double [R][rows][3], R ranks' triples, combined (Chan / Welford) in rank order; D > 0 the normaliser -> stats */
+int b200sht_geometric_norm_finalize(const double* partials, int R, int rows, double D, float eps, float* stats, void* stream);
+/* y = [gelu](gamma (x - mu) r + beta), written in the dtype of x */
+int b200sht_geometric_norm_apply(const void* x, void* y, const float* gamma, const float* beta, const float* stats, int dtype, int B, int C, int H, int W,
+                                 int gelu, void* stream);
+/* per row of this shard, the unweighted fp64 sums (S1, S2) */
+int b200sht_geometric_norm_backward_sums(const void* x, const void* dy, const float* gamma, const float* beta, const float* stats, double* sums,
+                                         float* workspace, int dtype, int B, int C, int H, int W, int gelu, void* stream);
+/* sums: double [R][rows][2], R ranks' (S1, S2) added in rank order -> dx by the formula above with the row's q[i] / D */
+int b200sht_geometric_norm_backward_apply(const void* x, const void* dy, void* dx, const float* gamma, const float* beta, const float* stats, const double* sums,
+                                          int R, const float* q, double D, int dtype, int B, int C, int H, int W, int gelu, void* stream);
+/* sums: double [B][C][2] of this shard (backward_sums) -> dgamma[c] = sum_b S2, dbeta[c] = sum_b S1 (float [C]; either may be null) */
+int b200sht_geometric_norm_param_grads(const double* sums, float* dgamma, float* dbeta, int B, int C, void* stream);
+
 /* ------------------------------------------------------------------ DISCO convolution on the sphere (SURVEY row N1)
  * Replaces the two sparse contractions of torch_harmonics.DiscreteContinuousConvS2 (built at makani/models/networks/fourcastnet3.py:117-252,
  * :364-381, :511-543, snonet.py).  The filter tensor psi[k, t, i, j] (K kernel functions, output latitude t, input latitude i, input longitude

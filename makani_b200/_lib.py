@@ -89,6 +89,14 @@ _SIGNATURES = {
     "b200sht_instance_norm_backward": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int64, c_int, _P]),
     "b200sht_bias_gelu_forward": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int64, _P]),
     "b200sht_bias_gelu_backward": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int64, _P]),
+    # quadrature-weighted instance norm on the sphere
+    "b200sht_geometric_norm_workspace_floats": (c_int64, [c_int, c_int, c_int64]),
+    "b200sht_geometric_norm_partials": (c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200sht_geometric_norm_finalize": (c_int, [_P, c_int, c_int, ctypes.c_double, c_float, _P, _P]),
+    "b200sht_geometric_norm_apply": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200sht_geometric_norm_backward_sums": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200sht_geometric_norm_backward_apply": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, _P, ctypes.c_double, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200sht_geometric_norm_param_grads": (c_int, [_P, _P, _P, c_int, c_int, _P]),
     # DISCO convolution (row N1)
     "b200sht_disco_plan_create": (c_int, [ctypes.POINTER(_P), c_int, c_int, c_int, c_int, c_int, c_int64, _P, _P, _P, _P, _P]),
     "b200sht_disco_plan_destroy": (c_int, [_P]),

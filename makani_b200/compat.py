@@ -9,6 +9,7 @@ registered in `sys.modules` BEFORE `import makani`:
     import makani_b200.compat as compat
     compat.install_torch_harmonics_shim()      # torch_harmonics -> makani_b200
     compat.patch_makani_spectral_layers()      # makani.models.common.SpectralConv/SpectralAttention -> makani_b200 (optional)
+    compat.patch_makani_norm_layers()          # makani's (Distributed)GeometricInstanceNormS2 -> makani_b200 (optional)
     import makani
 """
 import importlib
@@ -71,3 +72,24 @@ def patch_makani_spectral_layers():
             for name in ("SpectralConv", "SpectralAttention"):
                 if hasattr(m, name):
                     setattr(m, name, getattr(mb, name))
+
+
+def patch_makani_norm_layers():
+    """After `import makani`: point makani's GeometricInstanceNormS2 (makani.models.common, .layer_norm) and DistributedGeometricInstanceNormS2
+    (makani.mpu.layer_norm) at the CUDA-backed classes, including the names the networks imported at module load."""
+    from makani_b200 import distributed as mbd
+    from makani_b200.norm import GeometricInstanceNormS2
+
+    common = importlib.import_module("makani.models.common")
+    common.GeometricInstanceNormS2 = GeometricInstanceNormS2
+    for modname, name, cls in (("makani.models.common.layer_norm", "GeometricInstanceNormS2", GeometricInstanceNormS2),
+                               ("makani.mpu.layer_norm", "DistributedGeometricInstanceNormS2", mbd.DistributedGeometricInstanceNormS2)):
+        m = sys.modules.get(modname) or importlib.import_module(modname)
+        setattr(m, name, cls)
+    for modname in ("makani.models.networks.sfnonet", "makani.models.networks.snonet", "makani.models.networks.fourcastnet3",
+                    "makani.models.networks.fourcastnet3_1"):
+        m = sys.modules.get(modname)
+        if m is not None:
+            for name, cls in (("GeometricInstanceNormS2", GeometricInstanceNormS2), ("DistributedGeometricInstanceNormS2", mbd.DistributedGeometricInstanceNormS2)):
+                if hasattr(m, name):
+                    setattr(m, name, cls)

@@ -62,6 +62,16 @@ int instance_norm_backward(const void* x, const void* dy, void* dx, const float*
                            int B, int C, long long hw, int gelu, cudaStream_t st);
 int bias_gelu_forward(const void* x, const float* bias, void* y, int dtype, int B, int C, long long hw, cudaStream_t st);
 int bias_gelu_backward(const void* x, const float* bias, const void* dy, void* dx, float* row_sums, float* ws, int dtype, int B, int C, long long hw, cudaStream_t st);
+long long geometric_norm_workspace_doubles(int B, int C, long long hw);
+int geometric_norm_partials(const void* x, const float* q, double* partials, double* ws, int dtype, int B, int C, int H, int W, cudaStream_t st);
+int geometric_norm_finalize(const double* partials, int R, int rows, double D, float eps, float* stats, cudaStream_t st);
+int geometric_norm_apply(const void* x, void* y, const float* gamma, const float* beta, const float* stats, int dtype, int B, int C, int H, int W, int gelu,
+                         cudaStream_t st);
+int geometric_norm_backward_sums(const void* x, const void* dy, const float* gamma, const float* beta, const float* stats, double* sums, double* ws, int dtype,
+                                 int B, int C, int H, int W, int gelu, cudaStream_t st);
+int geometric_norm_backward_apply(const void* x, const void* dy, void* dx, const float* gamma, const float* beta, const float* stats, const double* sums, int R,
+                                  const float* q, double D, int dtype, int B, int C, int H, int W, int gelu, cudaStream_t st);
+int geometric_norm_param_grads(const double* sums, float* dgamma, float* dbeta, int B, int C, cudaStream_t st);
 
 static inline cudaStream_t S(void* s) { return static_cast<cudaStream_t>(s); }
 static inline int cp_of(int C) { return round_up(C, 4); }
@@ -783,6 +793,58 @@ int b200sht_bias_gelu_backward(const void* x, const float* bias, const void* dy,
   if (rc) return rc;
   B200_REQUIRE(dx && workspace, "bias_gelu_backward: null argument");
   return bias_gelu_backward(x, bias, dy, dx, row_sums, workspace, dtype, B, C, hw, S(stream));
+}
+
+// ------------------------------------------------------------------------------ quadrature-weighted instance norm on the sphere
+int64_t b200sht_geometric_norm_workspace_floats(int B, int C, int64_t hw) {
+  if (B <= 0 || C <= 0 || hw <= 0) return -1;
+  return 2 * (int64_t)geometric_norm_workspace_doubles(B, C, hw);
+}
+static int check_aligned8(const void* p, const char* who) {
+  B200_REQUIRE(p && (reinterpret_cast<uintptr_t>(p) & 7) == 0, "%s: null or not 8-byte aligned fp64 buffer", who);
+  return 0;
+}
+int b200sht_geometric_norm_partials(const void* x, const float* q, double* partials, float* workspace, int dtype, int B, int C, int H, int W, void* stream) {
+  int rc = check_pointwise(x, q, dtype, "geometric_norm_partials");
+  if (!rc) rc = check_aligned8(partials, "geometric_norm_partials");
+  if (!rc) rc = check_aligned8(workspace, "geometric_norm_partials");
+  if (rc) return rc;
+  return geometric_norm_partials(x, q, partials, reinterpret_cast<double*>(workspace), dtype, B, C, H, W, S(stream));
+}
+int b200sht_geometric_norm_finalize(const double* partials, int R, int rows, double D, float eps, float* stats, void* stream) {
+  int rc = check_aligned8(partials, "geometric_norm_finalize");
+  if (rc) return rc;
+  B200_REQUIRE(stats, "geometric_norm_finalize: null stats");
+  return geometric_norm_finalize(partials, R, rows, D, eps, stats, S(stream));
+}
+int b200sht_geometric_norm_apply(const void* x, void* y, const float* gamma, const float* beta, const float* stats, int dtype, int B, int C, int H, int W,
+                                 int gelu, void* stream) {
+  int rc = check_pointwise(x, y, dtype, "geometric_norm_apply");
+  if (rc) return rc;
+  B200_REQUIRE(stats, "geometric_norm_apply: null stats");
+  return geometric_norm_apply(x, y, gamma, beta, stats, dtype, B, C, H, W, gelu, S(stream));
+}
+int b200sht_geometric_norm_backward_sums(const void* x, const void* dy, const float* gamma, const float* beta, const float* stats, double* sums,
+                                         float* workspace, int dtype, int B, int C, int H, int W, int gelu, void* stream) {
+  int rc = check_pointwise(x, dy, dtype, "geometric_norm_backward_sums");
+  if (!rc) rc = check_aligned8(sums, "geometric_norm_backward_sums");
+  if (!rc) rc = check_aligned8(workspace, "geometric_norm_backward_sums");
+  if (rc) return rc;
+  B200_REQUIRE(stats, "geometric_norm_backward_sums: null stats");
+  return geometric_norm_backward_sums(x, dy, gamma, beta, stats, sums, reinterpret_cast<double*>(workspace), dtype, B, C, H, W, gelu, S(stream));
+}
+int b200sht_geometric_norm_backward_apply(const void* x, const void* dy, void* dx, const float* gamma, const float* beta, const float* stats, const double* sums,
+                                          int R, const float* q, double D, int dtype, int B, int C, int H, int W, int gelu, void* stream) {
+  int rc = check_pointwise(x, dy, dtype, "geometric_norm_backward_apply");
+  if (!rc) rc = check_aligned8(sums, "geometric_norm_backward_apply");
+  if (rc) return rc;
+  B200_REQUIRE(dx && stats && q, "geometric_norm_backward_apply: null argument");
+  return geometric_norm_backward_apply(x, dy, dx, gamma, beta, stats, sums, R, q, D, dtype, B, C, H, W, gelu, S(stream));
+}
+int b200sht_geometric_norm_param_grads(const double* sums, float* dgamma, float* dbeta, int B, int C, void* stream) {
+  int rc = check_aligned8(sums, "geometric_norm_param_grads");
+  if (rc) return rc;
+  return geometric_norm_param_grads(sums, dgamma, dbeta, B, C, S(stream));
 }
 
 int b200sht_debug_set_pdl(int on) {

@@ -492,3 +492,4 @@ class DistributedInverseRealVectorSHT(_DistributedBase):
 from .disco import DistributedDiscreteContinuousConvS2, DistributedDiscreteContinuousConvTransposeS2, set_disco_local_ops  # noqa: E402,F401
 from .resample import DistributedResampleS2, set_resample_local_ops  # noqa: E402,F401
 from .attention import DistributedNeighborhoodAttentionS2, set_attention_local_ops  # noqa: E402,F401
+from .norm import DistributedGeometricInstanceNormS2, set_norm_local_ops  # noqa: E402,F401

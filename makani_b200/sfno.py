@@ -212,10 +212,11 @@ class NeuralOperatorBlock(nn.Module):
         return gain
 
     def forward(self, x):
+        from .norm import GeometricInstanceNormS2
         from .norm import InstanceNorm2d as FusedInstanceNorm2d
 
         x, residual = self.filter(x)
-        if (isinstance(self.norm0, FusedInstanceNorm2d) and not hasattr(self, "inner_skip") and isinstance(self.act_layer0, nn.GELU)
+        if (isinstance(self.norm0, (FusedInstanceNorm2d, GeometricInstanceNormS2)) and not hasattr(self, "inner_skip") and isinstance(self.act_layer0, nn.GELU)
                 and getattr(self.act_layer0, "approximate", "none") == "none"):
             x = self.norm0(x, gelu=True)     # norm0 -> GELU in one pass (sfnonet.py:387-392 with inner_skip "none")
         else:
@@ -262,8 +263,18 @@ class SphericalFourierNeuralOperatorNet(nn.Module):
             from .norm import InstanceNorm2d as FusedInstanceNorm2d   # nn.InstanceNorm2d subclass: same parameters / state dict, CUDA kernels of csrc/norm.cu
 
             norm = partial(FusedInstanceNorm2d, num_features=embed_dim, eps=1e-6, affine=True, track_running_stats=False)
+            norm_inp = norm_mid = norm_out = norm
+        elif normalization_layer == "instance_norm_s2":
+            from .norm import GeometricInstanceNormS2   # quadrature-weighted statistics on the model grid, CUDA kernels of csrc/norm.cu
+
+            def s2norm(shape):
+                return partial(GeometricInstanceNormS2, img_shape=shape, crop_shape=shape, crop_offset=(0, 0), grid_type=model_grid_type,
+                               num_features=embed_dim, eps=1e-6, affine=True)
+
+            norm_inp = norm_mid = s2norm((self.h, self.w))
+            norm_out = s2norm(self.out_shape)     # the last block's filter returns the output grid (sfnonet.py:622-649)
         elif normalization_layer == "none":
-            norm = nn.Identity
+            norm_inp = norm_mid = norm_out = nn.Identity
         else:
             raise NotImplementedError(f"Error, normalization {normalization_layer} not implemented.")
 
@@ -271,8 +282,9 @@ class SphericalFourierNeuralOperatorNet(nn.Module):
         for i in range(num_layers):
             fwd = self.trans_down if i == 0 else self.trans
             inv = self.itrans_up if i == num_layers - 1 else self.itrans
+            norms = (norm_inp, norm_mid) if i == 0 else (norm_out, norm_out) if i == num_layers - 1 else (norm_mid, norm_mid)
             self.blocks.append(NeuralOperatorBlock(fwd, inv, embed_dim, filter_type=filter_type, operator_type=operator_type, mlp_ratio=mlp_ratio,
-                                                   mlp_drop_rate=mlp_drop_rate, path_drop_rate=dpr[i], act_layer=act, norm_layer=(norm, norm),
+                                                   mlp_drop_rate=mlp_drop_rate, path_drop_rate=dpr[i], act_layer=act, norm_layer=norms,
                                                    inner_skip="none", outer_skip="linear", use_mlp=use_mlp, rank=rank, separable=separable,
                                                    complex_activation=complex_activation, spectral_layers=spectral_layers, bias=bias,
                                                    checkpointing_level=checkpointing_level, backend=backend))
