@@ -15,9 +15,10 @@
 //   S -> V(j2), V(N2-j2) -> twiddle -> radix-8 -> scale/bias -> bf16 into a shared-memory output tile, written out by TMA bulk stores.
 // analysis kernel (rows -> latspec):    producer warps load the eight samples x[N2 j1 + j2] of a column (lanes = consecutive j2),
 //   butterfly + twiddle them and write the even/odd combinations (Ye, Yo) as K-major TF32 operand tiles [(c, k)][j2] (128-byte
-//   swizzle, conflict-free row stores); B = E resident (<= 24 KB); eight MMA warps (one class each) accumulate D[(c,k)][m2] in registers
-//   over the K-blocks and write latspec straight from their fragments (32-byte runs along k).
+//   swizzle, conflict-free row stores); B = E resident (<= 24 KB); two warpgroups contract them with wgmma.m64n32k8 (one class per warp)
+//   into D[(c,k)][m2] in registers over the K-blocks and write latspec straight from their fragments (32-byte runs along k).
 #include "umma_common.cuh"
+#include "wgmma_tf32.cuh"
 #include "dft_math.cuh"
 #include <cmath>
 #include <cstdlib>
@@ -160,6 +161,14 @@ __device__ __forceinline__ void prof_wait(unsigned long long* prof, int slot, ui
   mbar_wait(bar, parity);
   if (lead) atomicAdd(prof + slot, (unsigned long long)(clock64() - t0));
 }
+// the same for the kernel that holds wgmma (the analysis): a lost arrival traps without the printf, whose call would make ptxas serialize
+// every wgmma of the kernel; the counters are inline shared-memory atomics, so the profile build keeps the wgmma asynchronous too
+__device__ __forceinline__ void prof_wait_nocall(unsigned long long* prof, int slot, uint64_t* bar, uint32_t parity, bool lead) {
+  if (!kDftProfile || prof == nullptr) { mbar_wait_nocall(bar, parity); return; }
+  const long long t0 = clock64();
+  mbar_wait_nocall(bar, parity);
+  if (lead) atomicAdd(prof + slot, (unsigned long long)(clock64() - t0));
+}
 
 // 3-D view (nlon, nlat, rows) of the synthesis output, box (ow, 8, 1), no swizzle
 static int make_tmap_out(CUtensorMap* tm, void* base, bool bf16, int nlon, int nlat, long long rows, int ow) {
@@ -282,7 +291,8 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
   const uint32_t sA = base, sB = base + 32768, sO = sB + kDftSynStages * 16384;
   T* const outS = reinterpret_cast<T*>(gbase + (sO - base));
   float2* tws = reinterpret_cast<float2*>(gbase + (sO - base) + 2 * obytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(tws) + ((8 * N2 * 8 + 15) & ~15));
+  int* oofs = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(tws) + ((8 * N2 * 8 + 15) & ~15));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(oofs) + 8 * N2 * 4);
   uint64_t* full = bars;
   uint64_t* empty = full + kDftSynStages;
   uint64_t* e_full = empty + kDftSynStages;
@@ -305,6 +315,10 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
     prefetch_tmap(&p.tmY);
   }
   for (int i = threadIdx.x; i < 8 * p.N2; i += blockDim.x) tws[i] = p.tw[i];
+  for (int i = threadIdx.x; i < 8 * N2; i += blockDim.x) {   // output tile position of the longitude N2 j1 + j2 (row 0) at [j2][j1]
+    const int j = N2 * (i & 7) + (i >> 3);
+    oofs[i] = (j / ow) * 8 * ow + j % ow;
+  }
   __syncthreads();
   const long long t_cta0 = (kDftProfile && p.prof && threadIdx.x == 0) ? clock64() : 0;
   pdl_wait();   // the prologue read plan constants only (twiddles); the latspec tiles, bias and y belong to other kernels until here
@@ -349,6 +363,14 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
     const float smul = p.mode == 0 ? 2.f : 1.f;
     const int nyq_m = nlon / 2;
     const uint8_t* const gE = gbase;
+    // B fragment of the class c: K rows kk + q (+ 4), column 8 c + lane / 4 of the MN-major latspec stage.  Under the 128-byte swizzle the
+    // XOR term of those rows is (q (+ 4)) << 4 for every kk, so the lane's byte offset of column 8 (c % 4) + lane / 4 is fixed; the class
+    // block c / 4 (4096 B), kk (128 B rows) and the imaginary plane (8192 B) only add to it.
+    uint32_t zoff[2][4];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int cc = 0; cc < 4; ++cc) zoff[h][cc] = swz128((uint32_t)((kpi + 4 * h) * 128 + (8 * cc + (lane >> 2)) * 4));
     mbar_wait(e_full, 0);
     for (int task = warp; warp < nwork; task += nwork) {
       const int n = task / nblk, blk = task - n * nblk;   // tile n of this CTA, 8-column block blk
@@ -392,10 +414,11 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
           uint32_t fa[4];
           frag_a<false>(gE, 16 * blk, kk, fa);
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            uint32_t zr[2], zi[2];
-            frag_b<true>(zs, 8 * c, kk, zr);
-            frag_b<true>(zs + 8192, 8 * c, kk, zi);
+          for (int c = 0; c < 8; ++c) {   // frag_b<true>(zs (+ 8192), 8 c, kk) with the lane's swizzled offsets hoisted out of the task loop
+            const uint8_t* const zc = zs + (c >> 2) * 4096 + kk * 128;
+            const uint32_t zr[2] = {*reinterpret_cast<const uint32_t*>(zc + zoff[0][c & 3]), *reinterpret_cast<const uint32_t*>(zc + zoff[1][c & 3])};
+            const uint32_t zi[2] = {*reinterpret_cast<const uint32_t*>(zc + 8192 + zoff[0][c & 3]),
+                                    *reinterpret_cast<const uint32_t*>(zc + 8192 + zoff[1][c & 3])};
             mma_tf32(acc[0][c], fa, zr);
             mma_tf32(acc[1][c], fa, zi);
           }
@@ -425,11 +448,13 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
           }
           dft_syn_radix8<pr>(vr, vi, tw, x);
           const pr o0 = (j2 & 1) ? off_o : off_e, o1 = (j2 & 1) ? off_e : off_o;
+          const int4* const op = reinterpret_cast<const int4*>(oofs + 8 * (valid ? j2 : 0));
+          const int4 oa = op[0], ob4 = op[1];
+          const int of[8] = {oa.x, oa.y, oa.z, oa.w, ob4.x, ob4.y, ob4.z, ob4.w};
 #pragma unroll
-          for (int j1 = 0, bx = j2 / ow, jx = j2 - bx * ow; j1 < 8; ++j1) {   // longitude N2 j1 + j2 = bx ow + jx
+          for (int j1 = 0; j1 < 8; ++j1) {   // longitude N2 j1 + j2
             const pr o = rfma(x[j1], sc, (n2odd && (j1 & 1)) ? o1 : o0);
-            if (valid) { st_out<T>(ob + bx * 8 * ow + jx, o.v.x); st_out<T>(ob + bx * 8 * ow + jx + ow, o.v.y); }
-            for (jx += N2; jx >= ow; jx -= ow) ++bx;
+            if (valid) { st_out<T>(ob + of[j1], o.v.x); st_out<T>(ob + of[j1] + ow, o.v.y); }
           }
         }
         {
@@ -441,11 +466,13 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
           }
           dft_syn_radix8<pr>(vr, vi, tp, x);
           const pr o0 = (jp & 1) ? off_o : off_e, o1 = (jp & 1) ? off_e : off_o;
+          const int4* const op = reinterpret_cast<const int4*>(oofs + 8 * (paired ? jp : 0));
+          const int4 oa = op[0], ob4 = op[1];
+          const int of[8] = {oa.x, oa.y, oa.z, oa.w, ob4.x, ob4.y, ob4.z, ob4.w};
 #pragma unroll
-          for (int j1 = 0, bx = jp / ow, jx = jp - bx * ow; j1 < 8; ++j1) {   // not for the unpaired columns 0 and N2 / 2
+          for (int j1 = 0; j1 < 8; ++j1) {   // not for the unpaired columns 0 and N2 / 2
             const pr o = rfma(x[j1], sc, (n2odd && (j1 & 1)) ? o1 : o0);
-            if (paired) { st_out<T>(ob + bx * 8 * ow + jx, o.v.x); st_out<T>(ob + bx * 8 * ow + jx + ow, o.v.y); }
-            for (jx += N2; jx >= ow; jx -= ow) ++bx;
+            if (paired) { st_out<T>(ob + of[j1], o.v.x); st_out<T>(ob + of[j1] + ow, o.v.y); }
           }
         }
         fence_proxy_async();   // the bulk stores read the tile through the async proxy: every writing thread fences and arrives
@@ -493,7 +520,7 @@ int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int
   }
   const size_t obytes = (8 * (size_t)pl->nlon * (bf16 ? 2 : 4) + 1023) & ~(size_t)1023;
   const size_t smem = 1024 + 32768 + (size_t)kDftSynStages * 16384 + 2 * obytes + ((8 * (size_t)t->N2 * 8 + 15) & ~(size_t)15) +
-                      (2 * kDftSynStages + 5) * 8;
+                      8 * (size_t)t->N2 * 4 + (2 * kDftSynStages + 5) * 8;
   const int sms = usable_sms(pl->sm_count > 0 ? pl->sm_count : 132);
   const int ctas = p.ntiles < sms ? p.ntiles : sms;
 #define B200_LAUNCH_SYN(TT)                                                                                          \
@@ -539,7 +566,7 @@ static int make_tmap_segments(CUtensorMap* tm, const void* base, bool bf16, int 
 }
 
 constexpr int kDftAnaStages = 2;   // operand ring: one stage = one K-block (32 columns) of a 16-row tile = 4 planes x 16 KB
-constexpr int kDftAnaMma = 8, kDftAnaLoader = 8, kDftAnaProd0 = 9, kDftAnaThreads = 512;   // warp roles (below)
+constexpr int kDftAnaMma = 8, kDftAnaLoader = 8, kDftAnaProd0 = 9, kDftAnaThreads = 544;   // warp roles (below)
 
 struct DftAnaParams {
   alignas(64) CUtensorMap tmB;   // E tiles (32 j2 local, nkb * 64 rows), box (32, 32): K-major B operand
@@ -552,10 +579,9 @@ struct DftAnaParams {
   int R, nlat, nlon, kp, mmax, N2, half, M2, nkb, mode, ntiles, ktiles, nraw, gs;   // ktiles: 16-row tiles per image
 };
 
-// warps: 0..7 MMA + epilogue (rows 16 w .. + 15 of the tile = class w), 8 loader (TMA: the resident B, then the samples), 9..15 producers.
-// 16 warps = 4 per SM sub-partition, so every warp gets 128 registers: no spills.  The MMA warps were the bottleneck with four warps of two
-// classes each (the producers waited for a free operand stage 63 % of the time); one class per warp halves their serial MMA + epilogue work
-// per tile and gives each sub-partition two of them.
+// warps: 0..7 MMA + epilogue, two warpgroups of wgmma (rows 16 w .. + 15 of the tile = class w), 8 loader (TMA: the resident B, then the
+// samples), 9..16 producers.  On wgmma the MMA warps issue a few instructions per K-block and sleep in their waits, so the issue slots go to
+// the producers: eight of them (one item of every K-block each) at 17 warps and 120 registers, no spills.
 // shared memory: [B resident: nkb x (cos 4 KB | sin 4 KB)][A ring: 2 x 4 planes x 16 KB][raw ring: nraw x 16 boxes][twiddles][barriers]
 //
 // Data flow of one (tile, K-block): the loader thread brings the 8 + 8 sample boxes the K-block needs -- for each j1 the 32 columns
@@ -608,7 +634,7 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
     twS[i] = w;
   }
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kDftAnaStages; ++s) { mbar_init(&full[s], 8); mbar_init(&empty[s], kDftAnaMma); }   // a K-block = 8 row pairs
+    for (int s = 0; s < kDftAnaStages; ++s) { mbar_init(&full[s], 8 * 32); mbar_init(&empty[s], kDftAnaMma); }   // a K-block = 8 row pairs
     for (int s = 0; s < p.nraw; ++s) { mbar_init(&raw_full[s], 1); mbar_init(&raw_empty[s], 8); }
     mbar_init(b_full, 1);
     fence_barrier_init();
@@ -621,6 +647,7 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
     const int st = i >> 10, pl = (i >> 9) & 1, off = i & 511;
     reinterpret_cast<float*>(gA + (size_t)st * 65536)[(pl ? 12288 : 4096) + off] = 0.f;
   }
+  fence_proxy_async();   // wgmma reads them through the async proxy
   __syncthreads();
   const long long t_cta0 = (kDftProfile && p.prof && threadIdx.x == 0) ? clock64() : 0;
   pdl_wait();   // the prologue read plan constants only (twiddles); samples and latspec belong to other kernels until here
@@ -638,7 +665,7 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
         const int r = ti / p.ktiles, row0 = r * p.nlat + (ti - r * p.ktiles) * 16;
         for (int kb = 0; kb < nkb; ++kb) {
           const int g = n * nkb + kb, rs = g % p.nraw, it = g / p.nraw;
-          if (it > 0) prof_wait(prof, 2, &raw_empty[rs], (it - 1) & 1, true);
+          if (it > 0) prof_wait_nocall(prof, 2, &raw_empty[rs], (it - 1) & 1, true);
           mbar_expect_tx(&raw_full[rs], kRawBytes);
           const uint32_t dst = sRaw + rs * kRawBytes;
 #pragma unroll
@@ -655,63 +682,45 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
     __syncwarp();
   } else if (warp < kDftAnaMma) {
     // ------------------------------------------------------------------------------------------- MMA + epilogue
-    // D[(c, kr)][m2] = Xre: Ye_r cos + Yo_i sin,  Xim: Ye_i cos - Yo_r sin over the j2 of all K-blocks.  The m16 tile of this warp is class
-    // c = warp, its fragment rows are the latitudes kr = lane / 4 (+ 8), its columns the orders m2 = 8 j + 2 (lane % 4) (+ 1).
-    // K order: the sum over j2 is order-free, so within a K-block the thread of q = lane % 4 takes the columns 8 q .. 8 q + 7 -- two
-    // 16-byte loads per operand row, conflict-free under the 128-byte swizzle -- and step t of the four m16n8k8 steps contracts the columns
-    // 8 q + 2 t (fragment column q) and 8 q + 2 t + 1 (fragment column q + 4) of both operands.
+    // D[(c, kr)][m2] = Xre: Ye_r cos + Yo_i sin,  Xim: Ye_i cos - Yo_r sin over the j2 of all K-blocks, on wgmma.m64n32k8: warpgroup wg
+    // takes the rows 64 wg .. + 63 of the operand stage (classes 4 wg .. 4 wg + 3) against the 32 orders m2 of the resident E, four
+    // products per k8 step, the negated one through the instruction's B scale.  Each warp's part of the m64n32 accumulator is the m16n8
+    // fragment layout repeated: class c = warp, rows the latitudes kr = lane / 4 (+ 8), columns the orders m2 = 8 j + 2 (lane % 4) (+ 1).
+    // One K-block's wgmma stay in flight: the stage before is released once wait_group 1 has retired its group.  No function call may
+    // appear in this kernel (ptxas would serialize every wgmma): all its waits are the call-free ones.
     const size_t plane = (size_t)p.R * p.kp;
     const int c = warp, gq = lane >> 2, q = lane & 3;
-    mbar_wait(b_full, 0);
+    const uint32_t aw = sAr + (uint32_t)(warp >> 2) * 8192;   // this warpgroup's 64 rows of plane Ye_r of stage 0
+    mbar_wait_nocall(b_full, 0);
     int n = 0;
     for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
       const int r = ti / p.ktiles, k0 = (ti - r * p.ktiles) * 16;
-      float xr[4][4], xi[4][4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) { xr[j][e] = 0.f; xi[j][e] = 0.f; }
+      float acc[8][4];   // [0..3]: Xre, [4..7]: Xim, columns 8 j .. 8 j + 7
+      int prev = 0;
       for (int kb = 0; kb < nkb; ++kb) {
         const int g = n * nkb + kb, s = g % kDftAnaStages, it = g / kDftAnaStages;
-        prof_wait(prof, 3, &full[s], it & 1, lane == 0);
-        const uint8_t* const a0 = gA + (size_t)s * 65536;
-        const uint8_t* const bc = gbase + oB + kb * 8192;
+        prof_wait_nocall(prof, 3, &full[s], it & 1, lane == 0);
+        const uint32_t a0 = aw + (uint32_t)s * 65536;   // planes Ye_r, Ye_i, Yo_r, Yo_i, 16 KB apart
+        const uint64_t d_er = wgmma_desc_kmajor(a0), d_ei = wgmma_desc_kmajor(a0 + 16384);
+        const uint64_t d_or = wgmma_desc_kmajor(a0 + 32768), d_oi = wgmma_desc_kmajor(a0 + 49152);
+        const uint64_t d_c = wgmma_desc_kmajor(sBm + kb * 8192), d_s = wgmma_desc_kmajor(sBm + kb * 8192 + 4096);
+        wgmma_fence();
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {   // columns 8 q + 4 half .. + 3: steps t = 2 half, 2 half + 1
-          const uint32_t col = 32 * q + 16 * half;
-          uint4 av[4][2];   // [plane][row g, g + 8]
-#pragma unroll
-          for (int pl = 0; pl < 4; ++pl)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) av[pl][h] = lds128(a0 + pl * 16384, (16 * c + gq + 8 * h) * 128 + col);
-          // cos: Xre += Ye_r cos, Xim += Ye_i cos;  sin: Xre += Yo_i sin, Xim -= Yo_r sin.  Consecutive MMAs into the same accumulator are
-          // eight apart, so the dependent ones do not issue back to back.
-#pragma unroll
-          for (int cs = 0; cs < 2; ++cs) {
-            uint4 bv[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) bv[j] = lds128(bc + cs * 4096, (8 * j + gq) * 128 + col);
-            const int pr_ = cs ? 3 : 0, pi_ = cs ? 2 : 1;
-#pragma unroll
-            for (int t = 0; t < 2; ++t) {
-              uint32_t far_[4], fai[4];
-              far_[0] = t ? av[pr_][0].z : av[pr_][0].x; far_[1] = t ? av[pr_][1].z : av[pr_][1].x;
-              far_[2] = t ? av[pr_][0].w : av[pr_][0].y; far_[3] = t ? av[pr_][1].w : av[pr_][1].y;
-              fai[0] = t ? av[pi_][0].z : av[pi_][0].x; fai[1] = t ? av[pi_][1].z : av[pi_][1].x;
-              fai[2] = t ? av[pi_][0].w : av[pi_][0].y; fai[3] = t ? av[pi_][1].w : av[pi_][1].y;
-              if (cs) frag_neg(fai, fai);   // - Yo_r
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const uint32_t fb[2] = {t ? bv[j].z : bv[j].x, t ? bv[j].w : bv[j].y};
-                mma_tf32(xr[j], far_, fb);
-                mma_tf32(xi[j], fai, fb);
-              }
-            }
-          }
+        for (int k = 0; k < 4; ++k) {
+          const int sd = (kb > 0 || k > 0) ? 1 : 0;   // the first product of a tile initializes the accumulators
+          wgmma_tf32<32, 1, 8, 0>(acc, d_er + 2 * k, d_c + 2 * k, sd);    // Xre += Ye_r cos
+          wgmma_tf32<32, 1, 8, 4>(acc, d_ei + 2 * k, d_c + 2 * k, sd);    // Xim += Ye_i cos
+          wgmma_tf32<32, 1, 8, 0>(acc, d_oi + 2 * k, d_s + 2 * k, 1);     // Xre += Yo_i sin
+          wgmma_tf32<32, -1, 8, 4>(acc, d_or + 2 * k, d_s + 2 * k, 1);    // Xim -= Yo_r sin
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[s]);   // this warp's reads of the stage are done
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);   // this warp's wgmma of the K-block before have read its stage
+        prev = s;
       }
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc);
+      if (lane == 0) mbar_arrive(&empty[prev]);
       if (prof && lane == 0) atomicAdd(prof + 5, 1ull);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -731,8 +740,8 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
             // by 1 + 2^-10 / 3.
             const float sc = ((p.mode == 0) ? rs : ((m == 0 || 2 * m == p.nlon) ? 1.f : 2.f)) * kTruncComp;
             float* dst = xb + (size_t)m * 2 * plane;
-            dst[0] = __uint_as_float(__float_as_uint(xr[j][2 * h + e] * sc) & 0xffffe000u);
-            dst[plane] = __uint_as_float(__float_as_uint(xi[j][2 * h + e] * sc) & 0xffffe000u);
+            dst[0] = __uint_as_float(__float_as_uint(acc[j][2 * h + e] * sc) & 0xffffe000u);
+            dst[plane] = __uint_as_float(__float_as_uint(acc[4 + j][2 * h + e] * sc) & 0xffffe000u);
           }
       }
     }
@@ -757,7 +766,7 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
         const int g = n * nkb + kb;
         const int j2 = 32 * kb + lane;
         const int rs = g % p.nraw;
-        prof_wait(prof, 0, &raw_full[rs], (g / p.nraw) & 1, lane == 0);
+        prof_wait_nocall(prof, 0, &raw_full[rs], (g / p.nraw) & 1, lane == 0);
         if (prof && lane == 0) atomicAdd(prof + 7, 1ull);
         const T* const rb = rawS + (size_t)rs * (kRawBytes / sizeof(T));
         pr xa[8], xb[8];
@@ -785,8 +794,6 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
             xb[j1] = make_pr(reinterpret_cast<const float*>(b1)[ip], reinterpret_cast<const float*>(b1)[rowp + ip]);
           }
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&raw_empty[rs]);   // samples are in registers: the raw stage may be refilled
         if (kb == 0) {                                 // column 0 has no partner
 #pragma unroll
           for (int j1 = 0; j1 < 8; ++j1) xb[j1] = (lane == 0) ? make_pr(0.f, 0.f) : xb[j1];
@@ -808,8 +815,12 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
         dft_partner_twiddles(tw, tp);   // products of the tw components with constants of modulus 1: they carry the (1 + f) factor too
         dft_ana_radix8<pr>(xa, tw, er, ei);
         dft_ana_radix8<pr>(xb, tp, br, bi);
+        // the raw stage may be refilled once every lane's shared-memory loads of it have completed: the butterflies have consumed them.  (An
+        // arrival right after issuing the loads let the next TMA box overwrite samples that were still being read.)
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&raw_empty[rs]);
         const int s = g % kDftAnaStages, it = g / kDftAnaStages;
-        if (it > 0) prof_wait(prof, 1, &empty[s], (it - 1) & 1, lane == 0);
+        if (it > 0) prof_wait_nocall(prof, 1, &empty[s], (it - 1) & 1, lane == 0);
         float* const stg = reinterpret_cast<float*>(gA + (size_t)s * 65536);
         const int kr0 = 2 * q;
         // swizzled K-major position of (row c * 16 + kr, column lane): the XOR term depends on kr only (16 c is a multiple of 8)
@@ -828,9 +839,8 @@ __global__ void __launch_bounds__(kDftAnaThreads, 1) dft_analysis_kernel(const _
             d0[12288 + c * 512] = yo_i.v.x; d1[12288 + c * 512] = yo_i.v.y;
           }
         }
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&full[s]);
+        fence_proxy_async();   // wgmma reads the stage through the async proxy: every writing thread fences and arrives
+        mbar_arrive(&full[s]);
       }
     }
   }

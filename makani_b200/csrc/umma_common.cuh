@@ -117,7 +117,7 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) { asm volat
 //   K-major:  row r (an M or N index) holds 32 consecutive K values
 //   MN-major: blocks of [32 K-rows][32 consecutive M / N values], 4096 bytes apart
 // Hopper's wgmma reads TF32 operands from shared memory only K-major: umma.cu runs its GEMMs with two K-major operands on it (descriptors
-// below), the others on mma.m16n8k8.  The m16n8k8 fragments below (used by dft.cu) are loaded element by element, so both layouts feed the
+// below), and so does the analysis of dft.cu; the others run on mma.m16n8k8.  The m16n8k8 fragments below (used by dft.cu) are loaded element by element, so both layouts feed the
 // same instruction; the GEMM engine of umma.cu loads permuted fragments with 8- and 16-byte loads instead.
 __device__ __forceinline__ uint32_t swz128(uint32_t off) { return off ^ ((off >> 3) & 0x70u); }
 template <bool MN>

@@ -35,7 +35,7 @@ ctas = torch.cuda.get_device_properties(0).multi_processor_count   # one persist
 life = a[6] / ctas
 print(f"analysis: CTA lifetime {life:.0f} clk; items {a[7]:.0f}")
 names = ["producers wait samples (per warp)", "producers wait operand stage (per warp)", "loader waits raw stage", "MMA warps wait operand (per warp)"]
-div = [7, 7, 1, 8]   # warps per role in dft_analysis_kernel: producers, producers, loader, MMA
+div = [8, 8, 1, 8]   # warps per role in dft_analysis_kernel: producers, producers, loader, MMA
 for i, nme in enumerate(names):
     print(f"  {nme:45s} {a[i] / ctas / div[i]:10.0f} clk  = {100 * a[i] / ctas / div[i] / life:5.1f}% of the CTA lifetime")
 for _ in range(2):
