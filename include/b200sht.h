@@ -344,6 +344,21 @@ int b200sht_geometric_norm_backward_apply(const void* x, const void* dy, void* d
 /* sums: double [B][C][2] of this shard (backward_sums) -> dgamma[c] = sum_b S2, dbeta[c] = sum_b S1 (float [C]; either may be null) */
 int b200sht_geometric_norm_param_grads(const double* sums, float* dgamma, float* dbeta, int B, int C, void* stream);
 
+/* ------------------------------------------------------------------ channel layer norm (SURVEY row N2)
+ * Replaces makani's DistributedLayerNorm (makani/mpu/layer_norm.py:256-290: nn.LayerNorm(C) applied to an NCHW activation through two transposes),
+ * reducing over the channel axis in place.  x, dx: [B][C][hw] contiguous in dtype; y, dy: [B][C][hw] contiguous in out_dtype, which is dtype, or
+ * B200SHT_F32 for a bf16 x (makani's layer under autocast returns fp32).  gamma / beta: float [C] (null: 1 / 0).  Per grid point (b, p):
+ *   mu = mean_c x, var = mean_c (x - mu)^2 (biased), r = (var + eps)^-1/2, xhat = (x - mu) r, y = [gelu](gamma_c xhat + beta_c)
+ *   dx = r (gamma g - mean_c(gamma g) - xhat mean_c(gamma g xhat)),  g = dy, or dy gelu'(gamma xhat + beta) when gelu != 0
+ *   dgamma_c = sum_{b,p} g xhat, dbeta_c = sum_{b,p} g, from per-CTA partials added in a fixed order: bit-identical run to run
+ * stats: float [B*hw][2] (mu, r), written by forward, read by backward.  workspace: b200sht_layer_norm_workspace_floats floats. */
+int64_t b200sht_layer_norm_workspace_floats(int B, int C, int64_t hw);
+int b200sht_layer_norm_forward(const void* x, void* y, const float* gamma, const float* beta, float* stats, int dtype, int out_dtype, int B, int C,
+                               int64_t hw, float eps, int gelu, void* stream);
+/* dgamma / dbeta: float [C], either may be null */
+int b200sht_layer_norm_backward(const void* x, const void* dy, void* dx, const float* gamma, const float* beta, const float* stats, float* dgamma,
+                                float* dbeta, float* workspace, int dtype, int out_dtype, int B, int C, int64_t hw, int gelu, void* stream);
+
 /* ------------------------------------------------------------------ DISCO convolution on the sphere (SURVEY row N1)
  * Replaces the two sparse contractions of torch_harmonics.DiscreteContinuousConvS2 (built at makani/models/networks/fourcastnet3.py:117-252,
  * :364-381, :511-543, snonet.py).  The filter tensor psi[k, t, i, j] (K kernel functions, output latitude t, input latitude i, input longitude

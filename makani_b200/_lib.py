@@ -97,6 +97,10 @@ _SIGNATURES = {
     "b200sht_geometric_norm_backward_sums": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     "b200sht_geometric_norm_backward_apply": (c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, _P, ctypes.c_double, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     "b200sht_geometric_norm_param_grads": (c_int, [_P, _P, _P, c_int, c_int, _P]),
+    # channel layer norm
+    "b200sht_layer_norm_workspace_floats": (c_int64, [c_int, c_int, c_int64]),
+    "b200sht_layer_norm_forward": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int64, c_float, c_int, _P]),
+    "b200sht_layer_norm_backward": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int64, c_int, _P]),
     # DISCO convolution (row N1)
     "b200sht_disco_plan_create": (c_int, [ctypes.POINTER(_P), c_int, c_int, c_int, c_int, c_int, c_int64, _P, _P, _P, _P, _P]),
     "b200sht_disco_plan_destroy": (c_int, [_P]),

@@ -10,6 +10,7 @@ registered in `sys.modules` BEFORE `import makani`:
     compat.install_torch_harmonics_shim()      # torch_harmonics -> makani_b200
     compat.patch_makani_spectral_layers()      # makani.models.common.SpectralConv/SpectralAttention -> makani_b200 (optional)
     compat.patch_makani_norm_layers()          # makani's (Distributed)GeometricInstanceNormS2 -> makani_b200 (optional)
+    compat.patch_makani_layer_norm()           # makani's DistributedLayerNorm -> makani_b200 (optional)
     import makani
 """
 import importlib
@@ -93,3 +94,17 @@ def patch_makani_norm_layers():
             for name, cls in (("GeometricInstanceNormS2", GeometricInstanceNormS2), ("DistributedGeometricInstanceNormS2", mbd.DistributedGeometricInstanceNormS2)):
                 if hasattr(m, name):
                     setattr(m, name, cls)
+
+
+def patch_makani_layer_norm():
+    """After `import makani`: point makani.mpu.layer_norm.DistributedLayerNorm at the CUDA-backed class, and the name that sfnonet / snonet imported
+    at module load.  FourCastNet 3 and 3.1 import it inside a function, so the module attribute covers them.  makani's check that the matmul group
+    has one rank stays in makani's own class; this library has no matmul group."""
+    from makani_b200.norm import DistributedLayerNorm
+
+    m = sys.modules.get("makani.mpu.layer_norm") or importlib.import_module("makani.mpu.layer_norm")
+    m.DistributedLayerNorm = DistributedLayerNorm
+    for modname in ("makani.models.networks.sfnonet", "makani.models.networks.snonet"):
+        net = sys.modules.get(modname)
+        if net is not None and hasattr(net, "DistributedLayerNorm"):
+            net.DistributedLayerNorm = DistributedLayerNorm

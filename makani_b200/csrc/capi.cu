@@ -72,6 +72,11 @@ int geometric_norm_backward_sums(const void* x, const void* dy, const float* gam
 int geometric_norm_backward_apply(const void* x, const void* dy, void* dx, const float* gamma, const float* beta, const float* stats, const double* sums, int R,
                                   const float* q, double D, int dtype, int B, int C, int H, int W, int gelu, cudaStream_t st);
 int geometric_norm_param_grads(const double* sums, float* dgamma, float* dbeta, int B, int C, cudaStream_t st);
+long long layer_norm_workspace_floats(int B, int C, long long hw);
+int layer_norm_forward(const void* x, void* y, const float* gamma, const float* beta, float* stats, int dtype, int out_dtype, int B, int C, long long hw,
+                       float eps, int gelu, cudaStream_t st);
+int layer_norm_backward(const void* x, const void* dy, void* dx, const float* gamma, const float* beta, const float* stats, float* dgamma, float* dbeta,
+                        float* ws, int dtype, int out_dtype, int B, int C, long long hw, int gelu, cudaStream_t st);
 
 static inline cudaStream_t S(void* s) { return static_cast<cudaStream_t>(s); }
 static inline int cp_of(int C) { return round_up(C, 4); }
@@ -845,6 +850,32 @@ int b200sht_geometric_norm_param_grads(const double* sums, float* dgamma, float*
   int rc = check_aligned8(sums, "geometric_norm_param_grads");
   if (rc) return rc;
   return geometric_norm_param_grads(sums, dgamma, dbeta, B, C, S(stream));
+}
+
+// ------------------------------------------------------------------------------ channel layer norm
+int64_t b200sht_layer_norm_workspace_floats(int B, int C, int64_t hw) {
+  if (B <= 0 || C <= 0 || hw <= 0) return -1;
+  return (int64_t)layer_norm_workspace_floats(B, C, hw);
+}
+static int check_layer_norm_dtypes(int dtype, int out_dtype, const char* who) {
+  B200_REQUIRE(out_dtype == dtype || (dtype == B200SHT_BF16 && out_dtype == B200SHT_F32), "%s: unsupported dtype pair (x %d, y %d)", who, dtype, out_dtype);
+  return 0;
+}
+int b200sht_layer_norm_forward(const void* x, void* y, const float* gamma, const float* beta, float* stats, int dtype, int out_dtype, int B, int C,
+                               int64_t hw, float eps, int gelu, void* stream) {
+  int rc = check_pointwise(x, y, dtype, "layer_norm_forward");
+  if (!rc) rc = check_layer_norm_dtypes(dtype, out_dtype, "layer_norm_forward");
+  if (rc) return rc;
+  B200_REQUIRE(stats, "layer_norm_forward: null stats");
+  return layer_norm_forward(x, y, gamma, beta, stats, dtype, out_dtype, B, C, hw, eps, gelu, S(stream));
+}
+int b200sht_layer_norm_backward(const void* x, const void* dy, void* dx, const float* gamma, const float* beta, const float* stats, float* dgamma,
+                                float* dbeta, float* workspace, int dtype, int out_dtype, int B, int C, int64_t hw, int gelu, void* stream) {
+  int rc = check_pointwise(x, dy, dtype, "layer_norm_backward");
+  if (!rc) rc = check_layer_norm_dtypes(dtype, out_dtype, "layer_norm_backward");
+  if (rc) return rc;
+  B200_REQUIRE(dx && stats && workspace, "layer_norm_backward: null argument");
+  return layer_norm_backward(x, dy, dx, gamma, beta, stats, dgamma, dbeta, workspace, dtype, out_dtype, B, C, hw, gelu, S(stream));
 }
 
 int b200sht_debug_set_pdl(int on) {

@@ -622,3 +622,284 @@ int geometric_norm_param_grads(const double* sums, float* dgamma, float* dbeta, 
 }
 
 }  // namespace b200sht
+
+namespace b200sht {
+
+// ------------------------------------------------------------------------------------------------------------------------------------------------------
+// Channel layer norm (makani's DistributedLayerNorm, makani/mpu/layer_norm.py:256-290: nn.LayerNorm(C) over the channels of an NCHW activation, which
+// makani runs as transpose -> layer_norm -> transpose -> .contiguous()).  Per grid point (b, p), p = i W + j, over the C values x[b, c, p] that lie
+// hw elements apart:
+//   forward : mu = mean_c x, var = mean_c (x - mu)^2, r = (var + eps)^-1/2, y = [gelu](gamma_c (x - mu) r + beta_c)                 read x, write y
+//   backward: g = dy [gelu'(z)], dx = r (gamma g - mean_c(gamma g) - xhat mean_c(gamma g xhat))                            read x, dy, write dx
+//             dgamma_c = sum g xhat, dbeta_c = sum g: per-CTA partials in fixed order, then a per-channel fp64 finalize (no atomics)
+// A CTA takes a tile of 32 consecutive points (one warp wide, so every load of a channel row is 32 consecutive elements) and kLnMaxWarps warps
+// split the channel loop.  The tile (x, and dy in the backward) is staged in shared memory on the first pass, so the second pass reads no HBM;
+// a tile too large for shared memory is read twice from global memory instead (the second read mostly hits L2).  Statistics: fp32 Welford per
+// thread about the point's channel-0 value, Chan-combined over the warps in warp order (an offset common to all channels does not cancel).  x / dx in T, y / dy in TO: (float, float),
+// (bf16, bf16), and (bf16, float) for makani's layer under autocast, whose layer_norm returns fp32 for a bf16 input.
+constexpr int kLnPoints = 32;
+constexpr int kLnMaxWarps = 16;
+constexpr int kLnUnroll = 4;
+constexpr int kLnMaxStageBytes = 112 * 1024;   // at least two CTAs per SM
+
+__device__ __forceinline__ float tof(float v) { return v; }
+__device__ __forceinline__ float tof(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <typename T> __device__ __forceinline__ T fromf(float v);
+template <> __device__ __forceinline__ float fromf<float>(float v) { return v; }
+template <> __device__ __forceinline__ __nv_bfloat16 fromf<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+
+struct LnArgs {
+  const void* x;
+  const void* dy;
+  void* out;            // y (forward) / dx (backward)
+  const float* gamma;   // [C] or null (1)
+  const float* beta;    // [C] or null (0)
+  float* stats;         // [B * hw][2] mu, r
+  float* partial;       // backward: [gridDim.x][C][2] sum g xhat, sum g
+  long long hw, tiles_per_b, tiles;
+  int C, gelu;
+  float eps;
+};
+
+// the tile's first element of channel 0 and its lane's point
+__device__ __forceinline__ long long ln_tile(const LnArgs& a, long long t, long long& p) {
+  const long long b = t / a.tiles_per_b;
+  p = (t - b * a.tiles_per_b) * kLnPoints + threadIdx.x;
+  return b * a.C * a.hw;
+}
+
+template <typename T, typename TO, bool STAGE>
+__global__ void __launch_bounds__(kLnPoints * kLnMaxWarps) ln_forward_kernel(const LnArgs a) {
+  extern __shared__ __align__(16) unsigned char ln_smem[];
+  __shared__ float red[2][kLnMaxWarps][kLnPoints];
+  __shared__ float pt[2][kLnPoints];
+  T* sx = reinterpret_cast<T*>(ln_smem);
+  const int lane = threadIdx.x, wy = threadIdx.y, WY = blockDim.y, C = a.C;
+  long long p;
+  const long long base = ln_tile(a, blockIdx.x, p);
+  const bool valid = p < a.hw;
+  const T* x = static_cast<const T*>(a.x) + base + p;
+  TO* y = static_cast<TO*>(a.out) + base + p;
+
+  // Welford of d = x - x[channel 0]: for a point whose channels share a large offset, the d are exact (Sterbenz) and O(spread)
+  const float pivot = valid ? tof(x[0]) : 0.f;
+  float n = 0.f, mean = 0.f, m2 = 0.f;
+  for (int c0 = wy; c0 < C; c0 += WY * kLnUnroll) {
+    T v[kLnUnroll];
+#pragma unroll
+    for (int u = 0; u < kLnUnroll; ++u) {
+      const int c = c0 + u * WY;
+      v[u] = (valid && c < C) ? x[(long long)c * a.hw] : fromf<T>(0.f);
+      if (STAGE && c < C) sx[c * kLnPoints + lane] = v[u];
+    }
+#pragma unroll
+    for (int u = 0; u < kLnUnroll; ++u) {
+      if (c0 + u * WY < C) {
+        const float xv = tof(v[u]) - pivot;
+        n += 1.f;
+        const float d = xv - mean;
+        mean += d / n;
+        m2 = fmaf(d, xv - mean, m2);
+      }
+    }
+  }
+  red[0][wy][lane] = mean;
+  red[1][wy][lane] = m2;
+  __syncthreads();
+  if (wy == 0) {
+    float N = 0.f, M = 0.f, Q = 0.f;
+    for (int k = 0; k < WY; ++k) {
+      const float nb = (float)((C - k + WY - 1) / WY), nn = N + nb, d = red[0][k][lane] - M;
+      M += d * (nb / nn);
+      Q += red[1][k][lane] + d * d * (N * nb / nn);
+      N = nn;
+    }
+    const float r = 1.f / sqrtf(Q / (float)C + a.eps);
+    pt[0][lane] = pivot + M;
+    pt[1][lane] = r;
+    if (valid) { a.stats[2 * (base / C + p)] = pivot + M; a.stats[2 * (base / C + p) + 1] = r; }
+  }
+  __syncthreads();
+  const float mu = pt[0][lane], r = pt[1][lane];
+#pragma unroll kLnUnroll
+  for (int c = wy; c < C; c += WY) {
+    const float xv = tof(STAGE ? sx[c * kLnPoints + lane] : (valid ? x[(long long)c * a.hw] : fromf<T>(0.f)));
+    const float z = fmaf((xv - mu) * r, a.gamma ? __ldg(a.gamma + c) : 1.f, a.beta ? __ldg(a.beta + c) : 0.f);
+    if (valid) y[(long long)c * a.hw] = fromf<TO>(a.gelu ? gelu_f(z) : z);
+  }
+}
+
+// persistent: CTA k takes tiles k, k + gridDim.x, ... and accumulates its parameter-gradient partials in shared memory, one warp per channel
+template <typename T, typename TO, bool STAGE>
+__global__ void __launch_bounds__(kLnPoints * kLnMaxWarps) ln_backward_kernel(const LnArgs a) {
+  extern __shared__ __align__(16) unsigned char ln_smem[];
+  __shared__ float red[2][kLnMaxWarps][kLnPoints];
+  __shared__ float pt[2][kLnPoints];
+  const int lane = threadIdx.x, wy = threadIdx.y, WY = blockDim.y, C = a.C;
+  float* pacc = reinterpret_cast<float*>(ln_smem);                   // [C][2]
+  T* sx = reinterpret_cast<T*>(ln_smem + ((size_t)C * 8 + 15) / 16 * 16);
+  TO* sd = reinterpret_cast<TO*>(reinterpret_cast<unsigned char*>(sx) + ((size_t)C * kLnPoints * sizeof(T) + 15) / 16 * 16);
+  for (int i = wy * kLnPoints + lane; i < 2 * C; i += WY * kLnPoints) pacc[i] = 0.f;
+  __syncthreads();
+
+  for (long long t = blockIdx.x; t < a.tiles; t += gridDim.x) {
+    long long p;
+    const long long base = ln_tile(a, t, p);
+    const bool valid = p < a.hw;
+    const T* x = static_cast<const T*>(a.x) + base + p;
+    const TO* dy = static_cast<const TO*>(a.dy) + base + p;
+    T* dx = static_cast<T*>(a.out) + base + p;
+    const float mu = valid ? a.stats[2 * (base / C + p)] : 0.f, r = valid ? a.stats[2 * (base / C + p) + 1] : 0.f;
+
+    float s1 = 0.f, s2 = 0.f;   // sum gamma g, sum gamma g xhat over this thread's channels
+    for (int c0 = wy; c0 < C; c0 += WY * kLnUnroll) {
+      T xr[kLnUnroll];
+      TO dr[kLnUnroll];
+#pragma unroll
+      for (int u = 0; u < kLnUnroll; ++u) {
+        const int c = c0 + u * WY;
+        const bool in = valid && c < C;
+        xr[u] = in ? x[(long long)c * a.hw] : fromf<T>(0.f);
+        dr[u] = in ? dy[(long long)c * a.hw] : fromf<TO>(0.f);
+        if (STAGE && c < C) { sx[c * kLnPoints + lane] = xr[u]; sd[c * kLnPoints + lane] = dr[u]; }
+      }
+#pragma unroll
+      for (int u = 0; u < kLnUnroll; ++u) {
+        const int c = c0 + u * WY;
+        if (c < C) {
+          const float gm = a.gamma ? __ldg(a.gamma + c) : 1.f;
+          const float xh = (tof(xr[u]) - mu) * r;
+          const float g = a.gelu ? tof(dr[u]) * gelu_grad_f(fmaf(xh, gm, a.beta ? __ldg(a.beta + c) : 0.f)) : tof(dr[u]);
+          s1 = fmaf(gm, g, s1);
+          s2 = fmaf(gm * g, xh, s2);
+          float pg = g * xh, pb = g;
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) { pg += __shfl_xor_sync(0xffffffffu, pg, o); pb += __shfl_xor_sync(0xffffffffu, pb, o); }
+          if (lane == 0) { pacc[2 * c] += pg; pacc[2 * c + 1] += pb; }
+        }
+      }
+    }
+    red[0][wy][lane] = s1;
+    red[1][wy][lane] = s2;
+    __syncthreads();
+    if (wy == 0) {
+      float t1 = 0.f, t2 = 0.f;
+      for (int k = 0; k < WY; ++k) { t1 += red[0][k][lane]; t2 += red[1][k][lane]; }
+      pt[0][lane] = t1 / (float)C;
+      pt[1][lane] = t2 / (float)C;
+    }
+    __syncthreads();
+    const float m1 = pt[0][lane], m2 = pt[1][lane];
+#pragma unroll kLnUnroll
+    for (int c = wy; c < C; c += WY) {
+      const float xv = tof(STAGE ? sx[c * kLnPoints + lane] : (valid ? x[(long long)c * a.hw] : fromf<T>(0.f)));
+      const float dv = tof(STAGE ? sd[c * kLnPoints + lane] : (valid ? dy[(long long)c * a.hw] : fromf<TO>(0.f)));
+      const float gm = a.gamma ? __ldg(a.gamma + c) : 1.f;
+      const float xh = (xv - mu) * r;
+      const float g = a.gelu ? dv * gelu_grad_f(fmaf(xh, gm, a.beta ? __ldg(a.beta + c) : 0.f)) : dv;
+      if (valid) dx[(long long)c * a.hw] = fromf<T>(r * (gm * g - m1 - xh * m2));
+    }
+    __syncthreads();   // the next tile overwrites the staged tile and red / pt
+  }
+  for (int i = wy * kLnPoints + lane; i < 2 * C; i += WY * kLnPoints) a.partial[(size_t)blockIdx.x * 2 * C + i] = pacc[i];
+}
+
+// per channel: the CTAs' partials added in CTA order in fp64; either output may be null
+__global__ void ln_param_grad_kernel(const float* __restrict__ partial, float* __restrict__ dgamma, float* __restrict__ dbeta, int ctas, int C) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  double sg = 0.0, sb = 0.0;
+  for (int k = 0; k < ctas; ++k) { sg += partial[((size_t)k * C + c) * 2]; sb += partial[((size_t)k * C + c) * 2 + 1]; }
+  if (dgamma) dgamma[c] = (float)sg;
+  if (dbeta) dbeta[c] = (float)sb;
+}
+
+static int ln_fill(LnArgs* a, int B, int C, long long hw) {
+  B200_REQUIRE(B > 0 && C > 0 && hw > 0, "layer_norm: bad shape (B %d, C %d, H*W %lld)", B, C, hw);
+  memset(a, 0, sizeof(*a));
+  a->C = C; a->hw = hw;
+  a->tiles_per_b = (hw + kLnPoints - 1) / kLnPoints;
+  a->tiles = a->tiles_per_b * B;
+  B200_REQUIRE(a->tiles < (1LL << 31), "layer_norm: too many grid points (B %d, H*W %lld)", B, hw);
+  return 0;
+}
+
+static int ln_warps(int C) { return C < kLnMaxWarps ? C : kLnMaxWarps; }
+static size_t ln_fwd_stage_bytes(int C, size_t es) { return (size_t)C * kLnPoints * es; }
+static size_t ln_bwd_stage_bytes(int C, size_t es, size_t eso) {
+  return ((size_t)C * 8 + 15) / 16 * 16 + ((size_t)C * kLnPoints * es + 15) / 16 * 16 + (size_t)C * kLnPoints * eso;
+}
+
+// CTAs of the persistent backward: as many as fit on the device at once, at most one per tile
+static int ln_bwd_ctas(long long tiles, int smem_bytes, const void* kernel, int threads) {
+  int per_sm = 0;
+  if (kernel == nullptr || cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem_bytes) != cudaSuccess || per_sm < 1) per_sm = 1;
+  const long long n = (long long)per_sm * device_sms();
+  return (int)(tiles < n ? tiles : n);
+}
+
+long long layer_norm_workspace_floats(int B, int C, long long hw) {
+  const long long tiles = (long long)B * ((hw + kLnPoints - 1) / kLnPoints), cap = 32LL * device_sms();   // 32: most resident CTAs per SM
+  return 2LL * C * (tiles < cap ? tiles : cap);
+}
+
+template <typename T, typename TO>
+static int ln_forward_t(const LnArgs& a, cudaStream_t st) {
+  const int wy = ln_warps(a.C);
+  const size_t stage = ln_fwd_stage_bytes(a.C, sizeof(T));
+  const dim3 block(kLnPoints, wy);
+  if (stage <= (size_t)kLnMaxStageBytes) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(ln_forward_kernel<T, TO, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)stage));
+    ln_forward_kernel<T, TO, true><<<(unsigned)a.tiles, block, stage, st>>>(a);
+  } else {
+    ln_forward_kernel<T, TO, false><<<(unsigned)a.tiles, block, 0, st>>>(a);
+  }
+  B200_CHECK_LAUNCH();
+  return 0;
+}
+
+template <typename T, typename TO>
+static int ln_backward_t(LnArgs a, float* dgamma, float* dbeta, cudaStream_t st) {
+  const int wy = ln_warps(a.C);
+  const size_t stage = ln_bwd_stage_bytes(a.C, sizeof(T), sizeof(TO));
+  const size_t pacc = ((size_t)a.C * 8 + 15) / 16 * 16;
+  const bool staged = stage <= (size_t)kLnMaxStageBytes;
+  const void* k = staged ? (const void*)ln_backward_kernel<T, TO, true> : (const void*)ln_backward_kernel<T, TO, false>;
+  const int smem = (int)(staged ? stage : pacc);
+  B200_REQUIRE(smem <= 200 * 1024, "layer_norm_backward: C %d too large", a.C);
+  B200_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  const int ctas = ln_bwd_ctas(a.tiles, smem, k, kLnPoints * wy);
+  const dim3 block(kLnPoints, wy);
+  if (staged) ln_backward_kernel<T, TO, true><<<ctas, block, smem, st>>>(a);
+  else ln_backward_kernel<T, TO, false><<<ctas, block, smem, st>>>(a);
+  B200_CHECK_LAUNCH();
+  if (dgamma || dbeta) {
+    ln_param_grad_kernel<<<(a.C + 127) / 128, 128, 0, st>>>(a.partial, dgamma, dbeta, ctas, a.C);
+    B200_CHECK_LAUNCH();
+  }
+  return 0;
+}
+
+int layer_norm_forward(const void* x, void* y, const float* gamma, const float* beta, float* stats, int dtype, int out_dtype, int B, int C, long long hw,
+                       float eps, int gelu, cudaStream_t st) {
+  LnArgs a;
+  int rc = ln_fill(&a, B, C, hw);
+  if (rc) return rc;
+  a.x = x; a.out = y; a.gamma = gamma; a.beta = beta; a.stats = stats; a.eps = eps; a.gelu = gelu;
+  if (dtype == B200SHT_F32) return ln_forward_t<float, float>(a, st);
+  if (out_dtype == B200SHT_BF16) return ln_forward_t<__nv_bfloat16, __nv_bfloat16>(a, st);
+  return ln_forward_t<__nv_bfloat16, float>(a, st);
+}
+
+int layer_norm_backward(const void* x, const void* dy, void* dx, const float* gamma, const float* beta, const float* stats, float* dgamma, float* dbeta,
+                        float* ws, int dtype, int out_dtype, int B, int C, long long hw, int gelu, cudaStream_t st) {
+  LnArgs a;
+  int rc = ln_fill(&a, B, C, hw);
+  if (rc) return rc;
+  a.x = x; a.dy = dy; a.out = dx; a.gamma = gamma; a.beta = beta; a.stats = const_cast<float*>(stats); a.partial = ws; a.gelu = gelu;
+  if (dtype == B200SHT_F32) return ln_backward_t<float, float>(a, dgamma, dbeta, st);
+  if (out_dtype == B200SHT_BF16) return ln_backward_t<__nv_bfloat16, __nv_bfloat16>(a, dgamma, dbeta, st);
+  return ln_backward_t<__nv_bfloat16, float>(a, dgamma, dbeta, st);
+}
+
+}  // namespace b200sht

@@ -4,7 +4,8 @@
 /root/reference/makani/models/networks/sfnonet.py:618-620 (`num_features=embed_dim, eps=1e-6, affine=True, track_running_stats=False`); on CUDA tensors
 of dtype float32 / bfloat16 its forward runs `b200sht_instance_norm_forward` (csrc/norm.cu) and can fuse the GELU that follows it in
 `NeuralOperatorBlock.forward` (sfnonet.py:387-392).  `bias_gelu(x, bias)` is the `+ bias -> GELU` of the 1x1-convolution stacks
-(makani/models/common/layers.py:537-760).  Tensors on the CPU (the oracle-backend reference arm of bench.py, the CPU golden tests) and configurations the
+(makani/models/common/layers.py:537-760).  `DistributedLayerNorm` is makani's channel layer norm (makani/mpu/layer_norm.py:256-290) on
+`b200sht_layer_norm_forward` / `_backward`, also with GELU fused.  Tensors on the CPU (the oracle-backend reference arm of bench.py, the CPU golden tests) and configurations the
 kernels do not cover (running statistics, other dtypes) take torch's own operators -- these layers are outside the spherical-harmonic hot path, whose
 no-fallback rule (DESIGN.md section 1) is unchanged.  `B200SHT_FUSED_POINTWISE=0` switches the kernels off.
 """
@@ -361,3 +362,78 @@ class GeometricInstanceNormS2(nn.Module):
         stages = self._stages(x)
         w, b = (self.weight, self.bias) if self.affine else (None, None)
         return _GeometricNormFn.apply(x, w, b, self._q(x), self._normaliser(), self.eps, bool(gelu), stages, self._gather())
+
+
+# ------------------------------------------------------------------------------------------------------------------------------------------------------
+# Channel layer norm (makani's DistributedLayerNorm): nn.LayerNorm(C) at every grid point of an NCHW activation, which makani computes as transpose ->
+# layer_norm -> transpose -> .contiguous().  The kernels of csrc/norm.cu reduce over the strided channel axis in place: the forward reads x once and
+# writes y once, the backward reads x and dy once and writes dx once, and dgamma / dbeta come from fixed-order per-CTA partials.  The layer is
+# pointwise in space, so under h x w model parallelism the local shard is the whole problem and nothing is exchanged.
+
+def _layer_norm_out_dtype(x):
+    """the dtype makani's layer returns for a CUDA tensor x: layer_norm is on CUDA autocast's fp32 list, otherwise the output keeps the dtype of x"""
+    return torch.float32 if torch.is_autocast_enabled("cuda") else x.dtype
+
+
+class _LayerNormFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, eps, gelu, out_dtype):
+        x = x.contiguous()
+        B, C, H, W = x.shape
+        y = torch.empty(x.shape, dtype=out_dtype, device=x.device)
+        stats = torch.empty(B * H * W, 2, dtype=torch.float32, device=x.device)
+        w32 = weight.detach().to(torch.float32).contiguous() if weight is not None else None
+        b32 = bias.detach().to(torch.float32).contiguous() if bias is not None else None
+        _lib.call("b200sht_layer_norm_forward", _ptr(x), _ptr(y), _ptr(w32), _ptr(b32), _ptr(stats), _dt(x.dtype), _dt(out_dtype), B, C, H * W, float(eps),
+                  int(gelu), _lib.launch_stream(x.device))
+        ctx.save_for_backward(x, w32, b32, stats)
+        ctx.gelu, ctx.out_dtype = int(gelu), out_dtype
+        ctx.param_dtypes = (weight.dtype if weight is not None else None, bias.dtype if bias is not None else None)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w32, b32, stats = ctx.saved_tensors
+        B, C, H, W = x.shape
+        dy = dy.contiguous().to(ctx.out_dtype)
+        dx = torch.empty_like(x)
+        need_w = w32 is not None and ctx.needs_input_grad[1]
+        need_b = b32 is not None and ctx.needs_input_grad[2]
+        dw = torch.empty(C, dtype=torch.float32, device=x.device) if need_w else None
+        db = torch.empty(C, dtype=torch.float32, device=x.device) if need_b else None
+        ws = torch.empty(max(int(_lib.load().b200sht_layer_norm_workspace_floats(B, C, H * W)), 2), dtype=torch.float32, device=x.device)
+        _lib.call("b200sht_layer_norm_backward", _ptr(x), _ptr(dy), _ptr(dx), _ptr(w32), _ptr(b32), _ptr(stats), _ptr(dw), _ptr(db), _ptr(ws), _dt(x.dtype),
+                  _dt(ctx.out_dtype), B, C, H * W, ctx.gelu, _lib.launch_stream(x.device))
+        dw = dw.to(ctx.param_dtypes[0]) if need_w else None
+        db = db.to(ctx.param_dtypes[1]) if need_b else None
+        return (dx if ctx.needs_input_grad[0] else None), dw, db, None, None, None
+
+
+class DistributedLayerNorm(nn.Module):
+    """makani's DistributedLayerNorm (same constructor, `.norm` submodule nn.LayerNorm, state-dict keys `norm.weight` / `norm.bias`, the same
+    `is_shared_mp` / `sharded_dims_mp` tags): layer norm over the channels of an NCHW activation at every grid point, on one GPU and under h x w
+    spatial model parallelism alike.  CUDA float32 / bfloat16 4-D inputs normalised over their channel axis run on the kernels of csrc/norm.cu, and
+    `forward(x, gelu=True)` returns gelu(norm(x)) in the same passes; other inputs take makani's formula (transpose -> self.norm -> transpose)."""
+
+    def __init__(self, normalized_shape, eps=1e-05, elementwise_affine=True, bias=True, device=None, dtype=None):
+        super().__init__()
+        self.norm = nn.LayerNorm(normalized_shape, eps=eps, elementwise_affine=elementwise_affine, bias=bias, device=device, dtype=dtype)
+        if elementwise_affine:
+            self.norm.weight.is_shared_mp = ["model"]
+            self.norm.weight.sharded_dims_mp = [None]
+            if bias:
+                self.norm.bias.is_shared_mp = ["model"]
+                self.norm.bias.sharded_dims_mp = [None]
+
+    def _kernels_take(self, x):
+        if not (_ENABLED and x.is_cuda and x.dim() == 4 and x.dtype in (torch.float32, torch.bfloat16) and x.numel() > 0):
+            return False
+        if tuple(self.norm.normalized_shape) != (x.shape[1],):
+            return False
+        return all(p is None or (p.is_cuda and p.dtype in (torch.float32, x.dtype)) for p in (self.norm.weight, self.norm.bias))
+
+    def forward(self, x, gelu=False):
+        if self._kernels_take(x):
+            return _LayerNormFn.apply(x, self.norm.weight, self.norm.bias, self.norm.eps, bool(gelu), _layer_norm_out_dtype(x))
+        y = torch.transpose(self.norm(torch.transpose(x, 1, 3)), 1, 3).contiguous()
+        return F.gelu(y) if gelu else y

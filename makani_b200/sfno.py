@@ -212,11 +212,11 @@ class NeuralOperatorBlock(nn.Module):
         return gain
 
     def forward(self, x):
-        from .norm import GeometricInstanceNormS2
+        from .norm import DistributedLayerNorm, GeometricInstanceNormS2
         from .norm import InstanceNorm2d as FusedInstanceNorm2d
 
         x, residual = self.filter(x)
-        if (isinstance(self.norm0, (FusedInstanceNorm2d, GeometricInstanceNormS2)) and not hasattr(self, "inner_skip") and isinstance(self.act_layer0, nn.GELU)
+        if (isinstance(self.norm0, (FusedInstanceNorm2d, GeometricInstanceNormS2, DistributedLayerNorm)) and not hasattr(self, "inner_skip") and isinstance(self.act_layer0, nn.GELU)
                 and getattr(self.act_layer0, "approximate", "none") == "none"):
             x = self.norm0(x, gelu=True)     # norm0 -> GELU in one pass (sfnonet.py:387-392 with inner_skip "none")
         else:
@@ -259,7 +259,11 @@ class SphericalFourierNeuralOperatorNet(nn.Module):
         self.pos_drop = nn.Dropout(p=pos_drop_rate) if pos_drop_rate > 0.0 else nn.Identity()
         dpr = [v.item() for v in torch.linspace(0, path_drop_rate, num_layers)]
 
-        if normalization_layer == "instance_norm":
+        if normalization_layer == "layer_norm":
+            from .norm import DistributedLayerNorm   # makani's class: `.norm` nn.LayerNorm over the channels, CUDA kernels of csrc/norm.cu
+
+            norm_inp = norm_mid = norm_out = partial(DistributedLayerNorm, normalized_shape=(embed_dim), elementwise_affine=True, eps=1e-6)
+        elif normalization_layer == "instance_norm":
             from .norm import InstanceNorm2d as FusedInstanceNorm2d   # nn.InstanceNorm2d subclass: same parameters / state dict, CUDA kernels of csrc/norm.cu
 
             norm = partial(FusedInstanceNorm2d, num_features=embed_dim, eps=1e-6, affine=True, track_running_stats=False)
