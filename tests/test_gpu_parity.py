@@ -389,53 +389,7 @@ def test_full_size_properties_721x1440():
     assert abs(lhs.item() - rhs.item()) <= 2e-5 * max(abs(lhs.item()), 1.0), (lhs.item(), rhs.item())
 
 
-# ------------------------------------------------------------------------------- distributed local stages on one GPU
-def test_distributed_local_stages_cuda_subplans():
-    """The CUDA local stages of the h x w path (FFT-only plan on a latitude slice, Legendre plan with an order offset, latspec /
-    spec converters) against oracle slices -- shard geometry of rank (h=1 of 2, w=1 of 2) emulated on a single GPU."""
-    import makani_b200.distributed as mbd
-
-    torch.manual_seed(333)
-    nlat, nlon, lmax, mmax, B, C = 65, 128, 40, 45, 2, 5
-    for grid in ("equiangular", "legendre-gauss"):
-        t = mbd.DistributedRealSHT(nlat, nlon, lmax, mmax, grid, precision="fp32")
-        lat_shapes, m_shapes = mbd.compute_split_shapes(nlat, 2), mbd.compute_split_shapes(mmax, 2)
-        t.nlat_local, t.lat_offset = lat_shapes[1], lat_shapes[0]
-        t.mmax_local, t.m_offset = m_shapes[1], m_shapes[0]
-        ops = mbd.CudaLocalOps(t)
-        theta, w = O.precompute_latitudes(nlat, grid)
-        P = torch.from_numpy(O.legpoly(mmax, lmax, np.cos(theta)))[t.m_offset : t.m_offset + t.mmax_local]
-        wl = torch.from_numpy(w[t.lat_offset : t.lat_offset + t.nlat_local])
-        x = torch.randn(B, C, t.nlat_local, nlon)
-        xd = x.to(DEV).requires_grad_(True)
-        X = ops.fft(xd)
-        xr = x.double().requires_grad_(True)
-        Xref = 2 * math.pi * torch.fft.rfft(xr, dim=-1, norm="forward")[..., :mmax] * wl[:, None]
-        close(X, Xref, 1e-5, f"dist local fft {grid}")
-        g = torch.randn(B, C, t.nlat_local, mmax, dtype=torch.complex64)
-        X.backward(g.to(DEV))
-        Xref.backward(g.to(torch.complex128))
-        close(xd.grad, xr.grad, 1e-5, f"dist local fft grad {grid}")
-        xc = torch.randn(B, C, nlat, t.mmax_local, dtype=torch.complex64)
-        xcd = xc.to(DEV).requires_grad_(True)
-        Y = ops.legendre(xcd)
-        xcr = xc.to(torch.complex128).requires_grad_(True)
-        Yref = torch.einsum("...km,mlk->...lm", xcr, P.to(torch.complex128))
-        close(Y, Yref, 1e-5, f"dist local legendre {grid} (orders {t.m_offset}..{t.m_offset + t.mmax_local - 1})")
-        gl = torch.randn(B, C, lmax, t.mmax_local, dtype=torch.complex64)
-        Y.backward(gl.to(DEV))
-        Yref.backward(gl.to(torch.complex128))
-        close(xcd.grad, xcr.grad, 1e-5, f"dist local legendre grad {grid}")
-        c = torch.randn(B, C, lmax, t.mmax_local, dtype=torch.complex64)
-        Zc = ops.ilegendre(c.to(DEV))
-        close(Zc, torch.einsum("...lm,mlk->...km", c.to(torch.complex128), P.to(torch.complex128)), 1e-5, f"dist local ilegendre {grid}")
-        z = torch.randn(B, C, t.nlat_local, mmax, dtype=torch.complex64)
-        y = ops.ifft(z.to(DEV), torch.float32)
-        zz = z.to(torch.complex128).clone()
-        zz[..., 0] = zz[..., 0].real.to(torch.complex128)
-        close(y, torch.fft.irfft(zz, n=nlon, dim=-1, norm="forward"), 1e-5, f"dist local ifft {grid}")
-
-
+# ------------------------------------------------------------------------------- distributed modules on one GPU
 def test_distributed_modules_world1_and_dense_conv():
     """world size 1: Distributed* transforms (sub-plans + dense packed spectra + dense mix) == local transforms == oracle."""
     import makani_b200.distributed as mbd
