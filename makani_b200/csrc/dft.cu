@@ -9,9 +9,10 @@
 // pipe at TF32 and only one radix-8 stage stays on the CUDA cores; no shared-memory exchange between stages is left.
 //
 // synthesis kernel (latspec -> rows):   D[j2][(class c, latitude k)] for the columns j2 <= N2/2 and an 8-row tile.  A = E^T resident in
-//   shared memory (32 KB), B = the raw latspec tile [m2][(c, k)] streamed by TMA (16 KB per 8 rows) through an mbarrier ring, the cosine
-//   and sine sums of Zr and Zi in registers.  A task owns 8 columns j2; its m16n8 fragments give each thread the two latitudes
-//   2 (lane % 4), + 1 of the column j2 = lane / 4 for all eight classes, i.e. the inputs of its own butterflies:
+//   shared memory (32 KB) in fragment order, B = the latspec tile [m2][(c, k)] streamed by TMA (16 KB per 8 rows) through an mbarrier ring
+//   and rewritten in place into fragment order by the load warp, the cosine and sine sums of Zr and Zi in registers.  A task owns 8
+//   columns j2; its m16n8 fragments give each thread the two latitudes 2 (lane % 4), + 1 of the column j2 = lane / 4 for all eight classes,
+//   i.e. the inputs of its own butterflies:
 //   S -> V(j2), V(N2-j2) -> twiddle -> radix-8 -> scale/bias -> bf16 into a shared-memory output tile, written out by TMA bulk stores.
 // analysis kernel (rows -> latspec):    producer warps load the eight samples x[N2 j1 + j2] of a column (lanes = consecutive j2),
 //   butterfly + twiddle them and write the even/odd combinations (Ye, Yo) as K-major TF32 operand tiles [(c, k)][j2] (128-byte
@@ -37,6 +38,22 @@ __host__ __device__ constexpr int dft_out_box(int N2) {
   int d = N2 < 32 ? N2 : 32;
   while (N2 % d != 0) --d;
   return 8 * d;
+}
+
+// n / d for 0 <= n < 2^31 by a multiply-high and a shift (d > 0 fixed per launch): the per-task index arithmetic of the synthesis workers
+// without the ~25-instruction integer division
+struct FastDiv {
+  uint32_t m, s;
+  int d;
+  __device__ __forceinline__ int div(int n) const { return (int)((__umulhi((uint32_t)n, m) + (uint32_t)n) >> s); }
+};
+static FastDiv make_fastdiv(int d) {
+  FastDiv f;
+  f.d = d;
+  f.s = 0;
+  while ((1ll << f.s) < d) ++f.s;
+  f.m = (uint32_t)((((1ull << 32) * ((1ull << f.s) - (unsigned long long)d)) / (unsigned long long)d) + 1);
+  return f;
 }
 
 struct DftTables {
@@ -131,8 +148,9 @@ bool dft_usable(const Plan* pl) { return pl->dft_state != nullptr && dft_enabled
 // ----------------------------------------------------------------------------------------- wait-time profile
 // B200SHT_DFT_PROF=1: every role accumulates the SM clocks it spends in its mbarrier waits (one atomic per wait, lane 0 of the warp) into 16
 // counters, read back and cleared by b200sht_debug_dft_profile().  Slots -- analysis: 0 producers / raw samples, 1 producers / operand stage free,
-// 2 loader / raw stage free, 3 MMA warps / operand stage full, 5 MMA-warp tiles, 6 CTA lifetime, 7 producer items; synthesis: 8 TMA / stage free,
-// 9 MMA warps / stage full, 12 CTA lifetime, 13 MMA-warp tiles.
+// 2 loader / raw stage free, 3 MMA warps / operand stage full, 5 MMA-warp tiles, 6 CTA lifetime, 7 producer items; synthesis: 8 load warp /
+// stage free, 9 workers / stage rewritten, 10 workers / output tile free, 11 store warp / output tile written, 12 CTA lifetime, 13 worker
+// tasks, 14 load warp / tile landed.
 static unsigned long long* g_dft_prof = nullptr;
 static unsigned long long* dft_prof_buffer() {
   static const int on = [] { const char* e = getenv("B200SHT_DFT_PROF"); return e ? atoi(e) : 0; }();
@@ -197,9 +215,17 @@ static int make_tmap_out(CUtensorMap* tm, void* base, bool bf16, int nlon, int n
   return 0;
 }
 
-template <typename T> __device__ __forceinline__ void st_out(T* p, float v);
-template <> __device__ __forceinline__ void st_out<float>(float* p, float v) { *p = v; }
-template <> __device__ __forceinline__ void st_out<__nv_bfloat16>(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
+// the two latitudes of a synthesis thread: a at p0, b at p1 (bf16: one conversion of the pair)
+template <typename T> __device__ __forceinline__ void st_out2(uint8_t* p0, uint8_t* p1, float a, float b);
+template <> __device__ __forceinline__ void st_out2<float>(uint8_t* p0, uint8_t* p1, float a, float b) {
+  *reinterpret_cast<float*>(p0) = a;
+  *reinterpret_cast<float*>(p1) = b;
+}
+template <> __device__ __forceinline__ void st_out2<__nv_bfloat16>(uint8_t* p0, uint8_t* p1, float a, float b) {
+  const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+  *reinterpret_cast<__nv_bfloat16*>(p0) = v.x;
+  *reinterpret_cast<__nv_bfloat16*>(p1) = v.y;
+}
 // raw sample bits of the next item (converted when consumed): float bits, or the bf16 pattern in the low half
 template <typename T> __device__ __forceinline__ uint32_t ld_raw(const T* p);
 template <> __device__ __forceinline__ uint32_t ld_raw<float>(const float* p) { return __float_as_uint(__ldg(p)); }
@@ -250,27 +276,44 @@ template <> __device__ __forceinline__ float ld_in<__nv_bfloat16>(const __nv_bfl
 // ================================================================================================ synthesis
 struct DftSynParams {
   alignas(64) CUtensorMap tmZ;   // tiled latspec as ((c % 4, k % 8), c / 4, m2, p, tile), box (32, 1, 32, 1, 1): MN-major B operand, N = (c, k)
-  alignas(64) CUtensorMap tmE;   // E^T tiles (m2, 256 rows), box (32, 128): K-major A operand
   alignas(64) CUtensorMap tmY;   // the output as (nlon, nlat, R), box (ow, 8, 1), no swizzle: TMA clips the rows k >= nlat of an image's last tile
   const float* Z;
+  const float* et;   // E^T tiles, [16 blocks][cos, sin][8 rows j2][32 m2]: read once per CTA into fragment order
   const float2* tw;
   const float* rowscale;
   const float* bias;
   unsigned long long* prof;
-  int R, C, nlat, nlon, kp, mmax, N2, half, M2, mode, ntiles, ktiles, has_nyq, ow;   // ktiles: 8-row tiles per image
+  FastDiv ktiles, C;   // 8-row tiles per image; channels (bias index r % C)
+  int R, nlat, nlon, kp, mmax, N2, half, M2, mode, ntiles, has_nyq, ow;
 };
 
-// shared memory: [A: 16 blocks x (cos 8 rows | sin 8 rows), 32 KB][B ring: kDftSynStages x 16 KB][output: 2 x 8 rows x nlon]
-//                [tw table 8 x N2 float2][barriers]
-// warps 0 .. kDftSynWorkers - 1: MMA + epilogue; then the TMA load warp and the TMA store warp.  The work of a tile is split into `nblk` tasks, one per 8 columns j2 <= N2 / 2,
-// and the tasks (tile n, block b) of this CTA are dealt round-robin over `nwork` worker warps (task n * nblk + b), so each SM sub-partition
-// holds several tasks in flight: the epilogue of one overlaps the MMAs of another.  nwork <= 2 nblk bounds the lead of a warp: consecutive
-// tasks of a warp are at most two tiles apart, so when a warp reaches tile m, its previous task has seen tile m - 4 loaded (full) and
-// stored (ofree).  Every mbarrier wait is then for the next phase of its barrier and never for one two phases away, which the parity test
-// cannot tell apart.  All kDftSynWorkers warps work when nblk >= 5 (N2 >= 72).  The A tile of block b
-// stacks the cos and sin rows of its 8 columns, so the m16n8 accumulator fragment holds, per thread, S1 / S3 (B = Zr) and S4 / S2 (B = Zi) of
-// the column j2 = 8 b + lane / 4 and the latitude pair 2 (lane % 4), + 1 for all eight classes: exactly the inputs of the radix-8 epilogue of
-// j2 and N2 - j2, in 64 accumulator registers.
+// Order of the 32 orders m2 in the MMA K loop.  The sum over m2 may visit them in any order as long as A and B agree, and this one lets a
+// thread load its B fragments of two k8 steps with one 16-byte load: the thread (g, q) of step s holds, in its K slots q and q + 4, the
+// orders syn_kslot(s, q, 0 / 1) = 8 q + 4 (s / 2) + ((2 (s % 2) + 0 / 1 + q) % 4).  Over the four steps the slots of the lanes q hold
+// 8 q .. 8 q + 7, rotated by q inside each group of four: the rotation keeps the load warp's rewrite of the stage free of bank conflicts.
+__host__ __device__ constexpr int syn_kslot(int s, int q, int hi) { return 8 * q + 4 * (s >> 1) + ((2 * (s & 1) + hi + q) & 3); }
+// 16-byte unit of the thread (g, q) in each 512-byte block of a rewritten stage: the eight threads of a quarter warp hit distinct bank
+// groups both when the workers read (g = 2 t, 2 t + 1) and when the load warp writes (g = j, j + 4)
+__device__ __forceinline__ uint32_t syn_unit(int g, int q) { return (uint32_t)(8 * (g >> 1) + 4 * ((g ^ (g >> 2)) & 1) + q); }
+
+// shared memory: [A: 16 blocks x 4 k8 steps x 32 lanes x 16 B, 32 KB][B ring: kDftSynStages x 16 KB][output: 2 x 8 rows x nlon]
+//                [tw table N2 x 8 float2][output offsets 8 x N2 int][barriers]
+// warps 0 .. kDftSynWorkers - 1: MMA + epilogue; then the TMA load warp and the TMA store warp.
+// B stage: TMA lands the tile as [plane][c / 4][32 rows m2][(c % 4, k)] (128-byte swizzle).  The load warp then rewrites each 4 KB block
+// (plane, c / 4) in place as [c % 4][h][32 threads][4 orders]: the thread (g, q) finds the orders 8 q + 4 h + 0..3 (rotated by q, see
+// syn_kslot) of the latitude g and the class c in one 16-byte unit, so a task loads its 64 B-fragment registers with 32 LDS.128 instead of
+// 128 scalar loads, and the rewrite (32 LDS.128 + 32 STS.128 per lane and tile, conflict-free) is shared by all the tasks of the tile.
+// The load warp runs one tile ahead with its TMA loads: before it rewrites tile n it issues the load of tile n + 1 as soon as the workers
+// have released that stage (tile n - 3), so the workers find up to three tiles ready; it arrives on ready[s] when the rewrite is written.
+// (Issuing further ahead without blocking was slower, 158 against 135 us: the warp then only looks for free stages once per landed tile.)
+// The work of a tile is split into `nblk` tasks, one per 8 columns j2 <= N2 / 2, and the tasks (tile n, block b) of this CTA are dealt
+// round-robin over `nwork` worker warps (task n * nblk + b), so each SM sub-partition holds several tasks in flight: the epilogue of one
+// overlaps the MMAs of another.  nwork <= 2 nblk bounds the lead of a warp: consecutive tasks of a warp are at most two tiles apart, so when
+// a warp reaches tile m, its previous task has seen tile m - 4 rewritten (ready) and stored (ofree).  Every mbarrier wait is then for the
+// next phase of its barrier and never for one two phases away, which the parity test cannot tell apart.  All kDftSynWorkers warps work
+// when nblk >= kDftSynWorkers / 2.  The A tile of block b stacks the cos and sin rows of its 8 columns, so the m16n8 accumulator fragment
+// holds, per thread, S1 / S3 (B = Zr) and S4 / S2 (B = Zi) of the column j2 = 8 b + lane / 4 and the latitude pair 2 (lane % 4), + 1 for
+// all eight classes: exactly the inputs of the radix-8 epilogue of j2 and N2 - j2, in 64 accumulator registers.
 // Output: the epilogues write the finished values of tile n into the shared-memory tile n % 2, laid out as the TMA boxes of ow columns
 // x 8 rows; when all nblk tasks of the tile have arrived on staged[n % 2], the store warp writes it with bulk tensor stores (whole 128-byte
 // lines instead of 16-byte pieces of four rows per store instruction) and frees the buffer once the stores have read it.
@@ -288,15 +331,15 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
   const int nlon = 8 * N2;
   const int ow = p.ow;
   const uint32_t obytes = (8u * nlon * sizeof(T) + 1023u) & ~1023u;   // one output tile
-  const uint32_t sA = base, sB = base + 32768, sO = sB + kDftSynStages * 16384;
+  const uint32_t sB = base + 32768, sO = sB + kDftSynStages * 16384;
   T* const outS = reinterpret_cast<T*>(gbase + (sO - base));
-  float2* tws = reinterpret_cast<float2*>(gbase + (sO - base) + 2 * obytes);
-  int* oofs = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(tws) + ((8 * N2 * 8 + 15) & ~15));
+  float4* tws = reinterpret_cast<float4*>(gbase + (sO - base) + 2 * obytes);   // [j2][c / 2]: the twiddles of the classes 2 i, 2 i + 1
+  int* oofs = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(tws) + 8 * N2 * 8);
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(oofs) + 8 * N2 * 4);
-  uint64_t* full = bars;
-  uint64_t* empty = full + kDftSynStages;
-  uint64_t* e_full = empty + kDftSynStages;
-  uint64_t* staged = e_full + 1;   // [2] output tile written by all its tasks
+  uint64_t* full = bars;                  // [stages] TMA landed
+  uint64_t* ready = full + kDftSynStages;   // [stages] rewritten into fragment order
+  uint64_t* empty = ready + kDftSynStages;  // [stages] read by all the tasks of its tile
+  uint64_t* staged = empty + kDftSynStages;   // [2] output tile written by all its tasks
   uint64_t* ofree = staged + 2;    // [2] output tile read by its bulk stores
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
@@ -306,48 +349,113 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
   const bool is_tma = (warp == kDftSynWorkers), is_store = (warp == kDftSynWorkers + 1);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kDftSynStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], nblk); }
-    mbar_init(e_full, 1);
+    for (int s = 0; s < kDftSynStages; ++s) { mbar_init(&full[s], 1); mbar_init(&ready[s], 32); mbar_init(&empty[s], nblk); }
     for (int b = 0; b < 2; ++b) { mbar_init(&staged[b], 32 * nblk); mbar_init(&ofree[b], 1); }
     fence_barrier_init();
     prefetch_tmap(&p.tmZ);
-    prefetch_tmap(&p.tmE);
     prefetch_tmap(&p.tmY);
   }
-  for (int i = threadIdx.x; i < 8 * p.N2; i += blockDim.x) tws[i] = p.tw[i];
-  for (int i = threadIdx.x; i < 8 * N2; i += blockDim.x) {   // output tile position of the longitude N2 j1 + j2 (row 0) at [j2][j1]
+  {
+    // A in fragment order: [block][k8 step s][lane (g, q)] = (cos, sin of the column 8 block + g) at the orders syn_kslot(s, q, 0), then (1).
+    // All the 16-byte loads of a thread are issued before its stores: one memory latency for the prologue, not one per element.
+    constexpr int kEt4 = 16 * 2 * 8 * 32 / 4, kPer = (kEt4 + kDftSynThreads - 1) / kDftSynThreads;
+    float4 ev[kPer];
+#pragma unroll
+    for (int k = 0; k < kPer; ++k) {
+      const int i = threadIdx.x + k * kDftSynThreads;
+      if (i < kEt4) ev[k] = __ldg(reinterpret_cast<const float4*>(p.et) + i);
+    }
+#pragma unroll
+    for (int k = 0; k < kPer; ++k) {
+      const int i = threadIdx.x + k * kDftSynThreads;   // E^T float4: orders 4 (i % 8) .. + 3 of the row i / 8 = (block, cos / sin, g)
+      if (i >= kEt4) continue;
+      const int row = i >> 3, b = row >> 4, cs = (row >> 3) & 1, g = row & 7;
+      const float v[4] = {ev[k].x, ev[k].y, ev[k].z, ev[k].w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {   // the inverse of syn_kslot: order m2 -> (step s, slot half hi) of the lanes q = m2 / 8
+        const int m2 = 4 * (i & 7) + e, q = m2 >> 3, r = m2 & 7, u = ((r & 3) - q) & 3;
+        const int s = 2 * (r >> 2) + (u >> 1), hi = u & 1;
+        reinterpret_cast<float*>(gbase)[((b * 4 + s) * 32 + 4 * g + q) * 4 + 2 * hi + cs] = v[e];
+      }
+    }
+  }
+  for (int i = threadIdx.x; i < 4 * N2; i += blockDim.x) {
+    const int j2 = i >> 2, c = 2 * (i & 3);
+    tws[i] = make_float4(p.tw[c * N2 + j2].x, p.tw[c * N2 + j2].y, p.tw[(c + 1) * N2 + j2].x, p.tw[(c + 1) * N2 + j2].y);
+  }
+  for (int i = threadIdx.x; i < 8 * N2; i += blockDim.x) {   // output tile byte offset of the longitude N2 j1 + j2 (row 0) at [j2][j1]
     const int j = N2 * (i & 7) + (i >> 3);
-    oofs[i] = (j / ow) * 8 * ow + j % ow;
+    oofs[i] = ((j / ow) * 8 * ow + j % ow) * (int)sizeof(T);
   }
   __syncthreads();
   const long long t_cta0 = (kDftProfile && p.prof && threadIdx.x == 0) ? clock64() : 0;
-  pdl_wait();   // the prologue read plan constants only (twiddles); the latspec tiles, bias and y belong to other kernels until here
+  pdl_wait();   // the prologue read plan constants only (E^T, twiddles); the latspec tiles, bias and y belong to other kernels until here
 
   if (is_tma) {
-    if (lane == 0) {
-      mbar_expect_tx(e_full, 32768);
-      tma_load_2d(sA, &p.tmE, e_full, 0, 0);
-      tma_load_2d(sA + 16384, &p.tmE, e_full, 0, 128);
-      int n = 0;
-      for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
-        const int s = n % kDftSynStages, it = n / kDftSynStages;
-        if (it > 0) prof_wait(prof, 8, &empty[s], (it - 1) & 1, true);
-        mbar_expect_tx(&full[s], 16384);
-        const uint32_t st = sB + s * 16384;
-        tma_load_5d(st, &p.tmZ, &full[s], 0, 0, 0, 0, ti);           // re, classes 0..3
-        tma_load_5d(st + 4096, &p.tmZ, &full[s], 0, 1, 0, 0, ti);    // re, classes 4..7
-        tma_load_5d(st + 8192, &p.tmZ, &full[s], 0, 0, 0, 1, ti);    // im
-        tma_load_5d(st + 12288, &p.tmZ, &full[s], 0, 1, 0, 1, ti);
+    const int ntl = blockIdx.x < p.ntiles ? (p.ntiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;   // tiles of this CTA
+    auto load = [&](int n) {
+      const int s = n % kDftSynStages, it = n / kDftSynStages;
+      if (it > 0) prof_wait(prof, 8, &empty[s], (it - 1) & 1, true);
+      mbar_expect_tx(&full[s], 16384);
+      const uint32_t st = sB + s * 16384;
+      const int ti = blockIdx.x + n * gridDim.x;
+      tma_load_5d(st, &p.tmZ, &full[s], 0, 0, 0, 0, ti);           // re, classes 0..3
+      tma_load_5d(st + 4096, &p.tmZ, &full[s], 0, 1, 0, 0, ti);    // re, classes 4..7
+      tma_load_5d(st + 8192, &p.tmZ, &full[s], 0, 0, 0, 1, ti);    // im
+      tma_load_5d(st + 12288, &p.tmZ, &full[s], 0, 1, 0, 1, ti);
+    };
+    // rewrite of a 4 KB block (plane, c / 4): the lane (q, b, t) reads the rows 8 q + 4 h + (i + q) % 4 (i = 0..3, h = b ^ pass) at the
+    // latitudes 4 b .. 4 b + 3 of the class 4 (c / 4) + t, and writes the transposed 4 x 4 block as the units of the threads (4 b + j, q).
+    // A quarter warp (one t) reads eight distinct rows modulo 8 -- eight distinct chunks under the swizzle -- and writes eight distinct
+    // bank groups (syn_unit).
+    const int q = lane & 3, b = (lane >> 2) & 1, t = lane >> 3;
+    uint32_t src[2][4], dst[2][4];
+#pragma unroll
+    for (int pass = 0; pass < 2; ++pass) {
+      const int h = b ^ pass;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        src[pass][i] = swz128((uint32_t)((8 * q + 4 * h + ((i + q) & 3)) * 128 + (2 * t + b) * 16));
+        dst[pass][i] = (uint32_t)(t * 1024 + h * 512) + 16 * syn_unit(4 * b + i, q);
       }
     }
-    __syncwarp();
+    if (lane == 0 && ntl > 0) load(0);
+    for (int n = 0; n < ntl; ++n) {
+      if (lane == 0 && n + 1 < ntl) load(n + 1);   // blocks until the workers have released tile n - 3
+      const int s = n % kDftSynStages;
+      prof_wait(prof, 14, &full[s], (n / kDftSynStages) & 1, lane == 0);
+      uint8_t* const st = gbase + 32768 + s * 16384;
+      // all 32 loads of the lane before its stores: one shared-memory round trip per tile (a tile of a short row has few tasks to hide it)
+      float4 v[4][2][4];
+#pragma unroll
+      for (int blk4 = 0; blk4 < 4; ++blk4)   // (plane, c / 4): 4 KB apart
+#pragma unroll
+        for (int pass = 0; pass < 2; ++pass)
+#pragma unroll
+          for (int i = 0; i < 4; ++i) v[blk4][pass][i] = *reinterpret_cast<const float4*>(st + blk4 * 4096 + src[pass][i]);
+      __syncwarp();   // every lane has read the stage before any lane overwrites it
+#pragma unroll
+      for (int blk4 = 0; blk4 < 4; ++blk4) {
+        uint8_t* const sb = st + blk4 * 4096;
+        const float4(&w)[2][4] = v[blk4];
+#pragma unroll
+        for (int pass = 0; pass < 2; ++pass) {
+          *reinterpret_cast<float4*>(sb + dst[pass][0]) = make_float4(w[pass][0].x, w[pass][1].x, w[pass][2].x, w[pass][3].x);
+          *reinterpret_cast<float4*>(sb + dst[pass][1]) = make_float4(w[pass][0].y, w[pass][1].y, w[pass][2].y, w[pass][3].y);
+          *reinterpret_cast<float4*>(sb + dst[pass][2]) = make_float4(w[pass][0].z, w[pass][1].z, w[pass][2].z, w[pass][3].z);
+          *reinterpret_cast<float4*>(sb + dst[pass][3]) = make_float4(w[pass][0].w, w[pass][1].w, w[pass][2].w, w[pass][3].w);
+        }
+      }
+      fence_proxy_async();      // the next TMA load into the stage (async proxy) is ordered after these stores
+      mbar_arrive(&ready[s]);   // every lane: its stores of the stage are released to the workers
+    }
   } else if (is_store) {
     if (lane == 0) {
       int n = 0;
       for (int ti = blockIdx.x; ti < p.ntiles; ti += gridDim.x, ++n) {
         const int b = n & 1;
         prof_wait(prof, 11, &staged[b], (n >> 1) & 1, true);
-        const int r = ti / p.ktiles, k0 = (ti - r * p.ktiles) * 8;
+        const int r = p.ktiles.div(ti), k0 = (ti - r * p.ktiles.d) * 8;
         if (k0 < p.nlat)   // tiles of the padding rows kp > nlat: nothing to store (rows k >= nlat of a partial tile are clipped by TMA)
           for (int bx = 0; bx * ow < nlon; ++bx) tma_store_3d(&p.tmY, sO + b * obytes + bx * 8 * ow * (uint32_t)sizeof(T), bx * ow, k0, r);
         bulk_commit();
@@ -362,21 +470,14 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
     const bool n2odd = (N2 & 1) != 0;
     const float smul = p.mode == 0 ? 2.f : 1.f;
     const int nyq_m = nlon / 2;
-    const uint8_t* const gE = gbase;
-    // B fragment of the class c: K rows kk + q (+ 4), column 8 c + lane / 4 of the MN-major latspec stage.  Under the 128-byte swizzle the
-    // XOR term of those rows is (q (+ 4)) << 4 for every kk, so the lane's byte offset of column 8 (c % 4) + lane / 4 is fixed; the class
-    // block c / 4 (4096 B), kk (128 B rows) and the imaginary plane (8192 B) only add to it.
-    uint32_t zoff[2][4];
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) zoff[h][cc] = swz128((uint32_t)((kpi + 4 * h) * 128 + (8 * cc + (lane >> 2)) * 4));
-    mbar_wait(e_full, 0);
-    for (int task = warp; warp < nwork; task += nwork) {
-      const int n = task / nblk, blk = task - n * nblk;   // tile n of this CTA, 8-column block blk
+    const uint8_t* const zl = gbase + 32768 + syn_unit(lane >> 2, kpi) * 16;   // this lane's unit in block 0 of stage 0
+    const uint4* const al = reinterpret_cast<const uint4*>(gbase) + lane;
+    int n = 0, blk = warp;   // task n * nblk + blk
+    if (blk >= nblk) { blk -= nblk; ++n; }   // warp < nwork <= 2 nblk
+    while (warp < nwork) {
       const int ti = blockIdx.x + n * gridDim.x;
       if (ti >= p.ntiles) break;
-      const int r = ti / p.ktiles, k0 = (ti - r * p.ktiles) * 8;
+      const int r = p.ktiles.div(ti), k0 = (ti - r * p.ktiles.d) * 8;
       const int ka = k0 + 2 * kpi;
       const int s = n % kDftSynStages, it = n / kDftSynStages;
       // per-row output factors:  out = x * sc + off(parity of the longitude)
@@ -394,11 +495,11 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
           zna = zn.x; znb = zn.y;
         }
       }
-      const float bias = p.bias ? __ldg(p.bias + r % p.C) : 0.f;
+      const float bias = p.bias ? __ldg(p.bias + (r - p.C.div(r) * p.C.d)) : 0.f;
       const pr sc = make_pr(smul * rsa, smul * rsb);
       const pr off_e = make_pr(bias - rsa * (z0a + zna), bias - rsb * (z0b + znb));   // even longitude j
       const pr off_o = make_pr(bias - rsa * (z0a - zna), bias - rsb * (z0b - znb));   // odd longitude j
-      prof_wait(prof, 9, &full[s], it & 1, lane == 0);
+      prof_wait(prof, 9, &ready[s], it & 1, lane == 0);
       if (prof && lane == 0) atomicAdd(prof + 13, 1ull);
       // rows of the A tile blk: cos then sin of the columns j2 = 8 blk + lane / 4, so the accumulator elements 0, 1 / 2, 3 of
       // acc[0] are S1 = cos . Zr / S3 = sin . Zr, of acc[1] S4 = cos . Zi / S2 = sin . Zi (32 orders m2; columns (class c, latitude))
@@ -408,19 +509,21 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
 #pragma unroll
         for (int c = 0; c < 8; ++c) acc[a][c][0] = acc[a][c][1] = acc[a][c][2] = acc[a][c][3] = 0.f;
       {
-        const uint8_t* const zs = gbase + 32768 + (size_t)s * 16384;
+        const uint8_t* const zs = zl + s * 16384;
+        const uint4* const ab = al + blk * 128;
 #pragma unroll
-        for (int kk = 0; kk < 32; kk += 8) {
-          uint32_t fa[4];
-          frag_a<false>(gE, 16 * blk, kk, fa);
+        for (int h = 0; h < 2; ++h) {   // k8 steps 2 h, 2 h + 1: one 16-byte unit of B per class and plane
+          const uint4 a0 = ab[64 * h], a1 = ab[64 * h + 32];
+          const uint32_t fa0[4] = {a0.x, a0.y, a0.z, a0.w}, fa1[4] = {a1.x, a1.y, a1.z, a1.w};
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {   // frag_b<true>(zs (+ 8192), 8 c, kk) with the lane's swizzled offsets hoisted out of the task loop
-            const uint8_t* const zc = zs + (c >> 2) * 4096 + kk * 128;
-            const uint32_t zr[2] = {*reinterpret_cast<const uint32_t*>(zc + zoff[0][c & 3]), *reinterpret_cast<const uint32_t*>(zc + zoff[1][c & 3])};
-            const uint32_t zi[2] = {*reinterpret_cast<const uint32_t*>(zc + 8192 + zoff[0][c & 3]),
-                                    *reinterpret_cast<const uint32_t*>(zc + 8192 + zoff[1][c & 3])};
-            mma_tf32(acc[0][c], fa, zr);
-            mma_tf32(acc[1][c], fa, zi);
+          for (int c = 0; c < 8; ++c) {
+            const uint4 zr = *reinterpret_cast<const uint4*>(zs + (c >> 2) * 4096 + (c & 3) * 1024 + h * 512);
+            const uint4 zi = *reinterpret_cast<const uint4*>(zs + 8192 + (c >> 2) * 4096 + (c & 3) * 1024 + h * 512);
+            const uint32_t zr0[2] = {zr.x, zr.y}, zr1[2] = {zr.z, zr.w}, zi0[2] = {zi.x, zi.y}, zi1[2] = {zi.z, zi.w};
+            mma_tf32(acc[0][c], fa0, zr0);
+            mma_tf32(acc[1][c], fa0, zi0);
+            mma_tf32(acc[0][c], fa1, zr1);
+            mma_tf32(acc[1][c], fa1, zi1);
           }
         }
       }
@@ -432,12 +535,19 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
         const bool paired = valid && j2 != 0 && 2 * j2 != N2;
         const int jp = N2 - j2;
         float2 tw[8], tp[8];
-        tw[0] = make_float2(1.f, 0.f);
+        {
+          const float4* const tr = tws + 4 * (valid ? j2 : 0);   // class 0 of the table: 1
 #pragma unroll
-        for (int c = 1; c < 8; ++c) tw[c] = valid ? tws[c * N2 + j2] : make_float2(1.f, 0.f);
+          for (int i = 0; i < 4; ++i) {
+            const float4 w = tr[i];
+            tw[2 * i] = make_float2(w.x, w.y);
+            tw[2 * i + 1] = make_float2(w.z, w.w);
+          }
+        }
         dft_partner_twiddles(tw, tp);
-        // output tile element (row kr, longitude j) at ((j / ow) * 8 + kr) * ow + j % ow
-        T* const ob = outS + (size_t)(n & 1) * (obytes / sizeof(T)) + 2 * kpi * ow;
+        // output tile element (row kr, longitude j) at ((j / ow) * 8 + kr) * ow + j % ow; rows 2 kpi and 2 kpi + 1 of this thread
+        uint8_t* const ob0 = reinterpret_cast<uint8_t*>(outS) + (n & 1) * obytes + 2 * kpi * ow * (int)sizeof(T);
+        uint8_t* const ob1 = ob0 + ow * (int)sizeof(T);
         if (n >= 2) prof_wait(prof, 10, &ofree[n & 1], ((n >> 1) - 1) & 1, lane == 0);
         {
           pr vr[8], vi[8], x[8];
@@ -454,7 +564,7 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
 #pragma unroll
           for (int j1 = 0; j1 < 8; ++j1) {   // longitude N2 j1 + j2
             const pr o = rfma(x[j1], sc, (n2odd && (j1 & 1)) ? o1 : o0);
-            if (valid) { st_out<T>(ob + of[j1], o.v.x); st_out<T>(ob + of[j1] + ow, o.v.y); }
+            if (valid) st_out2<T>(ob0 + of[j1], ob1 + of[j1], o.v.x, o.v.y);
           }
         }
         {
@@ -472,12 +582,15 @@ __global__ void __launch_bounds__(kDftSynThreads, 1) dft_synthesis_kernel(const 
 #pragma unroll
           for (int j1 = 0; j1 < 8; ++j1) {   // not for the unpaired columns 0 and N2 / 2
             const pr o = rfma(x[j1], sc, (n2odd && (j1 & 1)) ? o1 : o0);
-            if (paired) { st_out<T>(ob + of[j1], o.v.x); st_out<T>(ob + of[j1] + ow, o.v.y); }
+            if (paired) st_out2<T>(ob0 + of[j1], ob1 + of[j1], o.v.x, o.v.y);
           }
         }
         fence_proxy_async();   // the bulk stores read the tile through the async proxy: every writing thread fences and arrives
         mbar_arrive(&staged[n & 1]);
       }
+      blk += nwork;   // next task: nwork <= 2 nblk, so at most two wraps
+      if (blk >= nblk) { blk -= nblk; ++n; }
+      if (blk >= nblk) { blk -= nblk; ++n; }
     }
   }
   __syncthreads();
@@ -492,10 +605,10 @@ int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int
   const int R = B * C;
   DftSynParams p;
   memset(&p, 0, sizeof(p));
-  p.Z = Z; p.tw = t->tw; p.rowscale = pl->d_rowscale; p.bias = bias; p.prof = dft_prof_buffer();
-  p.R = R; p.C = C; p.nlat = pl->nlat; p.nlon = pl->nlon; p.kp = pl->kp; p.mmax = pl->mmax;
+  p.Z = Z; p.et = t->et; p.tw = t->tw; p.rowscale = pl->d_rowscale; p.bias = bias; p.prof = dft_prof_buffer();
+  p.R = R; p.C = make_fastdiv(C); p.nlat = pl->nlat; p.nlon = pl->nlon; p.kp = pl->kp; p.mmax = pl->mmax;
   p.N2 = t->N2; p.half = t->half; p.mode = mode;
-  p.ktiles = pl->kp / 8; p.ntiles = R * p.ktiles;
+  p.ktiles = make_fastdiv(pl->kp / 8); p.ntiles = R * (pl->kp / 8);
   p.has_nyq = (pl->mmax == pl->nlon / 2 + 1) ? 1 : 0;
   p.M2 = t->M2;
   {
@@ -506,12 +619,6 @@ int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int
     int rc = make_tmap(&p.tmZ, Z, 5, d, s, bx);
     if (rc) return rc;
   }
-  {
-    long long d[2] = {32, 256}, s[2] = {1, 32};
-    int bx[2] = {32, 128};
-    int rc = make_tmap(&p.tmE, t->et, 2, d, s, bx);
-    if (rc) return rc;
-  }
   const bool bf16 = (dtype == B200SHT_BF16);
   p.ow = dft_out_box(t->N2);
   {
@@ -519,8 +626,8 @@ int dft_synthesis(const Plan* pl, const float* Z, void* y, int dtype, int B, int
     if (rc) return rc;
   }
   const size_t obytes = (8 * (size_t)pl->nlon * (bf16 ? 2 : 4) + 1023) & ~(size_t)1023;
-  const size_t smem = 1024 + 32768 + (size_t)kDftSynStages * 16384 + 2 * obytes + ((8 * (size_t)t->N2 * 8 + 15) & ~(size_t)15) +
-                      8 * (size_t)t->N2 * 4 + (2 * kDftSynStages + 5) * 8;
+  const size_t smem = 1024 + 32768 + (size_t)kDftSynStages * 16384 + 2 * obytes + 8 * (size_t)t->N2 * 8 + 8 * (size_t)t->N2 * 4 +
+                      (3 * kDftSynStages + 4) * 8;
   const int sms = usable_sms(pl->sm_count > 0 ? pl->sm_count : 132);
   const int ctas = p.ntiles < sms ? p.ntiles : sms;
 #define B200_LAUNCH_SYN(TT)                                                                                          \

@@ -45,6 +45,7 @@ _lib.call("b200sht_fft_synthesis", plan.handle, _ptr(lat), _ptr(y), 1, B, C, _VP
 a = read().astype(float)
 life = a[12] / ctas
 print(f"synthesis: CTA lifetime {life:.0f} clk; tasks (8 columns of a tile) {a[13]:.0f}")
-for i, nme, d in ((8, "TMA load waits stage free", 1), (9, "MMA + epilogue warps wait stage full (per warp)", 10),
+for i, nme, d in ((8, "load warp waits stage free", 1), (14, "load warp waits tile landed", 1),
+                  (9, "MMA + epilogue warps wait stage rewritten (per warp)", 10),
                   (10, "epilogues wait output tile free (per warp)", 10), (11, "TMA store waits output tile written", 1)):
     print(f"  {nme:45s} {a[i] / ctas / d:10.0f} clk  = {100 * a[i] / ctas / d / life:5.1f}% of the CTA lifetime")
