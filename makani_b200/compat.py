@@ -11,6 +11,7 @@ registered in `sys.modules` BEFORE `import makani`:
     compat.patch_makani_spectral_layers()      # makani.models.common.SpectralConv/SpectralAttention -> makani_b200 (optional)
     compat.patch_makani_norm_layers()          # makani's (Distributed)GeometricInstanceNormS2 -> makani_b200 (optional)
     compat.patch_makani_layer_norm()           # makani's DistributedLayerNorm -> makani_b200 (optional)
+    compat.patch_makani_instance_norm()        # makani's DistributedInstanceNorm2d -> makani_b200 (optional)
     import makani
 """
 import importlib
@@ -108,3 +109,17 @@ def patch_makani_layer_norm():
         net = sys.modules.get(modname)
         if net is not None and hasattr(net, "DistributedLayerNorm"):
             net.DistributedLayerNorm = DistributedLayerNorm
+
+
+def patch_makani_instance_norm():
+    """After `import makani`: point makani.mpu.layer_norm.DistributedInstanceNorm2d (SFNO's default `instance_norm` when the spatial group has more
+    than one rank) at the CUDA-backed class, and the name that sfnonet / snonet imported at module load.  FourCastNet 3 and 3.1 import it inside a
+    function, so the module attribute covers them.  makani's DistributedGeometricInstanceNormS2 keeps its own base class."""
+    from makani_b200.distributed import DistributedInstanceNorm2d
+
+    m = sys.modules.get("makani.mpu.layer_norm") or importlib.import_module("makani.mpu.layer_norm")
+    m.DistributedInstanceNorm2d = DistributedInstanceNorm2d
+    for modname in ("makani.models.networks.sfnonet", "makani.models.networks.snonet"):
+        net = sys.modules.get(modname)
+        if net is not None and hasattr(net, "DistributedInstanceNorm2d"):
+            net.DistributedInstanceNorm2d = DistributedInstanceNorm2d

@@ -19,6 +19,7 @@ DistributedDiscreteContinuousConvS2 (distributed/disco.py: a latitude halo and w
 (distributed/resample.py: whole spheres of a subset of planes) are FCN3's local operators under the same h x w grid;
 DistributedDiscreteContinuousConvTransposeS2 runs the DISCO stages the other way round, and DistributedNeighborhoodAttentionS2
 (distributed/attention.py) runs the attention kernels on window plans of the neighbourhood, over the same halo.
+DistributedGeometricInstanceNormS2 and DistributedInstanceNorm2d (distributed/norm.py) gather per-rank statistics between the staged norm kernels.
 """
 import ctypes
 
@@ -492,4 +493,4 @@ class DistributedInverseRealVectorSHT(_DistributedBase):
 from .disco import DistributedDiscreteContinuousConvS2, DistributedDiscreteContinuousConvTransposeS2, set_disco_local_ops  # noqa: E402,F401
 from .resample import DistributedResampleS2, set_resample_local_ops  # noqa: E402,F401
 from .attention import DistributedNeighborhoodAttentionS2, set_attention_local_ops  # noqa: E402,F401
-from .norm import DistributedGeometricInstanceNormS2, set_norm_local_ops  # noqa: E402,F401
+from .norm import DistributedGeometricInstanceNormS2, DistributedInstanceNorm2d, set_norm_local_ops  # noqa: E402,F401
