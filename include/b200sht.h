@@ -20,6 +20,7 @@
  *   b200sht_disco_forward/adjoint<- the psi contraction of torch_harmonics.DiscreteContinuousConvS2 and its adjoint (fourcastnet3.py:117-252, :511-543)
  *   b200sht_resample_forward/adjoint <- torch_harmonics.ResampleS2(mode="bilinear") and its adjoint (fourcastnet3.py:356-358)
  *   b200sht_attention_forward/backward <- the attention of torch_harmonics.NeighborhoodAttentionS2 (not constructed by makani)
+ *   b200sht_attention_global_forward/backward <- the attention of torch_harmonics.AttentionS2 (not constructed by makani)
  *
  * Conventions
  *   - every function returns 0 on success, a negative b200sht_status otherwise; b200sht_last_error() gives text.
@@ -414,6 +415,26 @@ int b200sht_attention_forward(const b200sht_disco_plan* plan, const float* q, co
 int b200sht_attention_backward(const b200sht_disco_plan* plan, const float* q, const float* k, const float* v, const float* y, const float* lse,
                                const float* dy, float* dq, float* dk, float* dv, float* D, int B, int heads, int ek, int ev, float scale,
                                void* stream);
+
+/* ------------------------------------------------------------------ global attention on the sphere
+ * The attention of torch_harmonics.AttentionS2 (makani_b200/attention.py, DESIGN.md section 4.10): SDPA with a float mask over the keys.
+ * Per head (b, h) of BH = B heads, with the per-key bias b_j (log w_j, -inf for a key that must drop out):
+ *   l_ij = scale <q_i, k_j> + b_j,   o_i = sum_j exp(l_ij) v_j / sum_j exp(l_ij),   lse_i = log sum_j exp(l_ij)
+ * Operands (fp32, device, contiguous): q, dq [BH][nq][dqk], k, dk [BH][nk][dqk], v, dv [BH][dv][nk] (channel-major: the NCHW order of a
+ *   head), o, dout [BH][nq][dv], lse [BH][nq], bias [nk] (shared by all heads).  Every query needs at least one key with a finite bias.
+ * precision: B200SHT_PREC_TF32 (TF32 wgmma, operands rounded to nearest, fp32 softmax and accumulators) or B200SHT_PREC_FP32X3 (the same
+ *   kernels with every operand split into TF32 hi + lo: a_lo b_hi + a_hi b_lo + a_hi b_hi); B200SHT_PREC_FP32 is B200SHT_ERR_UNSUPPORTED.
+ * workspace: b200sht_attention_global_workspace_floats(..., backward) floats (the operands in the layouts the GEMMs read; D of the backward).
+ * b200sht_attention_global_forward: writes o and lse (flash attention: online softmax with a running max, the bias added before the max).
+ * b200sht_attention_global_backward: given dout, writes dq, dk, dv from q, k, v, o and lse: D = rowsum(dout o), then dk / dv per key
+ *   block and dq per query block, each element summed in a fixed order without atomics: results are bit-identical run to run.
+ * Head dims dqk, dv: multiples of 8 up to 128, otherwise B200SHT_ERR_UNSUPPORTED (the workspace query returns -1).  BH at most 65535. */
+int64_t b200sht_attention_global_workspace_floats(int BH, int nq, int nk, int dqk, int dv, int precision, int backward);
+int b200sht_attention_global_forward(const float* q, const float* k, const float* v, const float* bias, float* o, float* lse, int BH, int nq,
+                                     int nk, int dqk, int dv, float scale, int precision, void* workspace, void* stream);
+int b200sht_attention_global_backward(const float* q, const float* k, const float* v, const float* bias, const float* o, const float* lse,
+                                      const float* dout, float* dq, float* dk, float* dv, int BH, int nq, int nk, int dqk, int dvh, float scale,
+                                      int precision, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------ bilinear resampling on the sphere
  * Replaces torch_harmonics.ResampleS2(mode="bilinear"), the upsampling of FCN3's DiscreteContinuousDecoder with upsample_sht=False

@@ -7,6 +7,7 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     DiscreteContinuousConvTransposeS2          <- torch_harmonics.DiscreteContinuousConvTransposeS2 (learnable upsampling; morlet basis)
     ResampleS2                                 <- torch_harmonics.ResampleS2 (FCN3's and SNO's decoders; mode "bilinear")
     NeighborhoodAttentionS2                    <- torch_harmonics.NeighborhoodAttentionS2 (local attention on the DISCO neighbourhoods)
+    AttentionS2                                <- torch_harmonics.AttentionS2 (global attention, quadrature-weighted keys)
     SpectralConv, SpectralAttention, ComplexReLU <- makani.models.common.*
     quadrature                                 <- torch_harmonics.quadrature
     distributed                                <- torch_harmonics.distributed (h x w spatial model parallelism; its
@@ -22,7 +23,7 @@ from .sht import RealSHT, InverseRealSHT, get_plan, resolve_precision  # noqa: F
 from .vector_sht import RealVectorSHT, InverseRealVectorSHT  # noqa: F401
 from .disco import DiscreteContinuousConvS2, DiscreteContinuousConvTransposeS2  # noqa: F401
 from .resample import ResampleS2  # noqa: F401
-from .attention import NeighborhoodAttentionS2  # noqa: F401
+from .attention import NeighborhoodAttentionS2, AttentionS2  # noqa: F401
 from .spectral_convolution import SpectralConv, SpectralAttention, ComplexReLU, mix_packed  # noqa: F401
 from .host_pipeline import HostFeed  # noqa: F401
 

@@ -110,6 +110,11 @@ _SIGNATURES = {
     # neighbourhood attention on the sphere (on a K = 1 DISCO plan)
     "b200sht_attention_forward": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, _P]),
     "b200sht_attention_backward": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, _P]),
+    # global attention on the sphere
+    "b200sht_attention_global_workspace_floats": (c_int64, [c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
+    "b200sht_attention_global_forward": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, _P, _P]),
+    "b200sht_attention_global_backward": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, _P,
+                                                  _P]),
     # bilinear resampling on the sphere
     "b200sht_resample_plan_create": (c_int, [ctypes.POINTER(_P), c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     "b200sht_resample_plan_destroy": (c_int, [_P]),

@@ -1,5 +1,6 @@
 """NeighborhoodAttentionS2 -- drop-in for `torch_harmonics.NeighborhoodAttentionS2`, the local attention of torch-harmonics' spherical
-transformers, with the attention on the sm_90a kernels of csrc/attention.cu.
+transformers, with the attention on the sm_90a kernels of csrc/attention.cu.  AttentionS2 -- drop-in for `torch_harmonics.AttentionS2`, the
+global attention of the same family, on the wgmma flash-attention kernels of csrc/attention_global.cu (see its class docstring).
 
     NeighborhoodAttentionS2(in_channels, in_shape, out_shape, grid_in="equiangular", grid_out="equiangular", num_heads=1, scale=None, bias=True,
                             theta_cutoff=None, k_channels=None, out_channels=None, optimized_kernel=True)
@@ -227,3 +228,170 @@ class NeighborhoodAttentionS2(nn.Module):
         v = _project_points(value, self.v_weights, self.v_bias)
         y = _NeighborhoodAttention.apply(q, k, v, self.plan(query.device), self.num_heads, self.scale)   # (B, HW_out, C_v)
         return _project_out(y, self.proj_weights, self.proj_bias).view(B, self.out_channels, self.nlat_out, self.nlon_out)
+
+
+# ------------------------------------------------------------------------------------------------------------------- global attention
+GLOBAL_MAX_HEAD_DIM = 128   # head dims served by csrc/attention_global.cu: multiples of 8 up to this
+
+
+def _global_precision():
+    """TF32 wgmma when torch allows TF32 matmuls, otherwise 3 x TF32 operand splitting in the same kernels"""
+    return _lib.PREC_TF32 if torch.backends.cuda.matmul.allow_tf32 else _lib.PREC_FP32X3
+
+
+def _global_workspace(BH, nq, nk, dqk, dv, precision, backward, device):
+    n = _lib.load().b200sht_attention_global_workspace_floats(BH, nq, nk, dqk, dv, precision, int(backward))
+    if n < 0:
+        raise B200ShtError(f"global attention: no workspace for head dims {dqk}, {dv}")
+    return torch.empty(n, dtype=torch.float32, device=device)
+
+
+def global_attention_forward(q, k, v, bias, scale, precision):
+    """q (B, H, nq, dqk), k (B, H, nk, dqk), v (B, H, dv, nk), bias (nk,): fp32 contiguous CUDA tensors -> o (B, H, nq, dv), lse (B, H, nq)"""
+    B, H, nq, dqk = q.shape
+    dv, nk = v.shape[2], v.shape[3]
+    o = torch.empty((B, H, nq, dv), dtype=torch.float32, device=q.device)
+    lse = torch.empty((B, H, nq), dtype=torch.float32, device=q.device)
+    ws = _global_workspace(B * H, nq, nk, dqk, dv, precision, False, q.device)
+    _lib.call("b200sht_attention_global_forward", _ptr(q), _ptr(k), _ptr(v), _ptr(bias), _ptr(o), _ptr(lse), B * H, nq, nk, dqk, dv,
+              float(scale), precision, _ptr(ws), _stream(q.device))
+    return o, lse
+
+
+def global_attention_backward(q, k, v, bias, o, lse, do, scale, precision):
+    """-> dq, dk, dv (shapes of q, k, v); do (B, H, nq, dv) fp32 contiguous"""
+    B, H, nq, dqk = q.shape
+    dv, nk = v.shape[2], v.shape[3]
+    dq, dk, dvt = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+    ws = _global_workspace(B * H, nq, nk, dqk, dv, precision, True, q.device)
+    _lib.call("b200sht_attention_global_backward", _ptr(q), _ptr(k), _ptr(v), _ptr(bias), _ptr(o), _ptr(lse), _ptr(do), _ptr(dq), _ptr(dk),
+              _ptr(dvt), B * H, nq, nk, dqk, dv, float(scale), precision, _ptr(ws), _stream(q.device))
+    return dq, dk, dvt
+
+
+class _GlobalAttention(torch.autograd.Function):
+    """o = softmax(scale q k^T + bias) v per head.  Saves q, k, v, o and lse."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, bias, scale, precision):
+        q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
+        o, lse = global_attention_forward(q, k, v, bias, scale, precision)
+        ctx.save_for_backward(q, k, v, o, lse)
+        ctx.bias, ctx.scale, ctx.precision = bias, scale, precision
+        return o
+
+    @staticmethod
+    def backward(ctx, do):
+        q, k, v, o, lse = ctx.saved_tensors
+        dq, dk, dv = global_attention_backward(q, k, v, ctx.bias, o, lse, do.to(torch.float32).contiguous(), ctx.scale, ctx.precision)
+        return dq, dk, dv, None, None, None
+
+
+def _project_channels(x, weight, bias):
+    """1x1 projection of x (B, C_in, H, W) into the channel-major (B, C_out, H W), fp32, one GEMM"""
+    B, C = x.shape[0], x.shape[1]
+    xf = x.to(torch.float32).reshape(B, C, -1)
+    w = weight.to(torch.float32).reshape(weight.shape[0], C).expand(B, -1, -1)
+    if bias is None:
+        return torch.bmm(w, xf)
+    return torch.baddbmm(bias.to(torch.float32).view(1, -1, 1).expand(B, -1, xf.shape[2]), w, xf)
+
+
+class AttentionS2(nn.Module):
+    """Global attention on the sphere (drop-in for torch_harmonics.AttentionS2).
+
+    AttentionS2(in_channels, num_heads, in_shape, out_shape, grid_in="equiangular", grid_out="equiangular", scale=None, bias=True,
+                k_channels=None, out_channels=None, drop_rate=0.0)
+    forward(query, key=None, value=None): query (B, C_in, *out_shape), key / value (B, C_in, *in_shape), fp32 / bf16 on a CUDA device
+                                          -> float32 (B, C_v, *out_shape)
+
+    Every output point attends to every input point, with the quadrature weight of the key as a float mask (SDPA with attn_mask = log w):
+
+        q = W_q query + b_q,  k = W_k key + b_k,  v = W_v value + b_v          (1x1 projections; head h on channels [h E, (h + 1) E))
+        y_h(i) = softmax_j(scale <q_h(i), k_h(j)> + log w_j) v_h(j),  w_j = 2 pi w_in[lat(j)] / nlon_in,  out = W_proj y + b_proj
+
+    A key of zero quadrature weight drops out (bias -inf).  Parameters as NeighborhoodAttentionS2's: q_weights, k_weights (C_k, C_in, 1, 1),
+    v_weights (C_v, C_in, 1, 1), proj_weights (C_v, C_v, 1, 1), xavier-uniform; with bias=True zero q_bias, k_bias (C_k,), v_bias,
+    proj_bias (C_v,).  Head dims C_k / num_heads and C_v / num_heads must be multiples of 8 up to 128.  scale defaults to
+    1 / sqrt(C_k / num_heads).  The key bias is a non-persistent buffer (a state dict holds the parameters only).  drop_rate > 0 is accepted
+    and raises NotImplementedError when it would drop (in training).  The projections are cuBLAS GEMMs; the attention runs on TF32 wgmma when
+    torch.backends.cuda.matmul.allow_tf32, otherwise on 3 x TF32 in the same kernels (fp32 accuracy)."""
+
+    def __init__(self, in_channels, num_heads, in_shape, out_shape, grid_in="equiangular", grid_out="equiangular", scale=None, bias=True,
+                 k_channels=None, out_channels=None, drop_rate=0.0):
+        super().__init__()
+        self.in_channels = in_channels
+        self.k_channels = k_channels if k_channels is not None else in_channels
+        self.out_channels = out_channels if out_channels is not None else in_channels
+        self.num_heads = num_heads
+        if num_heads < 1 or self.k_channels % num_heads or self.out_channels % num_heads:
+            raise ValueError(f"k_channels {self.k_channels} and out_channels {self.out_channels} must be divisible by num_heads {num_heads}")
+        ek, ev = self.k_channels // num_heads, self.out_channels // num_heads
+        for e in (ek, ev):
+            if e % 8 or e > GLOBAL_MAX_HEAD_DIM:
+                raise NotImplementedError(f"head dims {ek}, {ev}: the global attention kernels serve multiples of 8 up to {GLOBAL_MAX_HEAD_DIM}")
+        self.nlat_in, self.nlon_in = in_shape
+        self.nlat_out, self.nlon_out = out_shape
+        self.grid_in, self.grid_out = grid_in, grid_out
+        self.scale = float(scale) if scale is not None else 1.0 / math.sqrt(ek)
+        self.drop_rate = float(drop_rate)
+        _grid_np(self.nlat_out, grid_out)   # validates the output grid name
+        omega = 2.0 * np.pi * _grid_np(self.nlat_in, grid_in)[1] / self.nlon_in
+        if not np.any(omega > 0):
+            raise ValueError(f"every key of the {grid_in} grid {tuple(in_shape)} has zero quadrature weight: no query has a key to attend to")
+        with np.errstate(divide="ignore"):
+            log_w = np.where(omega > 0, np.log(np.where(omega > 0, omega, 1.0)), -np.inf)
+        self.register_buffer("key_bias", torch.from_numpy(np.repeat(log_w, self.nlon_in).astype(np.float32)), persistent=False)
+
+        def xavier(co, ci):
+            w = torch.empty(co, ci, 1, 1)
+            nn.init.xavier_uniform_(w)
+            return nn.Parameter(w)
+
+        self.q_weights = xavier(self.k_channels, in_channels)
+        self.k_weights = xavier(self.k_channels, in_channels)
+        self.v_weights = xavier(self.out_channels, in_channels)
+        self.proj_weights = xavier(self.out_channels, self.out_channels)
+        if bias:
+            self.q_bias = nn.Parameter(torch.zeros(self.k_channels))
+            self.k_bias = nn.Parameter(torch.zeros(self.k_channels))
+            self.v_bias = nn.Parameter(torch.zeros(self.out_channels))
+            self.proj_bias = nn.Parameter(torch.zeros(self.out_channels))
+        else:
+            self.q_bias = self.k_bias = self.v_bias = self.proj_bias = None
+
+    def extra_repr(self):
+        return (f"in_channels={self.in_channels}, k_channels={self.k_channels}, out_channels={self.out_channels}, num_heads={self.num_heads}, "
+                f"in_shape={(self.nlat_in, self.nlon_in)}, out_shape={(self.nlat_out, self.nlon_out)}, drop_rate={self.drop_rate}")
+
+    def _check(self, x, shape, what):
+        if not x.is_cuda:
+            raise B200ShtError(f"{type(self).__name__} runs on CUDA devices only; makani_b200 has no CPU fallback")
+        if x.dtype not in (torch.float32, torch.bfloat16):
+            raise TypeError(f"{what}: float32 or bfloat16 inputs are served, got {x.dtype}")
+        if x.dim() != 4 or x.shape[1] != self.in_channels or tuple(x.shape[2:]) != shape:
+            raise ValueError(f"{what}: expected (B, {self.in_channels}, {shape[0]}, {shape[1]}), got {tuple(x.shape)}")
+
+    def forward(self, query, key=None, value=None):
+        if (key is None or value is None) and (self.nlat_in, self.nlon_in) != (self.nlat_out, self.nlon_out):
+            raise ValueError("key and value default to query, which needs in_shape == out_shape")
+        if self.training and self.drop_rate > 0.0:
+            raise NotImplementedError("AttentionS2: attention dropout (drop_rate > 0 in training) is not implemented")
+        key = query if key is None else key
+        value = query if value is None else value
+        self._check(query, (self.nlat_out, self.nlon_out), "query")
+        self._check(key, (self.nlat_in, self.nlon_in), "key")
+        self._check(value, (self.nlat_in, self.nlon_in), "value")
+        if key.shape[0] != query.shape[0] or value.shape[0] != query.shape[0]:
+            raise ValueError("query, key and value must have the same batch size")
+        B, H = query.shape[0], self.num_heads
+        ek, ev = self.k_channels // H, self.out_channels // H
+        nq, nk = self.nlat_out * self.nlon_out, self.nlat_in * self.nlon_in
+        q = _project_channels(query, self.q_weights, self.q_bias).view(B, H, ek, nq).transpose(2, 3)   # (B, H, nq, ek)
+        k = _project_channels(key, self.k_weights, self.k_bias).view(B, H, ek, nk).transpose(2, 3)
+        v = _project_channels(value, self.v_weights, self.v_bias).view(B, H, ev, nk)                    # NCHW order of each head
+        o = _GlobalAttention.apply(q, k, v, self.key_bias.to(query.device), self.scale, _global_precision())   # (B, H, nq, ev)
+        y = o.transpose(2, 3).reshape(B, self.out_channels, nq)
+        wp = self.proj_weights.to(torch.float32).reshape(self.out_channels, self.out_channels).expand(B, -1, -1)
+        out = torch.bmm(wp, y) if self.proj_bias is None else torch.baddbmm(self.proj_bias.to(torch.float32).view(1, -1, 1).expand(B, -1, nq), wp, y)
+        return out.view(B, self.out_channels, self.nlat_out, self.nlon_out)

@@ -42,6 +42,7 @@ def install_torch_harmonics_shim(force=False):
     th.DiscreteContinuousConvTransposeS2 = mb.DiscreteContinuousConvTransposeS2
     th.ResampleS2 = mb.ResampleS2
     th.NeighborhoodAttentionS2 = mb.NeighborhoodAttentionS2
+    th.AttentionS2 = mb.AttentionS2
     fb = types.ModuleType("torch_harmonics.filter_basis")
     fb.get_filter_basis, fb.MorletFilterBasis = mbdisco.get_filter_basis, mbdisco.MorletFilterBasis
     th.filter_basis = fb

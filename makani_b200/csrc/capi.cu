@@ -95,6 +95,12 @@ int attention_forward(const b200sht_disco_plan* pl, const float* q, const float*
                       int EV, float scale, cudaStream_t st);
 int attention_backward(const b200sht_disco_plan* pl, const float* q, const float* k, const float* v, const float* y, const float* lse,
                        const float* dy, float* dq, float* dk, float* dv, float* D, int B, int H, int EK, int EV, float scale, cudaStream_t st);
+long long attention_global_workspace_floats(int BH, int nq, int nk, int dqk, int dv, int split, int backward);
+int attention_global_forward(const float* q, const float* k, const float* v, const float* bias, float* o, float* lse, int BH, int nq, int nk,
+                             int dqk, int dv, float scale, int split, float* ws, cudaStream_t st);
+int attention_global_backward(const float* q, const float* k, const float* v, const float* bias, const float* o, const float* lse, const float* dout,
+                              float* dq, float* dk, float* dv_, int BH, int nq, int nk, int dqk, int dv, float scale, int split, float* ws,
+                              cudaStream_t st);
 int resample_plan_create(b200sht_resample_plan** out, int nlat_in, int nlon_in, int nlat_out, int nlon_out, int expand_poles, const int* lat_idx,
                          const float* lat_w, const int* lon_left, const int* lon_right, const float* lon_w, cudaStream_t st);
 int resample_plan_destroy(b200sht_resample_plan* pl);
@@ -927,6 +933,35 @@ int b200sht_attention_backward(const b200sht_disco_plan* plan, const float* q, c
                                const float* dy, float* dq, float* dk, float* dv, float* D, int B, int heads, int ek, int ev, float scale,
                                void* stream) {
   return attention_backward(plan, q, k, v, y, lse, dy, dq, dk, dv, D, B, heads, ek, ev, scale, S(stream));
+}
+
+// ---- global attention on the sphere (attention_global.cu)
+static int attention_global_split(int precision) {
+  if (precision == B200SHT_PREC_TF32) return 0;
+  if (precision == B200SHT_PREC_FP32X3) return 1;
+  return -1;
+}
+
+int64_t b200sht_attention_global_workspace_floats(int BH, int nq, int nk, int dqk, int dv, int precision, int backward) {
+  const int split = attention_global_split(precision);
+  if (split < 0) return -1;
+  return attention_global_workspace_floats(BH, nq, nk, dqk, dv, split, backward);
+}
+
+int b200sht_attention_global_forward(const float* q, const float* k, const float* v, const float* bias, float* o, float* lse, int BH, int nq,
+                                     int nk, int dqk, int dv, float scale, int precision, void* workspace, void* stream) {
+  const int split = attention_global_split(precision);
+  if (split < 0) { set_error("attention_global: precision %d (TF32 or FP32X3 are served)", precision); return B200SHT_ERR_UNSUPPORTED; }
+  return attention_global_forward(q, k, v, bias, o, lse, BH, nq, nk, dqk, dv, scale, split, static_cast<float*>(workspace), S(stream));
+}
+
+int b200sht_attention_global_backward(const float* q, const float* k, const float* v, const float* bias, const float* o, const float* lse,
+                                      const float* dout, float* dq, float* dk, float* dv, int BH, int nq, int nk, int dqk, int dvh, float scale,
+                                      int precision, void* workspace, void* stream) {
+  const int split = attention_global_split(precision);
+  if (split < 0) { set_error("attention_global: precision %d (TF32 or FP32X3 are served)", precision); return B200SHT_ERR_UNSUPPORTED; }
+  return attention_global_backward(q, k, v, bias, o, lse, dout, dq, dk, dv, BH, nq, nk, dqk, dvh, scale, split, static_cast<float*>(workspace),
+                                   S(stream));
 }
 
 // ---- bilinear resampling on the sphere (resample.cu)
