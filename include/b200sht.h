@@ -21,6 +21,7 @@
  *   b200sht_resample_forward/adjoint <- torch_harmonics.ResampleS2(mode="bilinear") and its adjoint (fourcastnet3.py:356-358)
  *   b200sht_attention_forward/backward <- the attention of torch_harmonics.NeighborhoodAttentionS2 (not constructed by makani)
  *   b200sht_attention_global_forward/backward <- the attention of torch_harmonics.AttentionS2 (not constructed by makani)
+ *   b200sht_attention_global_rowdot/backward_kv/backward_q <- its backward per rank under h x w spatial model parallelism
  *
  * Conventions
  *   - every function returns 0 on success, a negative b200sht_status otherwise; b200sht_last_error() gives text.
@@ -425,9 +426,19 @@ int b200sht_attention_backward(const b200sht_disco_plan* plan, const float* q, c
  * precision: B200SHT_PREC_TF32 (TF32 wgmma, operands rounded to nearest, fp32 softmax and accumulators) or B200SHT_PREC_FP32X3 (the same
  *   kernels with every operand split into TF32 hi + lo: a_lo b_hi + a_hi b_lo + a_hi b_hi); B200SHT_PREC_FP32 is B200SHT_ERR_UNSUPPORTED.
  * workspace: b200sht_attention_global_workspace_floats(..., backward) floats (the operands in the layouts the GEMMs read; D of the backward).
+ *   The backward workspace of (BH, nq, nk, dqk, dv, precision) also serves b200sht_attention_global_backward_kv and _backward_q of the
+ *   same arguments.
  * b200sht_attention_global_forward: writes o and lse (flash attention: online softmax with a running max, the bias added before the max).
  * b200sht_attention_global_backward: given dout, writes dq, dk, dv from q, k, v, o and lse: D = rowsum(dout o), then dk / dv per key
- *   block and dq per query block, each element summed in a fixed order without atomics: results are bit-identical run to run.
+ *   block and dq per query block, each element summed in a fixed order without atomics: results are bit-identical run to run.  It is
+ *   b200sht_attention_global_rowdot followed by the kv pass and the q pass below, on one set of prepared operands.
+ * The backward as separable passes, so the query-side and key-side work may run on different query and key sets (a rank of a spatially
+ * sharded grid: its own queries against all keys, its own keys against all queries).  A row of dq depends only on its query and the keys,
+ * a row of dk / dv only on its key and the queries, so every output equals the matching slice of the full backward's bit for bit.
+ *   b200sht_attention_global_rowdot: D[r] = sum_c dout[r][c] o[r][c] for the rows = BH nq rows of o, dout [rows][dv]; D [rows].
+ *   b200sht_attention_global_backward_kv: dk, dv of the nk given keys against the nq given queries; bias [nk] of the given keys, lse, D
+ *     [BH][nq] of the given queries.
+ *   b200sht_attention_global_backward_q: dq of the nq given queries against the nk given keys (bias, lse, D as above).
  * Head dims dqk, dv: multiples of 8 up to 128, otherwise B200SHT_ERR_UNSUPPORTED (the workspace query returns -1).  BH at most 65535. */
 int64_t b200sht_attention_global_workspace_floats(int BH, int nq, int nk, int dqk, int dv, int precision, int backward);
 int b200sht_attention_global_forward(const float* q, const float* k, const float* v, const float* bias, float* o, float* lse, int BH, int nq,
@@ -435,6 +446,13 @@ int b200sht_attention_global_forward(const float* q, const float* k, const float
 int b200sht_attention_global_backward(const float* q, const float* k, const float* v, const float* bias, const float* o, const float* lse,
                                       const float* dout, float* dq, float* dk, float* dv, int BH, int nq, int nk, int dqk, int dvh, float scale,
                                       int precision, void* workspace, void* stream);
+int b200sht_attention_global_rowdot(const float* o, const float* dout, float* D, int64_t rows, int dv, void* stream);
+int b200sht_attention_global_backward_kv(const float* q, const float* k, const float* v, const float* bias, const float* lse, const float* D,
+                                         const float* dout, float* dk, float* dv, int BH, int nq, int nk, int dqk, int dvh, float scale,
+                                         int precision, void* workspace, void* stream);
+int b200sht_attention_global_backward_q(const float* q, const float* k, const float* v, const float* bias, const float* lse, const float* D,
+                                        const float* dout, float* dq, int BH, int nq, int nk, int dqk, int dvh, float scale, int precision,
+                                        void* workspace, void* stream);
 
 /* ------------------------------------------------------------------ bilinear resampling on the sphere
  * Replaces torch_harmonics.ResampleS2(mode="bilinear"), the upsampling of FCN3's DiscreteContinuousDecoder with upsample_sht=False

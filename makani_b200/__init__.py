@@ -11,7 +11,8 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     SpectralConv, SpectralAttention, ComplexReLU <- makani.models.common.*
     quadrature                                 <- torch_harmonics.quadrature
     distributed                                <- torch_harmonics.distributed (h x w spatial model parallelism; its
-                                                  DistributedNeighborhoodAttentionS2 is NeighborhoodAttentionS2 on a sharded grid)
+                                                  DistributedNeighborhoodAttentionS2 and DistributedAttentionS2 are
+                                                  NeighborhoodAttentionS2 and AttentionS2 on a sharded grid)
     install_torch_harmonics_shim()             <- makes `import torch_harmonics` resolve to this package
     HostFeed                                   <- double-buffered host->device input staging (the data loader's prefetch queue)
     sfno.SphericalFourierNeuralOperatorNet     <- makani.models.networks.sfnonet (same constructor / parameters / state dict)

@@ -115,6 +115,10 @@ _SIGNATURES = {
     "b200sht_attention_global_forward": (c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, _P, _P]),
     "b200sht_attention_global_backward": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, _P,
                                                   _P]),
+    "b200sht_attention_global_rowdot": (c_int, [_P, _P, _P, c_int64, c_int, _P]),
+    "b200sht_attention_global_backward_kv": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, _P,
+                                                     _P]),
+    "b200sht_attention_global_backward_q": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, _P, _P]),
     # bilinear resampling on the sphere
     "b200sht_resample_plan_create": (c_int, [ctypes.POINTER(_P), c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     "b200sht_resample_plan_destroy": (c_int, [_P]),

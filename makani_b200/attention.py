@@ -269,6 +269,36 @@ def global_attention_backward(q, k, v, bias, o, lse, do, scale, precision):
     return dq, dk, dvt
 
 
+def global_attention_rowdot(o, do):
+    """D = rowsum(do o): o, do (B, H, nq, dv) fp32 contiguous -> D (B, H, nq), the first stage of the backward"""
+    D = torch.empty(o.shape[:3], dtype=torch.float32, device=o.device)
+    _lib.call("b200sht_attention_global_rowdot", _ptr(o), _ptr(do), _ptr(D), D.numel(), o.shape[3], _stream(o.device))
+    return D
+
+
+def global_attention_backward_kv(q, k, v, bias, lse, D, do, scale, precision):
+    """dk, dv of the given keys against the given queries: q, do (B, H, nq, .), lse, D (B, H, nq) of the queries; k (B, H, nk, dqk),
+    v (B, H, dv, nk), bias (nk,) of the keys; fp32 contiguous -> dk, dv (shapes of k, v)"""
+    B, H, nq, dqk = q.shape
+    dv, nk = v.shape[2], v.shape[3]
+    dk, dvt = torch.empty_like(k), torch.empty_like(v)
+    ws = _global_workspace(B * H, nq, nk, dqk, dv, precision, True, q.device)
+    _lib.call("b200sht_attention_global_backward_kv", _ptr(q), _ptr(k), _ptr(v), _ptr(bias), _ptr(lse), _ptr(D), _ptr(do), _ptr(dk), _ptr(dvt),
+              B * H, nq, nk, dqk, dv, float(scale), precision, _ptr(ws), _stream(q.device))
+    return dk, dvt
+
+
+def global_attention_backward_q(q, k, v, bias, lse, D, do, scale, precision):
+    """dq of the given queries against the given keys (operands as global_attention_backward_kv) -> dq (shape of q)"""
+    B, H, nq, dqk = q.shape
+    dv, nk = v.shape[2], v.shape[3]
+    dq = torch.empty_like(q)
+    ws = _global_workspace(B * H, nq, nk, dqk, dv, precision, True, q.device)
+    _lib.call("b200sht_attention_global_backward_q", _ptr(q), _ptr(k), _ptr(v), _ptr(bias), _ptr(lse), _ptr(D), _ptr(do), _ptr(dq),
+              B * H, nq, nk, dqk, dv, float(scale), precision, _ptr(ws), _stream(q.device))
+    return dq
+
+
 class _GlobalAttention(torch.autograd.Function):
     """o = softmax(scale q k^T + bias) v per head.  Saves q, k, v, o and lse."""
 

@@ -539,21 +539,95 @@ int ag_check(int BH, int nq, int nk, int dqk, int dv) {
   return 0;
 }
 
+// offsets (floats) of the backward's operands in the layouts its GEMMs read, and of D; the workspace query counts the same layout, so one
+// backward workspace serves the full backward and either pass
+struct AgBwdWs {
+  size_t Q[2] = {}, Qt[2] = {}, K[2] = {}, Kt[2] = {}, Vn[2] = {}, dO[2] = {}, dOt[2] = {}, D = 0, total = 0;
+};
+
+AgBwdWs ag_bwd_ws(int BH, int nq, int nk, int dqk, int dv, int planes) {
+  const size_t ldq = round_up(nq, 4), ldk = round_up(nk, 4);
+  AgWs w;
+  AgBwdWs l;
+  for (int pl = 0; pl < planes; ++pl) {
+    l.Q[pl] = w.take((size_t)BH * nq * dqk);
+    l.Qt[pl] = w.take((size_t)BH * dqk * ldq);
+    l.K[pl] = w.take((size_t)BH * nk * dqk);
+    l.Kt[pl] = w.take((size_t)BH * dqk * ldk);
+    l.Vn[pl] = w.take((size_t)BH * nk * dv);
+    l.dO[pl] = w.take((size_t)BH * nq * dv);
+    l.dOt[pl] = w.take((size_t)BH * dv * ldq);
+  }
+  l.D = w.take((size_t)BH * nq);
+  l.total = w.off;
+  return l;
+}
+
+enum { kAgPassKv = 1, kAgPassQ = 2 };
+
+// the passes of the backward named in `passes`, given D: prepares each operand layout they read once, then dK / dV per key block (kv pass)
+// and dQ per query block (q pass).  The full backward runs both on the same layouts; either pass alone reads only its own operands.
+int ag_backward_passes(int passes, const float* q, const float* k, const float* v, const float* bias, const float* lse, const float* D,
+                       const float* dout, float* dq, float* dk, float* dv_, int BH, int nq, int nk, int dqk, int dv, float scale, int split,
+                       float* ws, cudaStream_t st) {
+  const bool kv = passes & kAgPassKv, qp = passes & kAgPassQ;
+  const int dc = ceil_div(std::max(dqk, dv), 32), ldq = round_up(nq, 4), ldk = round_up(nk, 4), planes = split ? 2 : 1;
+  const AgBwdWs l = ag_bwd_ws(BH, nq, nk, dqk, dv, planes);
+  float *Q[2] = {}, *Qt[2] = {}, *K[2] = {}, *Kt[2] = {}, *Vn[2] = {}, *dO[2] = {}, *dOt[2] = {};
+  for (int pl = 0; pl < planes; ++pl) {
+    Q[pl] = ws + l.Q[pl]; Qt[pl] = ws + l.Qt[pl]; K[pl] = ws + l.K[pl]; Kt[pl] = ws + l.Kt[pl];
+    Vn[pl] = ws + l.Vn[pl]; dO[pl] = ws + l.dO[pl]; dOt[pl] = ws + l.dOt[pl];
+  }
+  if (int rc = ag_prep(q, BH, nq, dqk, Q[0], Q[1], dqk, false, st)) return rc;
+  if (kv)
+    if (int rc = ag_prep(q, BH, nq, dqk, Qt[0], Qt[1], ldq, true, st)) return rc;
+  if (int rc = ag_prep(k, BH, nk, dqk, K[0], K[1], dqk, false, st)) return rc;
+  if (qp)
+    if (int rc = ag_prep(k, BH, nk, dqk, Kt[0], Kt[1], ldk, true, st)) return rc;
+  if (int rc = ag_prep(v, BH, dv, nk, Vn[0], Vn[1], dv, true, st)) return rc;
+  if (int rc = ag_prep(dout, BH, nq, dv, dO[0], dO[1], dv, false, st)) return rc;
+  if (kv)
+    if (int rc = ag_prep(dout, BH, nq, dv, dOt[0], dOt[1], ldq, true, st)) return rc;
+
+  AgParams p;
+  if (kv) {
+    memset(&p, 0, sizeof(p));
+    for (int pl = 0; pl < planes; ++pl) {   // dK / dV: resident K, V (key rows); per query block (Q, dO) rows, then (Q^T, dO^T) columns
+      if (int rc = ag_map_rows(&p.res[pl][0], K[pl], BH, nk, dqk, kAgBM)) return rc;
+      if (int rc = ag_map_rows(&p.res[pl][1], Vn[pl], BH, nk, dv, kAgBM)) return rc;
+      if (int rc = ag_map_rows(&p.item[pl][0][0], Q[pl], BH, nq, dqk, kAgBN)) return rc;
+      if (int rc = ag_map_rows(&p.item[pl][0][1], dO[pl], BH, nq, dv, kAgBN)) return rc;
+      if (int rc = ag_map_cols(&p.item[pl][1][0], Qt[pl], BH, nq, dqk, ldq, dc)) return rc;
+      if (int rc = ag_map_cols(&p.item[pl][1][1], dOt[pl], BH, nq, dv, ldq, dc)) return rc;
+    }
+    p.bias = bias; p.lse = lse; p.D = D; p.out0 = dk; p.out1 = dv_;
+    p.nq = nq; p.nk = nk; p.dqk = dqk; p.dv = dv; p.scale = scale;
+    if (int rc = ag_launch(kAgDkv, p, dc, split != 0, ceil_div(nk, kAgBM), BH, st)) return rc;
+  }
+  if (qp) {
+    memset(&p, 0, sizeof(p));
+    for (int pl = 0; pl < planes; ++pl) {   // dQ: resident Q, dO (query rows); per key block (K, V) rows, then K^T columns
+      if (int rc = ag_map_rows(&p.res[pl][0], Q[pl], BH, nq, dqk, kAgBM)) return rc;
+      if (int rc = ag_map_rows(&p.res[pl][1], dO[pl], BH, nq, dv, kAgBM)) return rc;
+      if (int rc = ag_map_rows(&p.item[pl][0][0], K[pl], BH, nk, dqk, kAgBN)) return rc;
+      if (int rc = ag_map_rows(&p.item[pl][0][1], Vn[pl], BH, nk, dv, kAgBN)) return rc;
+      if (int rc = ag_map_cols(&p.item[pl][1][0], Kt[pl], BH, nk, dqk, ldk, dc)) return rc;
+    }
+    p.bias = bias; p.lse = lse; p.D = D; p.out0 = dq;
+    p.nq = nq; p.nk = nk; p.dqk = dqk; p.dv = dv; p.scale = scale;
+    if (int rc = ag_launch(kAgDq, p, dc, split != 0, ceil_div(nq, kAgBM), BH, st)) return rc;
+  }
+  return 0;
+}
+
 }  // namespace
 
 long long attention_global_workspace_floats(int BH, int nq, int nk, int dqk, int dv, int split, int backward) {
   if (ag_check(BH, nq, nk, dqk, dv)) return -1;
-  const size_t planes = split ? 2 : 1, ldq = round_up(nq, 4), ldk = round_up(nk, 4);
+  const size_t planes = split ? 2 : 1, ldk = round_up(nk, 4);
+  if (backward) return (long long)ag_bwd_ws(BH, nq, nk, dqk, dv, (int)planes).total;
   AgWs w;
-  if (!backward) {
-    for (size_t pl = 0; pl < planes; ++pl) { w.take((size_t)BH * nq * dqk); w.take((size_t)BH * nk * dqk); w.take((size_t)BH * dv * ldk); }
-  } else {
-    for (size_t pl = 0; pl < planes; ++pl) {
-      w.take((size_t)BH * nq * dqk); w.take((size_t)BH * dqk * ldq); w.take((size_t)BH * nk * dqk); w.take((size_t)BH * dqk * ldk);
-      w.take((size_t)BH * nk * dv); w.take((size_t)BH * nq * dv); w.take((size_t)BH * dv * ldq);
-    }
-    w.take((size_t)BH * nq);
-  }
+  for (size_t pl = 0; pl < planes; ++pl) { w.take((size_t)BH * nq * dqk); w.take((size_t)BH * nk * dqk); w.take((size_t)BH * dv * ldk); }
   return (long long)w.off;
 }
 
@@ -584,60 +658,39 @@ int attention_global_forward(const float* q, const float* k, const float* v, con
   return ag_launch(kAgFwd, p, dc, split != 0, ceil_div(nq, kAgBM), BH, st);
 }
 
+int attention_global_rowdot(const float* o, const float* dout, float* D, long long rows, int dv, cudaStream_t st) {
+  B200_REQUIRE(rows >= 1 && dv >= 1, "attention_global_rowdot: rows %lld and dv %d must be positive", rows, dv);
+  B200_REQUIRE(o && dout && D, "attention_global_rowdot: null pointer");
+  attention_global_rowdot_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, st>>>(o, dout, D, rows, dv);
+  B200_CHECK_LAUNCH();
+  return 0;
+}
+
+int attention_global_backward_kv(const float* q, const float* k, const float* v, const float* bias, const float* lse, const float* D,
+                                 const float* dout, float* dk, float* dv_, int BH, int nq, int nk, int dqk, int dv, float scale, int split,
+                                 float* ws, cudaStream_t st) {
+  if (int rc = ag_check(BH, nq, nk, dqk, dv)) return rc;
+  B200_REQUIRE(q && k && v && bias && lse && D && dout && dk && dv_ && ws, "attention_global_backward_kv: null pointer");
+  return ag_backward_passes(kAgPassKv, q, k, v, bias, lse, D, dout, nullptr, dk, dv_, BH, nq, nk, dqk, dv, scale, split, ws, st);
+}
+
+int attention_global_backward_q(const float* q, const float* k, const float* v, const float* bias, const float* lse, const float* D,
+                                const float* dout, float* dq, int BH, int nq, int nk, int dqk, int dv, float scale, int split, float* ws,
+                                cudaStream_t st) {
+  if (int rc = ag_check(BH, nq, nk, dqk, dv)) return rc;
+  B200_REQUIRE(q && k && v && bias && lse && D && dout && dq && ws, "attention_global_backward_q: null pointer");
+  return ag_backward_passes(kAgPassQ, q, k, v, bias, lse, D, dout, dq, nullptr, nullptr, BH, nq, nk, dqk, dv, scale, split, ws, st);
+}
+
+// rowdot, then the kv and q passes on one set of prepared operands; D lives in the workspace
 int attention_global_backward(const float* q, const float* k, const float* v, const float* bias, const float* o, const float* lse, const float* dout,
                               float* dq, float* dk, float* dv_, int BH, int nq, int nk, int dqk, int dv, float scale, int split, float* ws,
                               cudaStream_t st) {
   if (int rc = ag_check(BH, nq, nk, dqk, dv)) return rc;
   B200_REQUIRE(q && k && v && bias && o && lse && dout && dq && dk && dv_ && ws, "attention_global_backward: null pointer");
-  const int dc = ceil_div(std::max(dqk, dv), 32), ldq = round_up(nq, 4), ldk = round_up(nk, 4), planes = split ? 2 : 1;
-  AgWs w;
-  float *Q[2] = {}, *Qt[2] = {}, *K[2] = {}, *Kt[2] = {}, *Vn[2] = {}, *dO[2] = {}, *dOt[2] = {};
-  for (int pl = 0; pl < planes; ++pl) {
-    Q[pl] = ws + w.take((size_t)BH * nq * dqk);
-    Qt[pl] = ws + w.take((size_t)BH * dqk * ldq);
-    K[pl] = ws + w.take((size_t)BH * nk * dqk);
-    Kt[pl] = ws + w.take((size_t)BH * dqk * ldk);
-    Vn[pl] = ws + w.take((size_t)BH * nk * dv);
-    dO[pl] = ws + w.take((size_t)BH * nq * dv);
-    dOt[pl] = ws + w.take((size_t)BH * dv * ldq);
-  }
-  float* D = ws + w.take((size_t)BH * nq);
-  const long long rows = (long long)BH * nq;
-  attention_global_rowdot_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, st>>>(o, dout, D, rows, dv);
-  B200_CHECK_LAUNCH();
-  if (int rc = ag_prep(q, BH, nq, dqk, Q[0], Q[1], dqk, false, st)) return rc;
-  if (int rc = ag_prep(q, BH, nq, dqk, Qt[0], Qt[1], ldq, true, st)) return rc;
-  if (int rc = ag_prep(k, BH, nk, dqk, K[0], K[1], dqk, false, st)) return rc;
-  if (int rc = ag_prep(k, BH, nk, dqk, Kt[0], Kt[1], ldk, true, st)) return rc;
-  if (int rc = ag_prep(v, BH, dv, nk, Vn[0], Vn[1], dv, true, st)) return rc;
-  if (int rc = ag_prep(dout, BH, nq, dv, dO[0], dO[1], dv, false, st)) return rc;
-  if (int rc = ag_prep(dout, BH, nq, dv, dOt[0], dOt[1], ldq, true, st)) return rc;
-
-  AgParams p;
-  memset(&p, 0, sizeof(p));
-  for (int pl = 0; pl < planes; ++pl) {   // dK / dV: resident K, V (key rows); per query block (Q, dO) rows, then (Q^T, dO^T) columns
-    if (int rc = ag_map_rows(&p.res[pl][0], K[pl], BH, nk, dqk, kAgBM)) return rc;
-    if (int rc = ag_map_rows(&p.res[pl][1], Vn[pl], BH, nk, dv, kAgBM)) return rc;
-    if (int rc = ag_map_rows(&p.item[pl][0][0], Q[pl], BH, nq, dqk, kAgBN)) return rc;
-    if (int rc = ag_map_rows(&p.item[pl][0][1], dO[pl], BH, nq, dv, kAgBN)) return rc;
-    if (int rc = ag_map_cols(&p.item[pl][1][0], Qt[pl], BH, nq, dqk, ldq, dc)) return rc;
-    if (int rc = ag_map_cols(&p.item[pl][1][1], dOt[pl], BH, nq, dv, ldq, dc)) return rc;
-  }
-  p.bias = bias; p.lse = lse; p.D = D; p.out0 = dk; p.out1 = dv_;
-  p.nq = nq; p.nk = nk; p.dqk = dqk; p.dv = dv; p.scale = scale;
-  if (int rc = ag_launch(kAgDkv, p, dc, split != 0, ceil_div(nk, kAgBM), BH, st)) return rc;
-
-  memset(&p, 0, sizeof(p));
-  for (int pl = 0; pl < planes; ++pl) {   // dQ: resident Q, dO (query rows); per key block (K, V) rows, then K^T columns
-    if (int rc = ag_map_rows(&p.res[pl][0], Q[pl], BH, nq, dqk, kAgBM)) return rc;
-    if (int rc = ag_map_rows(&p.res[pl][1], dO[pl], BH, nq, dv, kAgBM)) return rc;
-    if (int rc = ag_map_rows(&p.item[pl][0][0], K[pl], BH, nk, dqk, kAgBN)) return rc;
-    if (int rc = ag_map_rows(&p.item[pl][0][1], Vn[pl], BH, nk, dv, kAgBN)) return rc;
-    if (int rc = ag_map_cols(&p.item[pl][1][0], Kt[pl], BH, nk, dqk, ldk, dc)) return rc;
-  }
-  p.bias = bias; p.lse = lse; p.D = D; p.out0 = dq;
-  p.nq = nq; p.nk = nk; p.dqk = dqk; p.dv = dv; p.scale = scale;
-  return ag_launch(kAgDq, p, dc, split != 0, ceil_div(nq, kAgBM), BH, st);
+  float* D = ws + ag_bwd_ws(BH, nq, nk, dqk, dv, split ? 2 : 1).D;
+  if (int rc = attention_global_rowdot(o, dout, D, (long long)BH * nq, dv, st)) return rc;
+  return ag_backward_passes(kAgPassKv | kAgPassQ, q, k, v, bias, lse, D, dout, dq, dk, dv_, BH, nq, nk, dqk, dv, scale, split, ws, st);
 }
 
 }  // namespace b200sht

@@ -101,6 +101,13 @@ int attention_global_forward(const float* q, const float* k, const float* v, con
 int attention_global_backward(const float* q, const float* k, const float* v, const float* bias, const float* o, const float* lse, const float* dout,
                               float* dq, float* dk, float* dv_, int BH, int nq, int nk, int dqk, int dv, float scale, int split, float* ws,
                               cudaStream_t st);
+int attention_global_rowdot(const float* o, const float* dout, float* D, long long rows, int dv, cudaStream_t st);
+int attention_global_backward_kv(const float* q, const float* k, const float* v, const float* bias, const float* lse, const float* D,
+                                 const float* dout, float* dk, float* dv_, int BH, int nq, int nk, int dqk, int dv, float scale, int split,
+                                 float* ws, cudaStream_t st);
+int attention_global_backward_q(const float* q, const float* k, const float* v, const float* bias, const float* lse, const float* D,
+                                const float* dout, float* dq, int BH, int nq, int nk, int dqk, int dv, float scale, int split, float* ws,
+                                cudaStream_t st);
 int resample_plan_create(b200sht_resample_plan** out, int nlat_in, int nlon_in, int nlat_out, int nlon_out, int expand_poles, const int* lat_idx,
                          const float* lat_w, const int* lon_left, const int* lon_right, const float* lon_w, cudaStream_t st);
 int resample_plan_destroy(b200sht_resample_plan* pl);
@@ -962,6 +969,28 @@ int b200sht_attention_global_backward(const float* q, const float* k, const floa
   if (split < 0) { set_error("attention_global: precision %d (TF32 or FP32X3 are served)", precision); return B200SHT_ERR_UNSUPPORTED; }
   return attention_global_backward(q, k, v, bias, o, lse, dout, dq, dk, dv, BH, nq, nk, dqk, dvh, scale, split, static_cast<float*>(workspace),
                                    S(stream));
+}
+
+int b200sht_attention_global_rowdot(const float* o, const float* dout, float* D, int64_t rows, int dv, void* stream) {
+  return attention_global_rowdot(o, dout, D, rows, dv, S(stream));
+}
+
+int b200sht_attention_global_backward_kv(const float* q, const float* k, const float* v, const float* bias, const float* lse, const float* D,
+                                         const float* dout, float* dk, float* dv, int BH, int nq, int nk, int dqk, int dvh, float scale,
+                                         int precision, void* workspace, void* stream) {
+  const int split = attention_global_split(precision);
+  if (split < 0) { set_error("attention_global: precision %d (TF32 or FP32X3 are served)", precision); return B200SHT_ERR_UNSUPPORTED; }
+  return attention_global_backward_kv(q, k, v, bias, lse, D, dout, dk, dv, BH, nq, nk, dqk, dvh, scale, split, static_cast<float*>(workspace),
+                                      S(stream));
+}
+
+int b200sht_attention_global_backward_q(const float* q, const float* k, const float* v, const float* bias, const float* lse, const float* D,
+                                        const float* dout, float* dq, int BH, int nq, int nk, int dqk, int dvh, float scale, int precision,
+                                        void* workspace, void* stream) {
+  const int split = attention_global_split(precision);
+  if (split < 0) { set_error("attention_global: precision %d (TF32 or FP32X3 are served)", precision); return B200SHT_ERR_UNSUPPORTED; }
+  return attention_global_backward_q(q, k, v, bias, lse, D, dout, dq, BH, nq, nk, dqk, dvh, scale, split, static_cast<float*>(workspace),
+                                     S(stream));
 }
 
 // ---- bilinear resampling on the sphere (resample.cu)

@@ -18,7 +18,9 @@ channels, the longitude stages see the 2C component rows and the Legendre stage 
 DistributedDiscreteContinuousConvS2 (distributed/disco.py: a latitude halo and window plans of psi_hat) and DistributedResampleS2
 (distributed/resample.py: whole spheres of a subset of planes) are FCN3's local operators under the same h x w grid;
 DistributedDiscreteContinuousConvTransposeS2 runs the DISCO stages the other way round, and DistributedNeighborhoodAttentionS2
-(distributed/attention.py) runs the attention kernels on window plans of the neighbourhood, over the same halo.
+(distributed/attention.py) runs the attention kernels on window plans of the neighbourhood, over the same halo.  DistributedAttentionS2
+(distributed/attention.py) is the global attention on the same grid: each rank attends with its own queries to every key, gathered in
+global (lat, lon) order, and its backward splits the kernels' query-side and key-side passes over the ranks' own queries and keys.
 DistributedGeometricInstanceNormS2 and DistributedInstanceNorm2d (distributed/norm.py) gather per-rank statistics between the staged norm kernels.
 """
 import ctypes
@@ -492,5 +494,5 @@ class DistributedInverseRealVectorSHT(_DistributedBase):
 
 from .disco import DistributedDiscreteContinuousConvS2, DistributedDiscreteContinuousConvTransposeS2, set_disco_local_ops  # noqa: E402,F401
 from .resample import DistributedResampleS2, set_resample_local_ops  # noqa: E402,F401
-from .attention import DistributedNeighborhoodAttentionS2, set_attention_local_ops  # noqa: E402,F401
+from .attention import DistributedAttentionS2, DistributedNeighborhoodAttentionS2, set_attention_local_ops, set_global_attention_local_ops  # noqa: E402,F401,E501
 from .norm import DistributedGeometricInstanceNormS2, DistributedInstanceNorm2d, set_norm_local_ops  # noqa: E402,F401
