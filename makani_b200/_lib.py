@@ -6,7 +6,8 @@ The product path has no CPU or PyTorch fallback: if the library cannot be loaded
 import ctypes
 import os
 import re
-import threading
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # B200SHT_LIBRARY: another build of the same library (e.g. the wait-profile build of scripts/dft_waitprof.py); default: the in-tree one
@@ -177,30 +178,41 @@ def check(rc, what=""):
         raise B200ShtError(f"{what} failed (status {rc}): {msg}")
 
 
-_tls = threading.local()
+def ptr(t):
+    """the `void*` argument of a tensor (None -> NULL)"""
+    return c_void_p(t.data_ptr()) if t is not None else c_void_p(0)
+
+
+def dtype_code(dtype):
+    """the activation dtype code of the C ABI (B200SHT_F32 / B200SHT_BF16)"""
+    if dtype == torch.float32:
+        return F32
+    if dtype == torch.bfloat16:
+        return BF16
+    raise B200ShtError(f"unsupported activation dtype {dtype} (float32 and bfloat16 are supported)")
+
+
+class LaunchStream(c_void_p):
+    """A `void* stream` argument that also names the CUDA device the stream belongs to (`.device`, an index)."""
 
 
 def launch_stream(device):
-    """The stream argument of a library call: torch's current stream of `device`.  Also remembers the device for `call`, which makes it
-    current around the launch when it is not (a tensor on cuda:1 while cuda:0 is current would otherwise launch into the wrong context)."""
-    import torch
-
+    """The stream argument of a library call: torch's current stream of `device`, carrying the device index for `call`."""
     dev = torch.device(device)
-    _tls.device = dev.index if dev.index is not None else torch.cuda.current_device()
-    return c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    stream = LaunchStream(torch.cuda.current_stream(dev).cuda_stream)
+    stream.device = dev.index if dev.index is not None else torch.cuda.current_device()
+    return stream
 
 
 def call(name, *args):
+    """Run entry point `name`; a non-zero status raises B200ShtError.  Every entry point that takes a stream takes it last: when that is a
+    `launch_stream` handle whose device is not the current one, the device is made current around the call, because the library keeps its
+    per-device state (scratch buffers, SM count, tensor-core setup) by the current device.  A plain c_void_p stream is passed as it is."""
     lib = load()
-    dev = getattr(_tls, "device", None)
-    _tls.device = None
-    if dev is not None:
-        import torch
-
-        if dev != torch.cuda.current_device():
-            with torch.cuda.device(dev):
-                rc = getattr(lib, name)(*args)
-            check(rc, name)
-            return
-    rc = getattr(lib, name)(*args)
+    stream = args[-1] if args else None
+    if isinstance(stream, LaunchStream) and stream.device != torch.cuda.current_device():
+        with torch.cuda.device(stream.device):
+            rc = getattr(lib, name)(*args)
+    else:
+        rc = getattr(lib, name)(*args)
     check(rc, name)

@@ -25,10 +25,9 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import B200ShtError
+from ._lib import B200ShtError, launch_stream as _stream, ptr as _ptr
 from .disco import DiscoPlan, DiscoPsi, support_search
 from .quadrature import _grid_np
-from .sht import _ptr, _stream
 
 MAX_HEAD_DIM = 64     # the kernels' largest head dimension (include/b200sht.h)
 

@@ -25,9 +25,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import B200ShtError
+from ._lib import B200ShtError, dtype_code as _dtype_code, launch_stream as _stream, ptr as _ptr
 from .quadrature import _grid_np
-from .sht import _dtype_code, _ptr, _stream
 
 CUTOFF_SLACK = 1e-3      # support r <= (1 + CUTOFF_SLACK) theta_cutoff
 NORM_EPS = 1e-9          # psi_hat = psi q / (d + NORM_EPS)
@@ -182,9 +181,8 @@ class DiscoPlan:
         ker, col = np.ascontiguousarray(psi.ker, np.int32), np.ascontiguousarray(psi.col, np.int32)
         val = np.ascontiguousarray(psi.val, np.float64)
         h = _lib.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.call("b200sht_disco_plan_create", _lib.ctypes.byref(h), self.nlat_in, self.nlon_in, self.nlat_out, self.nlon_out, self.K,
-                      len(val), ker.ctypes.data, lat.ctypes.data, col.ctypes.data, val.ctypes.data, _stream(self.device))
+        _lib.call("b200sht_disco_plan_create", _lib.ctypes.byref(h), self.nlat_in, self.nlon_in, self.nlat_out, self.nlon_out, self.K,
+                  len(val), ker.ctypes.data, lat.ctypes.data, col.ctypes.data, val.ctypes.data, _stream(self.device))
         self.handle, self._lib = h, lib
 
     def query(self, what):

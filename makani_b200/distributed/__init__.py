@@ -23,12 +23,12 @@ DistributedDiscreteContinuousConvTransposeS2 runs the DISCO stages the other way
 global (lat, lon) order, and its backward splits the kernels' query-side and key-side passes over the ranks' own queries and keys.
 DistributedGeometricInstanceNormS2 and DistributedInstanceNorm2d (distributed/norm.py) gather per-rank statistics between the staged norm kernels.
 """
-import ctypes
-
 import torch
 import torch.distributed as dist
 import torch.nn as nn
 
+from .. import _lib
+from .._lib import dtype_code as _dtype_code, launch_stream as _stream, ptr as _ptr
 from . import primitives
 from .primitives import compute_split_shapes, split_tensor_along_dim, _transpose, _gather, _split, _reduce, _DistributedTranspose  # noqa: F401
 
@@ -129,7 +129,6 @@ class CudaLocalOps:
 
     def _vleg_plan(self, device):
         """vector plan (tables D and Q) of this rank's orders m_offset .. m_offset + mmax_local - 1 over all latitudes"""
-        from .. import _lib as L
         from ..sht import Plan, _plan_cache, _plan_lock
         from ..quadrature import _grid_np
         t = self.t
@@ -138,7 +137,7 @@ class CudaLocalOps:
             p = _plan_cache.get(key)
             if p is None:
                 cost, w = _grid_np(t.nlat, t.grid)
-                p = Plan.create_ex(t.nlat, t.nlon, t.lmax, t.mmax_local, t.m_offset, L.PLAN_VECTOR, cost, w, t.csphase, device)
+                p = Plan.create_ex(t.nlat, t.nlon, t.lmax, t.mmax_local, t.m_offset, _lib.PLAN_VECTOR, cost, w, t.csphase, device)
                 _plan_cache[key] = p
             return p
 
@@ -174,91 +173,68 @@ class CudaLocalOps:
         return _LocalIVLegendre.apply(xc.to(torch.complex64).contiguous(), self._vleg_plan(xc.device), self._vprec())
 
 
-def _lib():
-    from .. import _lib as L
-    return L
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
-
-
-def _st(dev):
-    return _lib().launch_stream(dev)
-
-
-def _dt(dtype):
-    from ..sht import _dtype_code
-    return _dtype_code(dtype)
-
-
 class _LocalFFT(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, plan, prec):
-        L = _lib()
         B, C = x.shape[:2]
         lat = torch.empty(plan.latspec_elems(B, C), dtype=torch.float32, device=x.device)
         out = torch.empty(B, C, plan.nlat, plan.mmax, dtype=torch.complex64, device=x.device)
-        L.call("b200sht_fft_analysis", plan.handle, _p(x), _dt(x.dtype), B, C, _p(lat), 0 | (2 if prec == L.PREC_TF32 else 0), _st(x.device))
-        L.call("b200sht_latspec_unpack", plan.handle, _p(lat), _p(out), B, C, _st(x.device))
+        _lib.call("b200sht_fft_analysis", plan.handle, _ptr(x), _dtype_code(x.dtype), B, C, _ptr(lat), 0 | (2 if prec == _lib.PREC_TF32 else 0), _stream(x.device))
+        _lib.call("b200sht_latspec_unpack", plan.handle, _ptr(lat), _ptr(out), B, C, _stream(x.device))
         ctx.plan, ctx.shape, ctx.dtype, ctx.prec = plan, tuple(x.shape), x.dtype, prec
         return out
 
     @staticmethod
     def backward(ctx, g):
-        L = _lib()
         plan = ctx.plan
         B, C = ctx.shape[:2]
         g = g.contiguous()
         lat = torch.empty(plan.latspec_elems(B, C), dtype=torch.float32, device=g.device)
         gx = torch.empty(ctx.shape, dtype=ctx.dtype, device=g.device)
-        L.call("b200sht_latspec_pack", plan.handle, _p(g), _p(lat), B, C, _st(g.device))
-        L.call("b200sht_fft_synthesis", plan.handle, _p(lat), _p(gx), _dt(ctx.dtype), B, C, ctypes.c_void_p(0), 1, _st(g.device))   # standard latspec layout (from the transposes): CUDA-core FFT
+        _lib.call("b200sht_latspec_pack", plan.handle, _ptr(g), _ptr(lat), B, C, _stream(g.device))
+        _lib.call("b200sht_fft_synthesis", plan.handle, _ptr(lat), _ptr(gx), _dtype_code(ctx.dtype), B, C, _ptr(None), 1, _stream(g.device))   # standard latspec layout (from the transposes): CUDA-core FFT
         return gx, None, None
 
 
 class _LocalIFFT(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xc, plan, prec, dtype):
-        L = _lib()
         B, C = xc.shape[:2]
         lat = torch.empty(plan.latspec_elems(B, C), dtype=torch.float32, device=xc.device)
         y = torch.empty(B, C, plan.nlat, plan.nlon, dtype=dtype, device=xc.device)
-        L.call("b200sht_latspec_pack", plan.handle, _p(xc), _p(lat), B, C, _st(xc.device))
-        L.call("b200sht_fft_synthesis", plan.handle, _p(lat), _p(y), _dt(dtype), B, C, ctypes.c_void_p(0), 0, _st(xc.device))
+        _lib.call("b200sht_latspec_pack", plan.handle, _ptr(xc), _ptr(lat), B, C, _stream(xc.device))
+        _lib.call("b200sht_fft_synthesis", plan.handle, _ptr(lat), _ptr(y), _dtype_code(dtype), B, C, _ptr(None), 0, _stream(xc.device))
         ctx.plan, ctx.prec = plan, prec
         return y
 
     @staticmethod
     def backward(ctx, gy):
-        L = _lib()
         plan = ctx.plan
         gy = gy.contiguous()
         B, C = gy.shape[:2]
         lat = torch.empty(plan.latspec_elems(B, C), dtype=torch.float32, device=gy.device)
         g = torch.empty(B, C, plan.nlat, plan.mmax, dtype=torch.complex64, device=gy.device)
-        L.call("b200sht_fft_analysis", plan.handle, _p(gy), _dt(gy.dtype), B, C, _p(lat), 1 | (2 if ctx.prec == L.PREC_TF32 else 0), _st(gy.device))
-        L.call("b200sht_latspec_unpack", plan.handle, _p(lat), _p(g), B, C, _st(gy.device))
+        _lib.call("b200sht_fft_analysis", plan.handle, _ptr(gy), _dtype_code(gy.dtype), B, C, _ptr(lat), 1 | (2 if ctx.prec == _lib.PREC_TF32 else 0), _stream(gy.device))
+        _lib.call("b200sht_latspec_unpack", plan.handle, _ptr(lat), _ptr(g), B, C, _stream(gy.device))
         return g, None, None, None
 
 
 def _legendre_call(plan, prec, xc, direction):
     """direction 0: (B,C,nlat,m) -> (B,C,L,m); 1: (B,C,L,m) -> (B,C,nlat,m)"""
-    L = _lib()
     B, C = xc.shape[:2]
     dev = xc.device
     lat = torch.empty(plan.latspec_elems(B, C), dtype=torch.float32, device=dev)
     spec = torch.empty(plan.spec_elems(B, C), dtype=torch.float32, device=dev)
     if direction == 0:
         out = torch.empty(B, C, plan.lmax, plan.mmax, dtype=torch.complex64, device=dev)
-        L.call("b200sht_latspec_pack", plan.handle, _p(xc), _p(lat), B, C, _st(dev))
-        L.call("b200sht_legendre_analysis", plan.handle, _p(lat), _p(spec), B, C, prec, _st(dev))
-        L.call("b200sht_spec_unpack_ex", plan.lmax, plan.mmax, plan.m_offset, 0, _p(spec), _p(out), B, C, _st(dev))
+        _lib.call("b200sht_latspec_pack", plan.handle, _ptr(xc), _ptr(lat), B, C, _stream(dev))
+        _lib.call("b200sht_legendre_analysis", plan.handle, _ptr(lat), _ptr(spec), B, C, prec, _stream(dev))
+        _lib.call("b200sht_spec_unpack_ex", plan.lmax, plan.mmax, plan.m_offset, 0, _ptr(spec), _ptr(out), B, C, _stream(dev))
     else:
         out = torch.empty(B, C, plan.nlat, plan.mmax, dtype=torch.complex64, device=dev)
-        L.call("b200sht_spec_pack_ex", plan.lmax, plan.mmax, plan.m_offset, 0, _p(xc), _p(spec), B, C, _st(dev))
-        L.call("b200sht_legendre_synthesis", plan.handle, _p(spec), _p(lat), B, C, prec, _st(dev))
-        L.call("b200sht_latspec_unpack", plan.handle, _p(lat), _p(out), B, C, _st(dev))
+        _lib.call("b200sht_spec_pack_ex", plan.lmax, plan.mmax, plan.m_offset, 0, _ptr(xc), _ptr(spec), B, C, _stream(dev))
+        _lib.call("b200sht_legendre_synthesis", plan.handle, _ptr(spec), _ptr(lat), B, C, prec, _stream(dev))
+        _lib.call("b200sht_latspec_unpack", plan.handle, _ptr(lat), _ptr(out), B, C, _stream(dev))
     return out
 
 
@@ -287,21 +263,20 @@ class _LocalILegendre(torch.autograd.Function):
 def _vlegendre_call(plan, prec, xc, direction, scaled):
     """vector plan of an order shard.  direction 0: (B,C,2,nlat,m) -> (B,C,2,L,m), latspec pack -> analysis -> vector_spec_unpack(scaled);
     1: (B,C,2,L,m) -> (B,C,2,nlat,m), vector_spec_pack(scaled) -> synthesis -> latspec unpack.  The C vector fields are 2C component rows."""
-    L = _lib()
     B, C = xc.shape[:2]
     dev = xc.device
     lat = torch.empty(plan.latspec_elems(B, 2 * C), dtype=torch.float32, device=dev)
     spec = torch.empty(plan.spec_elems(B, 2 * C), dtype=torch.float32, device=dev)
     if direction == 0:
         out = torch.empty(B, C, 2, plan.lmax, plan.mmax, dtype=torch.complex64, device=dev)
-        L.call("b200sht_latspec_pack", plan.handle, _p(xc), _p(lat), B, 2 * C, _st(dev))
-        L.call("b200sht_vector_legendre_analysis", plan.handle, _p(lat), _p(spec), B, C, prec, _st(dev))
-        L.call("b200sht_vector_spec_unpack", plan.handle, _p(spec), _p(out), B, C, scaled, _st(dev))
+        _lib.call("b200sht_latspec_pack", plan.handle, _ptr(xc), _ptr(lat), B, 2 * C, _stream(dev))
+        _lib.call("b200sht_vector_legendre_analysis", plan.handle, _ptr(lat), _ptr(spec), B, C, prec, _stream(dev))
+        _lib.call("b200sht_vector_spec_unpack", plan.handle, _ptr(spec), _ptr(out), B, C, scaled, _stream(dev))
     else:
         out = torch.empty(B, C, 2, plan.nlat, plan.mmax, dtype=torch.complex64, device=dev)
-        L.call("b200sht_vector_spec_pack", plan.handle, _p(xc), _p(spec), B, C, scaled, _st(dev))
-        L.call("b200sht_vector_legendre_synthesis", plan.handle, _p(spec), _p(lat), B, C, prec, _st(dev))
-        L.call("b200sht_latspec_unpack", plan.handle, _p(lat), _p(out), B, 2 * C, _st(dev))
+        _lib.call("b200sht_vector_spec_pack", plan.handle, _ptr(xc), _ptr(spec), B, C, scaled, _stream(dev))
+        _lib.call("b200sht_vector_legendre_synthesis", plan.handle, _ptr(spec), _ptr(lat), B, C, prec, _stream(dev))
+        _lib.call("b200sht_latspec_unpack", plan.handle, _ptr(lat), _ptr(out), B, 2 * C, _stream(dev))
     return out
 
 

@@ -9,7 +9,6 @@ of dtype float32 / bfloat16 its forward runs `b200sht_instance_norm_forward` (cs
 kernels do not cover (running statistics, other dtypes) take torch's own operators -- these layers are outside the spherical-harmonic hot path, whose
 no-fallback rule (DESIGN.md section 1) is unchanged.  `B200SHT_FUSED_POINTWISE=0` switches the kernels off.
 """
-import ctypes
 import os
 
 import torch
@@ -17,8 +16,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib
+from ._lib import dtype_code as _dtype_code, ptr as _ptr
 
-_VP = ctypes.c_void_p
 _ENABLED = os.environ.get("B200SHT_FUSED_POINTWISE", "1") != "0"
 
 
@@ -31,14 +30,6 @@ def set_fused_pointwise(on):
 
 def fused_pointwise_enabled():
     return _ENABLED
-
-
-def _ptr(t):
-    return _VP(t.data_ptr()) if t is not None else _VP(0)
-
-
-def _dt(dtype):
-    return _lib.BF16 if dtype == torch.bfloat16 else _lib.F32
 
 
 def _usable(x):
@@ -61,7 +52,7 @@ class _InstanceNormFn(torch.autograd.Function):
         ws = _workspace(B, C, hw, x.device)
         w32 = weight.detach().to(torch.float32).contiguous() if weight is not None else None
         b32 = bias.detach().to(torch.float32).contiguous() if bias is not None else None
-        _lib.call("b200sht_instance_norm_forward", _ptr(x), _ptr(y), _ptr(w32), _ptr(b32), _ptr(stats), _ptr(ws), _dt(x.dtype), B, C, hw, float(eps), int(gelu),
+        _lib.call("b200sht_instance_norm_forward", _ptr(x), _ptr(y), _ptr(w32), _ptr(b32), _ptr(stats), _ptr(ws), _dtype_code(x.dtype), B, C, hw, float(eps), int(gelu),
                   _lib.launch_stream(x.device))
         ctx.save_for_backward(x, w32, b32, stats)
         ctx.gelu, ctx.has_affine = int(gelu), (weight is not None, bias is not None)
@@ -77,7 +68,7 @@ class _InstanceNormFn(torch.autograd.Function):
         dx = torch.empty_like(x)
         sums = torch.empty(B * C, 2, dtype=torch.float32, device=x.device)
         ws = _workspace(B, C, hw, x.device)
-        _lib.call("b200sht_instance_norm_backward", _ptr(x), _ptr(dy), _ptr(dx), _ptr(w32), _ptr(b32), _ptr(stats), _ptr(sums), _ptr(ws), _dt(x.dtype), B, C, hw,
+        _lib.call("b200sht_instance_norm_backward", _ptr(x), _ptr(dy), _ptr(dx), _ptr(w32), _ptr(b32), _ptr(stats), _ptr(sums), _ptr(ws), _dtype_code(x.dtype), B, C, hw,
                   ctx.gelu, _lib.launch_stream(x.device))
         per_c = sums.view(B, C, 2).sum(dim=0)
         dw = per_c[:, 1].to(ctx.param_dtypes[0]) if (ctx.has_affine[0] and ctx.needs_input_grad[1]) else None
@@ -92,7 +83,7 @@ class _BiasGeluFn(torch.autograd.Function):
         B, C, H, W = x.shape
         y = torch.empty_like(x)
         b32 = bias.detach().to(torch.float32).contiguous() if bias is not None else None
-        _lib.call("b200sht_bias_gelu_forward", _ptr(x), _ptr(b32), _ptr(y), _dt(x.dtype), B, C, H * W, _lib.launch_stream(x.device))
+        _lib.call("b200sht_bias_gelu_forward", _ptr(x), _ptr(b32), _ptr(y), _dtype_code(x.dtype), B, C, H * W, _lib.launch_stream(x.device))
         ctx.save_for_backward(x, b32)
         ctx.bias_dtype = bias.dtype if bias is not None else None
         return y
@@ -107,7 +98,7 @@ class _BiasGeluFn(torch.autograd.Function):
         need_b = b32 is not None and ctx.needs_input_grad[1]
         sums = torch.empty(B * C, 2, dtype=torch.float32, device=x.device) if need_b else None
         ws = _workspace(B, C, hw, x.device)
-        _lib.call("b200sht_bias_gelu_backward", _ptr(x), _ptr(b32), _ptr(dy), _ptr(dx), _ptr(sums), _ptr(ws), _dt(x.dtype), B, C, hw, _lib.launch_stream(x.device))
+        _lib.call("b200sht_bias_gelu_backward", _ptr(x), _ptr(b32), _ptr(dy), _ptr(dx), _ptr(sums), _ptr(ws), _dtype_code(x.dtype), B, C, hw, _lib.launch_stream(x.device))
         db = sums.view(B, C, 2)[:, :, 0].sum(dim=0).to(ctx.bias_dtype) if need_b else None
         return dx, db
 
@@ -154,7 +145,7 @@ class CudaGeometricNormStages:
     def partials(self, x, q):
         B, C, H, W = x.shape
         out = torch.empty(B * C, 3, dtype=torch.float64, device=x.device)
-        _lib.call("b200sht_geometric_norm_partials", _ptr(x), _ptr(q), _ptr(out), _ptr(_gw_workspace(B, C, H * W, x.device)), _dt(x.dtype), B, C, H, W,
+        _lib.call("b200sht_geometric_norm_partials", _ptr(x), _ptr(q), _ptr(out), _ptr(_gw_workspace(B, C, H * W, x.device)), _dtype_code(x.dtype), B, C, H, W,
                   _lib.launch_stream(x.device))
         return out
 
@@ -167,7 +158,7 @@ class CudaGeometricNormStages:
     def apply(self, x, w32, b32, stats, gelu):
         B, C, H, W = x.shape
         y = torch.empty_like(x)
-        _lib.call("b200sht_geometric_norm_apply", _ptr(x), _ptr(y), _ptr(w32), _ptr(b32), _ptr(stats), _dt(x.dtype), B, C, H, W, int(gelu),
+        _lib.call("b200sht_geometric_norm_apply", _ptr(x), _ptr(y), _ptr(w32), _ptr(b32), _ptr(stats), _dtype_code(x.dtype), B, C, H, W, int(gelu),
                   _lib.launch_stream(x.device))
         return y
 
@@ -175,14 +166,14 @@ class CudaGeometricNormStages:
         B, C, H, W = x.shape
         sums = torch.empty(B * C, 2, dtype=torch.float64, device=x.device)
         _lib.call("b200sht_geometric_norm_backward_sums", _ptr(x), _ptr(dy), _ptr(w32), _ptr(b32), _ptr(stats), _ptr(sums),
-                  _ptr(_gw_workspace(B, C, H * W, x.device)), _dt(x.dtype), B, C, H, W, int(gelu), _lib.launch_stream(x.device))
+                  _ptr(_gw_workspace(B, C, H * W, x.device)), _dtype_code(x.dtype), B, C, H, W, int(gelu), _lib.launch_stream(x.device))
         return sums
 
     def backward_apply(self, x, dy, w32, b32, stats, sums, q, D, gelu):
         B, C, H, W = x.shape
         dx = torch.empty_like(x)
         _lib.call("b200sht_geometric_norm_backward_apply", _ptr(x), _ptr(dy), _ptr(dx), _ptr(w32), _ptr(b32), _ptr(stats), _ptr(sums.contiguous()),
-                  sums.shape[0], _ptr(q), float(D), _dt(x.dtype), B, C, H, W, int(gelu), _lib.launch_stream(x.device))
+                  sums.shape[0], _ptr(q), float(D), _dtype_code(x.dtype), B, C, H, W, int(gelu), _lib.launch_stream(x.device))
         return dx
 
     def param_grads(self, sums, B, C):
@@ -384,7 +375,7 @@ class _LayerNormFn(torch.autograd.Function):
         stats = torch.empty(B * H * W, 2, dtype=torch.float32, device=x.device)
         w32 = weight.detach().to(torch.float32).contiguous() if weight is not None else None
         b32 = bias.detach().to(torch.float32).contiguous() if bias is not None else None
-        _lib.call("b200sht_layer_norm_forward", _ptr(x), _ptr(y), _ptr(w32), _ptr(b32), _ptr(stats), _dt(x.dtype), _dt(out_dtype), B, C, H * W, float(eps),
+        _lib.call("b200sht_layer_norm_forward", _ptr(x), _ptr(y), _ptr(w32), _ptr(b32), _ptr(stats), _dtype_code(x.dtype), _dtype_code(out_dtype), B, C, H * W, float(eps),
                   int(gelu), _lib.launch_stream(x.device))
         ctx.save_for_backward(x, w32, b32, stats)
         ctx.gelu, ctx.out_dtype = int(gelu), out_dtype
@@ -402,8 +393,8 @@ class _LayerNormFn(torch.autograd.Function):
         dw = torch.empty(C, dtype=torch.float32, device=x.device) if need_w else None
         db = torch.empty(C, dtype=torch.float32, device=x.device) if need_b else None
         ws = torch.empty(max(int(_lib.load().b200sht_layer_norm_workspace_floats(B, C, H * W)), 2), dtype=torch.float32, device=x.device)
-        _lib.call("b200sht_layer_norm_backward", _ptr(x), _ptr(dy), _ptr(dx), _ptr(w32), _ptr(b32), _ptr(stats), _ptr(dw), _ptr(db), _ptr(ws), _dt(x.dtype),
-                  _dt(ctx.out_dtype), B, C, H * W, ctx.gelu, _lib.launch_stream(x.device))
+        _lib.call("b200sht_layer_norm_backward", _ptr(x), _ptr(dy), _ptr(dx), _ptr(w32), _ptr(b32), _ptr(stats), _ptr(dw), _ptr(db), _ptr(ws), _dtype_code(x.dtype),
+                  _dtype_code(ctx.out_dtype), B, C, H * W, ctx.gelu, _lib.launch_stream(x.device))
         dw = dw.to(ctx.param_dtypes[0]) if need_w else None
         db = db.to(ctx.param_dtypes[1]) if need_b else None
         return (dx if ctx.needs_input_grad[0] else None), dw, db, None, None, None

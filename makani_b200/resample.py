@@ -18,9 +18,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import B200ShtError
+from ._lib import B200ShtError, launch_stream as _stream, ptr as _ptr
 from .quadrature import precompute_latitudes, precompute_longitudes
-from .sht import _ptr, _stream
 
 # lat_idx / lat_w (nlat_out): expanded input rows a, a + 1 and weight of output row t; lon_left / lon_right / lon_w (nlon_out)
 ResampleTables = namedtuple("ResampleTables", "lat_idx lat_w lon_left lon_right lon_w expand_poles")
@@ -56,9 +55,8 @@ class ResamplePlan:
         f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)   # noqa: E731
         lat_idx, lat_w, left, right, lon_w = i32(tables.lat_idx), f32(tables.lat_w), i32(tables.lon_left), i32(tables.lon_right), f32(tables.lon_w)
         h = _lib.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.call("b200sht_resample_plan_create", _lib.ctypes.byref(h), nlat_in, nlon_in, nlat_out, nlon_out, int(tables.expand_poles),
-                      lat_idx.ctypes.data, lat_w.ctypes.data, left.ctypes.data, right.ctypes.data, lon_w.ctypes.data, _stream(self.device))
+        _lib.call("b200sht_resample_plan_create", _lib.ctypes.byref(h), nlat_in, nlon_in, nlat_out, nlon_out, int(tables.expand_poles),
+                  lat_idx.ctypes.data, lat_w.ctypes.data, left.ctypes.data, right.ctypes.data, lon_w.ctypes.data, _stream(self.device))
         self.handle, self._lib = h, lib
 
     def query(self, what):

@@ -17,26 +17,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import B200ShtError
+from ._lib import B200ShtError, c_void_p as _VP, dtype_code as _dtype_code, launch_stream as _stream, ptr as _ptr  # scripts import these from here
 from .quadrature import _grid_np
-
-_VP = ctypes.c_void_p
-
-
-def _ptr(t):
-    return _VP(t.data_ptr()) if t is not None else _VP(0)
-
-
-def _stream(device):
-    return _lib.launch_stream(device)
-
-
-def _dtype_code(dt):
-    if dt == torch.float32:
-        return _lib.F32
-    if dt == torch.bfloat16:
-        return _lib.BF16
-    raise B200ShtError(f"unsupported activation dtype {dt} (float32 and bfloat16 are supported)")
 
 
 def resolve_precision(precision="auto"):
@@ -60,24 +42,24 @@ class Plan:
 
     def __init__(self, nlat, nlon, lmax, mmax, grid, csphase, device, vector=False):
         """vector=True: a vector-SHT plan (tables D and Q instead of P) for RealVectorSHT / InverseRealVectorSHT."""
+        cost, w = _grid_np(nlat, grid)
+        self._create(nlat, nlon, lmax, mmax, 0, _lib.PLAN_VECTOR if vector else 0, cost, w, csphase, device)
+
+    @classmethod
+    def create_ex(cls, nlat, nlon, lmax, mmax, m_offset, flags, cost, quad_w, csphase, device):
+        """Sub-plans of the distributed SHT (b200sht_plan_create_ex): order offset and/or FFT-only (flags & 1)."""
+        self = cls.__new__(cls)
+        self._create(nlat, nlon, lmax, mmax, m_offset, flags, cost, quad_w, csphase, device)
+        return self
+
+    def _create(self, nlat, nlon, lmax, mmax, m_offset, flags, cost, quad_w, csphase, device):
         if device.type != "cuda":
             raise B200ShtError("makani_b200 transforms run on CUDA devices only (no CPU fallback)")
-        lib = _lib.load()
-        cost, w = _grid_np(nlat, grid)
         cost = np.ascontiguousarray(cost, dtype=np.float64)
-        w = np.ascontiguousarray(w, dtype=np.float64)
+        quad_w = np.ascontiguousarray(quad_w, dtype=np.float64)
         handle = _VP()
-        with torch.cuda.device(device):
-            if vector:
-                rc = lib.b200sht_plan_create_ex(ctypes.byref(handle), nlat, nlon, lmax, mmax, 0, _lib.PLAN_VECTOR, cost.ctypes.data_as(_VP),
-                                                w.ctypes.data_as(_VP), 1 if csphase else 0, _stream(device))
-            else:
-                rc = lib.b200sht_plan_create(ctypes.byref(handle), nlat, nlon, lmax, mmax, cost.ctypes.data_as(_VP), w.ctypes.data_as(_VP),
-                                             1 if csphase else 0, _stream(device))
-        _lib.check(rc, "b200sht_plan_create")
-        self._finish(handle, device, nlat, nlon, lmax, mmax, 0)
-
-    def _finish(self, handle, device, nlat, nlon, lmax, mmax, m_offset):
+        _lib.call("b200sht_plan_create_ex", ctypes.byref(handle), nlat, nlon, lmax, mmax, m_offset, flags, cost.ctypes.data_as(_VP),
+                  quad_w.ctypes.data_as(_VP), 1 if csphase else 0, _stream(device))
         lib = _lib.load()
         self.handle = handle
         self.device = device
@@ -91,23 +73,6 @@ class Plan:
         """b200sht_plan_query: 0 nlat, 1 nlon, 2 lmax, 3 mmax, 4 kp, 5 table bytes, 6 tensor-core path available, 7 m_offset, 8 tensor-core DFT available,
         9 vector plan."""
         return int(_lib.load().b200sht_plan_query(self.handle, what))
-
-    @classmethod
-    def create_ex(cls, nlat, nlon, lmax, mmax, m_offset, flags, cost, quad_w, csphase, device):
-        """Sub-plans of the distributed SHT (b200sht_plan_create_ex): order offset and/or FFT-only (flags & 1)."""
-        if device.type != "cuda":
-            raise B200ShtError("makani_b200 transforms run on CUDA devices only (no CPU fallback)")
-        lib = _lib.load()
-        cost = np.ascontiguousarray(cost, dtype=np.float64)
-        quad_w = np.ascontiguousarray(quad_w, dtype=np.float64)
-        handle = _VP()
-        with torch.cuda.device(device):
-            rc = lib.b200sht_plan_create_ex(ctypes.byref(handle), nlat, nlon, lmax, mmax, m_offset, flags, cost.ctypes.data_as(_VP),
-                                            quad_w.ctypes.data_as(_VP), 1 if csphase else 0, _stream(device))
-        _lib.check(rc, "b200sht_plan_create_ex")
-        self = cls.__new__(cls)
-        self._finish(handle, device, nlat, nlon, lmax, mmax, m_offset)
-        return self
 
     def latspec_elems(self, B, C):
         return int(_lib.load().b200sht_latspec_elems(self.handle, B, C))

@@ -18,10 +18,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import B200ShtError
-from .sht import RealSHT, InverseRealSHT, _ptr, _stream, resolve_precision, _SpecPack, _SpecUnpack
-
-_VP = ctypes.c_void_p
+from ._lib import B200ShtError, dtype_code as _dtype_code, launch_stream as _stream, ptr as _ptr
+from .sht import RealSHT, InverseRealSHT, resolve_precision, _SpecPack, _SpecUnpack
 
 _DENSE_OPS = (_lib.OP_DHCONV, _lib.OP_SHARED, _lib.OP_LDEP)
 
@@ -148,7 +146,6 @@ class _SpectralConvOneCall(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, bias, mod):
-        from .sht import _dtype_code
         lib = _lib.load()
         dev = x.device
         B = x.shape[0]
@@ -208,7 +205,7 @@ class _SpectralConvOneCall(torch.autograd.Function):
             gw = torch.empty(wshape, dtype=torch.complex64, device=dev) if op in _DENSE_OPS else gw_dev
         ev = ctx.wgrad_event
         _lib.call("b200sht_spectral_conv_backward_ex", pf.handle, pi.handle, dptr, _ptr(gy), _ptr(gres), _ptr(spec_saved), _ptr(wdev), _ptr(gx), _ptr(gw_dev),
-                  _ptr(gb), _ptr(ws), _ptr(gw) if (need_w and op in _DENSE_OPS) else _VP(0), _VP(ev.cuda_event) if ev is not None else _VP(0), _stream(dev))
+                  _ptr(gb), _ptr(ws), _ptr(gw if (need_w and op in _DENSE_OPS) else None), ctypes.c_void_p(ev.cuda_event if ev is not None else 0), _stream(dev))
         gbias = gb.reshape(binfo[0]).to(binfo[1]) if need_b else None
         return gx, gw, gbias, None
 

@@ -13,8 +13,8 @@ D = dP/dtheta and Q = m P / sin(theta) (DESIGN.md section 3).
 import torch
 
 from . import _lib
-from ._lib import B200ShtError
-from .sht import _TransformBase, _dtype_code, _ptr, _stream, get_plan, resolve_precision
+from ._lib import B200ShtError, dtype_code as _dtype_code, launch_stream as _stream, ptr as _ptr
+from .sht import _TransformBase, get_plan, resolve_precision
 
 
 def _vector_precision(precision):
