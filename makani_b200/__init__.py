@@ -16,6 +16,8 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     install_torch_harmonics_shim()             <- makes `import torch_harmonics` resolve to this package
     HostFeed                                   <- double-buffered host->device input staging (the data loader's prefetch queue)
     sfno.SphericalFourierNeuralOperatorNet     <- makani.models.networks.sfnonet (same constructor / parameters / state dict)
+    fcn3.AtmoSphericNeuralOperatorNet          <- makani.models.networks.fourcastnet3 (FourCastNet 3; same constructor / parameters / state dict;
+                                                  also its NeuralOperatorBlock, DiscreteContinuousEncoder / Decoder, LayerScale)
     norm.InstanceNorm2d, norm.bias_gelu        <- torch.nn.InstanceNorm2d (+ GELU), bias + GELU on the library's kernels (row N2)
 """
 from ._lib import B200ShtError, load as load_library  # noqa: F401

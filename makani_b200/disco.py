@@ -273,6 +273,7 @@ class _DiscoConv(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             dX = torch.matmul(Wg.transpose(1, 2), gyg)                                      # (B, G, C_in/G * K, HW)
             dx = plan.adjoint(dX.view(B, C, plan.K, plan.nlat_out, plan.nlon_out), x.dtype)
+            del dX      # X and dX are K times the input each (20 GB apiece for FCN3's decoder): never hold both
         if ctx.needs_input_grad[1]:
             X = plan.forward(x).view(B, G, -1, plan.nlat_out * plan.nlon_out)
             dw = torch.matmul(gyg, X.transpose(2, 3)).sum(0).reshape(weight.shape).to(weight.dtype)
