@@ -245,3 +245,43 @@ def test_every_instantiation_runs_on_wgmma(compiled):
         # k8 steps per streamed block: forward S (4 dc) + PV (4); dK / dV two S-type (8 dc) + two PV-type (8); dQ 8 dc + 4
         per_block = {0: 4 * dc + 4, 1: 8 * dc + 8, 2: 8 * dc + 4}[kind]
         assert hgmma == per_block * (3 if split else 1) and hmma == 0, (name, hgmma, hmma)
+
+
+def _built_instantiations(sass):
+    """{(KIND, DC, SPLIT)} of attention_global_kernel in the SASS function names"""
+    return {(int(k), int(d), s == "1") for k, d, s in re.findall(r"Function : \S*attention_global_kernelILi(\d)ELi(\d)ELb(\d)E", sass)}
+
+
+def test_the_gpu_case_table_runs_every_instantiation(compiled):
+    """each row of the per-element GPU table launches its forward, dK / dV and dQ instantiations at its DC in both precisions (asserted
+    there through the profiler); together they must be every instantiation the compiler built.  Dropping the last row of one DC fails here."""
+    from test_gpu_attention_global import CASES, TF32, X3, case_kernels
+
+    built = _built_instantiations(compiled[0])
+    assert len(built) == 24, sorted(built)
+    covered = {x for c in CASES for prec in (TF32, X3) for x in case_kernels(c, prec)}
+    assert not built - covered, f"built but run by no GPU case: {sorted(built - covered)}"
+    assert not covered - built, f"named by a GPU case but not built: {sorted(covered - built)}"
+
+
+def test_the_gpu_case_table_names_what_the_dispatch_picks_and_reaches_the_edges():
+    """DC is ceil(max(dqk, dv) / 32), as the host code computes it; every DC has a row whose rings wrap three times and more (forward
+    nk >= 400 keys in 32-row blocks through at most 4 slots, dK / dV 2 ceil(nq / 32) >= 14 items, dQ 2 ceil(nk / 32)), with partial last
+    streamed blocks, partial last 64-row resident tiles at grid.x >= 3, BH >= 2 and dqk != dv; and the edges the table is there for"""
+    from test_gpu_attention_global import CASES
+
+    src = open(os.path.join(ROOT, "makani_b200", "csrc", "attention_global.cu")).read()
+    assert len(re.findall(r"dc = ceil_div\(std::max\(dqk, dv\), 32\)", src)) == 2
+    assert re.search(r"constexpr int kAgBM = 64;", src) and re.search(r"constexpr int kAgBN = 32;", src)
+    assert re.search(r"constexpr int kAgMaxStages = 4;", src)
+    for c in CASES:
+        assert c[-1] == -(-max(c[4], c[5]) // 32), c
+    for dc in (1, 2, 3, 4):
+        hard = [c for c in CASES if c[-1] == dc and c[2] >= 200 and c[3] >= 400 and c[2] % 32 and c[3] % 32 and c[2] % 64 and c[3] % 64
+                and -(-c[2] // 64) >= 3 and -(-c[3] // 64) >= 3 and c[0] * c[1] >= 2 and c[4] != c[5]]
+        assert hard, dc
+        assert {c[6] for c in hard} >= {"random", "large", "ascending", "descending"}, dc
+    nqs, nks = {c[2] for c in CASES}, {c[3] for c in CASES}
+    assert 1 in nqs and 1 in nks and {31, 32, 33} <= nks and any(c[2] == 128 and c[3] == 64 for c in CASES)
+    assert {c[7] for c in CASES} == {"none", "first", "last", "one"}
+    assert {(3, 96, 72), (3, 72, 96), (3, 88, 8)} <= {(c[-1], c[4], c[5]) for c in CASES}

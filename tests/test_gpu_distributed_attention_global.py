@@ -3,8 +3,8 @@
 * the separable backward of the C ABI on the full grid: rowdot, the kv pass and the q pass give dq, dk and dv bit for bit equal to
   b200sht_attention_global_backward, in TF32 and 3 x TF32;
 * virtual ranks on one GPU (h x w in {2 x 1, 1 x 2, 2 x 2, 4 x 2}) at 181 x 360 equiangular, 91 x 180 Legendre-Gauss <- 181 x 360
-  equiangular and a small odd grid with dropped keys at d = 8 and d = 128: every rank's o, lse, D, dq (its queries against every key) and
-  dk, dv (its keys against every query), computed by the module's per-rank stage, are torch.equal to the matching slices of the serial
+  equiangular and a small odd grid with dropped keys at d = 8, d = 128 and (dqk, dv) = (96, 72): every rank's o, lse, D, dq (its
+  queries against every key) and dk, dv (its keys against every query),computed by the module's per-rank stage, are torch.equal to the matching slices of the serial
   kernels' outputs on the same operands, in both precisions; two runs are bit-identical, and the per-rank calls launch the same
   attention_global_kernel instantiations as the serial call;
 * the module itself on gloo process groups whose ranks share the GPU: every rank's output and input gradients, and the rank-summed
@@ -56,7 +56,8 @@ def _masked_bias(nk, seed):
 
 
 @pytest.mark.parametrize("prec", PRECS, ids=PREC_IDS)
-@pytest.mark.parametrize("size", [(2, 2, 700, 1100, 64, 64), (1, 3, 130, 97, 8, 128), (1, 1, 1, 5, 40, 8)], ids=lambda s: "x".join(map(str, s)))
+@pytest.mark.parametrize("size", [(2, 2, 700, 1100, 64, 64), (1, 3, 130, 97, 8, 128), (1, 1, 1, 5, 40, 8),
+                                  (2, 1, 150, 301, 88, 72)], ids=lambda s: "x".join(map(str, s)))
 def test_split_backward_equals_the_full_backward(size, prec):
     B, H, nq, nk, dqk, dv = size
     q, k, v, do, bias = _operands(B, H, nq, nk, dqk, dv, _masked_bias(nk, 1), seed=nq + nk)
@@ -95,9 +96,10 @@ def _per_rank(ops, q, k, v, do, bias, lse, D, qi, ki, prec):
 
 
 # (out grid, in grid, B, H, dqk, dv, bias): 181 x 360 equiangular, 91 x 180 Legendre-Gauss <- 181 x 360 equiangular, an odd grid with
-# dropped keys at d = 8 and d = 128
+# dropped keys at d = 8, d = 128 and dqk, dv = 96, 72 (three head-dim chunks)
 GEOMS = [((181, 360), (181, 360), 1, 2, 32, 32, "equiangular"), ((91, 180), (181, 360), 1, 2, 64, 64, "equiangular"),
-         ((13, 27), (15, 29), 2, 2, 8, 8, "masked"), ((13, 27), (15, 29), 1, 2, 128, 128, "masked")]
+         ((13, 27), (15, 29), 2, 2, 8, 8, "masked"), ((13, 27), (15, 29), 1, 2, 128, 128, "masked"),
+         ((13, 27), (15, 29), 2, 1, 96, 72, "masked")]
 GRIDS = [(2, 1), (1, 2), (2, 2), (4, 2)]
 
 
