@@ -483,6 +483,34 @@ int64_t b200sht_resample_plan_query(const b200sht_resample_plan* plan, int what)
 int b200sht_resample_forward(const b200sht_resample_plan* plan, const float* x, float* y, int planes, void* stream);
 int b200sht_resample_adjoint(const b200sht_resample_plan* plan, const float* dy, float* dx, int planes, void* stream);
 
+/* ---------------------------------------------------------------------------------- spherical noise
+ * The state update, the synthesis input and the sigma gradient of makani's IsotropicGaussianRandomFieldS2 and DiffusionNoiseS2
+ * (makani/models/noise.py:376-954; makani_b200/noise.py).  state: fp32 [B][T][C][L][M][2], makani's layout (this rank's L x M shard under
+ * h x w); as a complex tensor it is [B][T*C][L][M].  The standard normal draws xi are supplied by the caller (makani's generator, shapes and
+ * order), so a seed gives makani's noise.
+ *
+ * b200sht_noise_update advances the state in place, r = -1 if `reflect` else +1; one thread owns one (b, c, l, m) column over all T steps:
+ *   B200SHT_NOISE_AR          xi [B][1][C][L][M][2]: state[T-1] <- phi[c] state[T-1] + r sigma[c][l] xi, the older steps move down by one.
+ *                             Separate fp32 multiplies and adds: bit for bit torch's sequence.
+ *   B200SHT_NOISE_STATIONARY  xi like state: w = r sigma[c][l] xi, w[0] /= sqrt(1 - phi[c]^2) (IEEE sqrt and division; bit for bit torch's
+ *                             sequence), then for T > 1 state[t] = sum_{q <= t} discount[c][t][q] w[q] as fp32 FMAs in q order (discount
+ *                             [C][T][T], lower triangular: entries above the diagonal are not read).
+ *   B200SHT_NOISE_BASE        xi like state: state <- r xi (sigma, phi, discount unused; may be null).
+ *   sigma [C][L], phi [C].
+ * b200sht_noise_spectrum writes what the synthesis reads, for TC = T*C channels: z = (state / sqrt 2) sigma[l][m] (an isotropic field's sigma
+ *   [L][M]; state / sqrt 2 as torch computes it on CUDA, a multiply by the fp32 reciprocal, and (a + i b) sigma as torch's complex-by-real
+ *   multiply, (a sigma - b 0) + i (a 0 + b sigma), so zeros carry torch's sign too) or, with sigma null, the state as it is:
+ *   packed = 1  out = packed spec [L][M][2][B][cp] (cp = TC rounded up to 4) of a plan with m_offset 0: the entries b200sht_spec_pack writes
+ *               (l >= lstart(m), zeros in the padding channels), bit for bit makani's torch.complex(...) * sigma_l and the pack;
+ *   packed = 0  out = complex [B][TC][L][M], every entry (the local coefficients of DistributedInverseRealSHT).
+ * b200sht_noise_sigma_grad: dsigma [L][M] = sum_b sum_c Re(conj(g) state / sqrt 2), b outer and c inner, one fp32 FMA chain per (l, m): the
+ *   result is bit-identical run to run.  g = the packed gradient (packed = 1; entries l < m get 0) or complex [B][TC][L][M] (packed = 0). */
+enum { B200SHT_NOISE_AR = 0, B200SHT_NOISE_STATIONARY = 1, B200SHT_NOISE_BASE = 2 };
+int b200sht_noise_update(float* state, const float* xi, const float* sigma, const float* phi, const float* discount, int B, int T, int C, int L, int M,
+                         int mode, int reflect, void* stream);
+int b200sht_noise_spectrum(const float* state, const float* sigma, float* out, int B, int TC, int L, int M, int packed, void* stream);
+int b200sht_noise_sigma_grad(const float* state, const float* grad, float* dsigma, int B, int TC, int L, int M, int packed, void* stream);
+
 /* Programmatic dependent launch between the tensor-core kernels of a call sequence (prologue of kernel i+1 under the tail of kernel i; environment
  * B200SHT_PDL sets the initial value, default on).  Returns the previous setting.  Results do not depend on it. */
 int b200sht_debug_set_pdl(int on);

@@ -18,6 +18,8 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     sfno.SphericalFourierNeuralOperatorNet     <- makani.models.networks.sfnonet (same constructor / parameters / state dict)
     fcn3.AtmoSphericNeuralOperatorNet          <- makani.models.networks.fourcastnet3 (FourCastNet 3; same constructor / parameters / state dict;
                                                   also its NeuralOperatorBlock, DiscreteContinuousEncoder / Decoder, LayerScale)
+    noise.DiffusionNoiseS2, noise.IsotropicGaussianRandomFieldS2, noise.DummyNoiseS2, noise.build_noise
+                                               <- makani.models.noise (FCN3's input noise: the state update and the synthesis input on sm_90a)
     norm.InstanceNorm2d, norm.bias_gelu        <- torch.nn.InstanceNorm2d (+ GELU), bias + GELU on the library's kernels (row N2)
 """
 from ._lib import B200ShtError, load as load_library  # noqa: F401
@@ -29,5 +31,6 @@ from .resample import ResampleS2  # noqa: F401
 from .attention import NeighborhoodAttentionS2, AttentionS2  # noqa: F401
 from .spectral_convolution import SpectralConv, SpectralAttention, ComplexReLU, mix_packed  # noqa: F401
 from .host_pipeline import HostFeed  # noqa: F401
+from . import noise  # noqa: F401
 
 __version__ = "0.1.0"

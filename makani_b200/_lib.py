@@ -17,6 +17,7 @@ HEADER_PATH = os.path.join(_HERE, "..", "include", "b200sht.h")
 F32, BF16 = 0, 1
 PREC_FP32, PREC_TF32, PREC_FP32X3 = 0, 1, 2
 PLAN_FFT_ONLY, PLAN_VECTOR = 1, 2
+NOISE_AR, NOISE_STATIONARY, NOISE_BASE = 0, 1, 2
 OP_DHCONV, OP_DIAGONAL, OP_SEP_DHCONV, OP_SEP_DIAGONAL, OP_SHARED, OP_LDEP = range(6)
 DENSE_FLAG = 0x100
 
@@ -126,6 +127,10 @@ _SIGNATURES = {
     "b200sht_resample_plan_query": (c_int64, [_P, c_int]),
     "b200sht_resample_forward": (c_int, [_P, _P, _P, c_int, _P]),
     "b200sht_resample_adjoint": (c_int, [_P, _P, _P, c_int, _P]),
+    # spherical noise
+    "b200sht_noise_update": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200sht_noise_spectrum": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
+    "b200sht_noise_sigma_grad": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     # debug / CPU-testable entry points (same device code compiled for the host)
     "b200sht_debug_fft_host": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P]),
     "b200sht_debug_dft_host": (c_int, [c_int, c_int, c_int, c_int, c_float, _P, _P]),

@@ -7,7 +7,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200sht.so")
-SOURCES = ["capi.cu", "fft.cu", "legendre.cu", "mix.cu", "act.cu", "umma.cu", "dft.cu", "norm.cu", "disco.cu", "resample.cu", "attention.cu", "attention_global.cu"]
+SOURCES = ["capi.cu", "fft.cu", "legendre.cu", "mix.cu", "act.cu", "umma.cu", "dft.cu", "norm.cu", "disco.cu", "resample.cu", "attention.cu", "attention_global.cu", "noise.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]

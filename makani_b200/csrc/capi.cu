@@ -114,6 +114,10 @@ int resample_plan_destroy(b200sht_resample_plan* pl);
 long long resample_plan_query(const b200sht_resample_plan* pl, int what);
 int resample_forward(const b200sht_resample_plan* pl, const float* x, float* y, int planes, cudaStream_t st);
 int resample_adjoint(const b200sht_resample_plan* pl, const float* dy, float* dx, int planes, cudaStream_t st);
+int noise_update(float* state, const float* xi, const float* sigma, const float* phi, const float* discount, int B, int T, int C, int L, int M,
+                 int mode, int reflect, cudaStream_t st);
+int noise_spectrum(const float* state, const float* sigma, float* out, int B, int TC, int L, int M, int packed, cudaStream_t st);
+int noise_sigma_grad(const float* state, const float* grad, float* dsigma, int B, int TC, int L, int M, int packed, cudaStream_t st);
 
 }  // namespace b200sht
 
@@ -1009,6 +1013,19 @@ int b200sht_resample_forward(const b200sht_resample_plan* plan, const float* x, 
 
 int b200sht_resample_adjoint(const b200sht_resample_plan* plan, const float* dy, float* dx, int planes, void* stream) {
   return resample_adjoint(plan, dy, dx, planes, S(stream));
+}
+
+int b200sht_noise_update(float* state, const float* xi, const float* sigma, const float* phi, const float* discount, int B, int T, int C, int L, int M,
+                         int mode, int reflect, void* stream) {
+  return noise_update(state, xi, sigma, phi, discount, B, T, C, L, M, mode, reflect, S(stream));
+}
+
+int b200sht_noise_spectrum(const float* state, const float* sigma, float* out, int B, int TC, int L, int M, int packed, void* stream) {
+  return noise_spectrum(state, sigma, out, B, TC, L, M, packed, S(stream));
+}
+
+int b200sht_noise_sigma_grad(const float* state, const float* grad, float* dsigma, int B, int TC, int L, int M, int packed, void* stream) {
+  return noise_sigma_grad(state, grad, dsigma, B, TC, L, M, packed, S(stream));
 }
 
 }  // extern "C"
