@@ -17,7 +17,11 @@ Public surface (mirrors the reference, see INTEGRATION.md):
     HostFeed                                   <- double-buffered host->device input staging (the data loader's prefetch queue)
     sfno.SphericalFourierNeuralOperatorNet     <- makani.models.networks.sfnonet (same constructor / parameters / state dict)
     fcn3.AtmoSphericNeuralOperatorNet          <- makani.models.networks.fourcastnet3 (FourCastNet 3; same constructor / parameters / state dict;
-                                                  also its NeuralOperatorBlock, DiscreteContinuousEncoder / Decoder, LayerScale)
+                                                  also its NeuralOperatorBlock, DiscreteContinuousEncoder / Decoder, LayerScale); on
+                                                  a grid set by distributed.init it builds makani's distributed modules and tags
+    distributed.scatter_state_dict, gather_state_dict, sync_shared_params, reduce_shared_gradients
+                                               <- makani.utils.checkpoint_helpers / mpu.helpers / the DDP comm hook of mpu.mappings
+                                                  (global checkpoints and shared-parameter gradients under h x w)
     noise.DiffusionNoiseS2, noise.IsotropicGaussianRandomFieldS2, noise.DummyNoiseS2, noise.build_noise
                                                <- makani.models.noise (FCN3's input noise: the state update and the synthesis input on sm_90a)
     norm.InstanceNorm2d, norm.bias_gelu        <- torch.nn.InstanceNorm2d (+ GELU), bias + GELU on the library's kernels (row N2)

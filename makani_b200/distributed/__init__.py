@@ -22,6 +22,9 @@ DistributedDiscreteContinuousConvTransposeS2 runs the DISCO stages the other way
 (distributed/attention.py) is the global attention on the same grid: each rank attends with its own queries to every key, gathered in
 global (lat, lon) order, and its backward splits the kernels' query-side and key-side passes over the ranks' own queries and keys.
 DistributedGeometricInstanceNormS2 and DistributedInstanceNorm2d (distributed/norm.py) gather per-rank statistics between the staged norm kernels.
+makani_b200.fcn3 builds FourCastNet 3 from these modules when the grid has more than one rank.  scatter_state_dict / gather_state_dict,
+sync_shared_params and reduce_shared_gradients (distributed/helpers.py) load and save global checkpoints, keep replicated parameters in step and
+reduce their gradients, for any model carrying makani's is_shared_mp / sharded_dims_mp tags.
 """
 import torch
 import torch.distributed as dist
@@ -471,3 +474,4 @@ from .disco import DistributedDiscreteContinuousConvS2, DistributedDiscreteConti
 from .resample import DistributedResampleS2, set_resample_local_ops  # noqa: E402,F401
 from .attention import DistributedAttentionS2, DistributedNeighborhoodAttentionS2, set_attention_local_ops, set_global_attention_local_ops  # noqa: E402,F401,E501
 from .norm import DistributedGeometricInstanceNormS2, DistributedInstanceNorm2d, set_norm_local_ops  # noqa: E402,F401
+from .helpers import gather_state_dict, reduce_shared_gradients, scatter_state_dict, sync_shared_params  # noqa: E402,F401

@@ -8,8 +8,17 @@ Restates, with the same constructor arguments, module tree, parameter names, sha
   get_channel_groups, get_water_channels makani/utils/features.py:69-140
   LayerScale                             makani/models/common/layers.py:154-197
 so that a checkpoint of the reference network loads with `load_state_dict(strict=True)` and gives the same outputs (tests/golden/fcn3_golden.npz is
-produced by the REFERENCE class, tests/golden/make_fcn3_golden.py).  Single process (h = w = matmul = 1); FCN3 under h x w spatial model parallelism
-runs through makani's own class and makani_b200.distributed.
+produced by the REFERENCE class, tests/golden/make_fcn3_golden.py).
+
+Under h x w spatial model parallelism (the process grid of makani_b200.distributed.init(polar_group, azimuth_group) has more than one rank, read
+where makani reads comm.get_size("spatial")), the network builds what makani builds there (fourcastnet3.py:63-114, 190, 340-366, 519, 927-936):
+DistributedDiscreteContinuousConvS2 in the encoders, local blocks and decoders, DistributedResampleS2 (or the DistributedRealSHT /
+DistributedInverseRealSHT pair with `upsample_sht`), the distributed SHT pair for the processor, DistributedInstanceNorm2d /
+DistributedGeometricInstanceNormS2, and it tags the convolution weights and biases is_shared_mp = ["spatial"].  Module tree, parameter names and
+state-dict keys stay those of the serial network; inputs and outputs are this rank's (lat, lon) shard of the data grid (`compute_split_shapes`).
+Every other operation (MLPs, layer scale, skips, big skip, water clamp, the scatter of `decode`) acts on local pixels.  Loading a global
+checkpoint, keeping the shared parameters in step and reducing their gradients: makani_b200.distributed.scatter_state_dict, gather_state_dict,
+sync_shared_params and reduce_shared_gradients.  makani's `matmul` feature parallelism (DistributedMLP) is not built.
 
 On the CUDA backend every FLOP-heavy operation runs on this library's sm_90a kernels or a cuBLAS GEMM: the DISCO convolutions (csrc/disco.cu), the
 bilinear resampling (csrc/resample.cu), the SHT pair and the dhconv SpectralConv (tensor-core engine), the 1x1 convolutions as GEMMs on the NCHW tensor
@@ -45,6 +54,53 @@ class _Backend(_SpectralBackend):
         self.InstanceNorm2d = norm.InstanceNorm2d
         self.LayerNorm = norm.DistributedLayerNorm
         self.GeometricInstanceNormS2 = norm.GeometricInstanceNormS2
+
+
+class _DistributedBackend(_Backend):
+    """the classes makani builds at spatial model parallelism > 1, on the process grid of makani_b200.distributed"""
+
+    def __init__(self, precision="auto"):
+        super().__init__(precision)
+        from . import distributed as mbd
+
+        self.RealSHT = partial(mbd.DistributedRealSHT, precision=precision)
+        self.InverseRealSHT = partial(mbd.DistributedInverseRealSHT, precision=precision)
+        self.DiscreteContinuousConvS2 = mbd.DistributedDiscreteContinuousConvS2
+        self.ResampleS2 = mbd.DistributedResampleS2
+        self.InstanceNorm2d = mbd.DistributedInstanceNorm2d
+        self.GeometricInstanceNormS2 = mbd.DistributedGeometricInstanceNormS2
+
+
+def _spatial_size():
+    """makani's comm.get_size("spatial"): the ranks of the h x w grid set by makani_b200.distributed.init (1 without one)"""
+    from . import distributed as mbd
+
+    return mbd.polar_group_size() * mbd.azimuth_group_size()
+
+
+def _default_backend(precision="auto"):
+    return _DistributedBackend(precision) if _spatial_size() > 1 else _Backend(precision)
+
+
+def _tag_spatial_conv(conv):
+    """makani's tags of a DISCO convolution under spatial model parallelism: weight and bias replicated on every spatial rank"""
+    if _spatial_size() > 1:
+        conv.weight.is_shared_mp = ["spatial"]
+        conv.weight.sharded_dims_mp = [None, None, None]
+        if conv.bias is not None:
+            conv.bias.is_shared_mp = ["spatial"]
+            conv.bias.sharded_dims_mp = [None]
+
+
+def _refuse_oversplit(lat_sizes, lon_sizes):
+    """each latitude-like size split over the polar group and each longitude-like size over the azimuth group must leave every rank at least
+    one point; a module would otherwise fail deep inside its forward"""
+    from . import distributed as mbd
+
+    for sizes, n_ranks, what in ((lat_sizes, mbd.polar_group_size(), "polar (h)"), (lon_sizes, mbd.azimuth_group_size(), "azimuth (w)")):
+        for name, n in sizes.items():
+            if n_ranks > 1 and min(mbd.compute_split_shapes(n, n_ranks)) < 1:
+                raise ValueError(f"{name} = {n} cannot be split over the {n_ranks} ranks of the {what} group: every rank needs at least one point")
 
 
 def _compute_cutoff_radius(nlat, kernel_shape, basis_type):
@@ -107,10 +163,12 @@ class LayerScale(nn.Module):
 def _get_norm_layer_handle(h, w, embed_dim, normalization_layer="none", sht_grid_type="legendre-gauss", backend=None):
     """the norm constructor of fourcastnet3.py:63-114 on the backend's classes.  "instance_norm_s2": makani's handle also passes `pole_mask=0`, which
     its GeometricInstanceNormS2 does not take (so makani's class cannot be built with this setting); pole_mask 0 masks nothing and is not passed."""
-    backend = backend or _Backend()
+    backend = backend or _default_backend()
     if normalization_layer == "layer_norm":
         return partial(backend.LayerNorm, normalized_shape=(embed_dim), elementwise_affine=True, eps=1e-6)
     if normalization_layer == "instance_norm":
+        if _spatial_size() > 1:         # makani's DistributedInstanceNorm2d keeps no running statistics to switch off
+            return partial(backend.InstanceNorm2d, num_features=embed_dim, eps=1e-6, affine=True)
         return partial(backend.InstanceNorm2d, num_features=embed_dim, eps=1e-6, affine=True, track_running_stats=False)
     if normalization_layer == "instance_norm_s2":
         return partial(backend.GeometricInstanceNormS2, img_shape=(h, w), crop_shape=(h, w), crop_offset=(0, 0), grid_type=sht_grid_type,
@@ -127,11 +185,12 @@ class DiscreteContinuousEncoder(nn.Module):
                  kernel_shape=(3, 3), basis_type="harmonic", basis_norm_mode="mean", use_mlp=False, mlp_ratio=2.0, activation_function=nn.GELU, groups=1,
                  bias=False, backend=None):
         super().__init__()
-        backend = backend or _Backend()
+        backend = backend or _default_backend()
         theta_cutoff = _compute_cutoff_radius(nlat=inp_shape[0], kernel_shape=kernel_shape, basis_type=basis_type)
         self.conv = backend.DiscreteContinuousConvS2(inp_chans, out_chans, in_shape=inp_shape, out_shape=out_shape, kernel_shape=kernel_shape,
                                                      basis_type=basis_type, basis_norm_mode=basis_norm_mode, grid_in=grid_in, grid_out=grid_out,
                                                      groups=groups, bias=bias, theta_cutoff=theta_cutoff)
+        _tag_spatial_conv(self.conv)
         if use_mlp:
             with torch.no_grad():
                 self.conv.weight *= math.sqrt(2.0)
@@ -156,7 +215,7 @@ class DiscreteContinuousDecoder(nn.Module):
                  kernel_shape=(3, 3), basis_type="harmonic", basis_norm_mode="mean", use_mlp=False, mlp_ratio=2.0, activation_function=nn.GELU, groups=1,
                  bias=False, upsample_sht=False, backend=None):
         super().__init__()
-        backend = backend or _Backend()
+        backend = backend or _default_backend()
         if use_mlp:
             self.mlp = EncoderDecoder(num_layers=1, input_dim=inp_chans, output_dim=inp_chans, hidden_dim=int(mlp_ratio * inp_chans),
                                       act_layer=activation_function, input_format="nchw", gain=2.0)
@@ -171,6 +230,7 @@ class DiscreteContinuousDecoder(nn.Module):
         self.conv = backend.DiscreteContinuousConvS2(inp_chans, out_chans, in_shape=out_shape, out_shape=out_shape, kernel_shape=kernel_shape,
                                                      basis_type=basis_type, basis_norm_mode=basis_norm_mode, grid_in=grid_out, grid_out=grid_out,
                                                      groups=groups, bias=False, theta_cutoff=theta_cutoff)
+        _tag_spatial_conv(self.conv)
 
     def forward(self, x):
         dtype = x.dtype
@@ -190,7 +250,7 @@ class NeuralOperatorBlock(nn.Module):
                  path_drop_rate=0.0, act_layer=nn.GELU, normalization_layer="none", num_groups=1, skip="identity", layer_scale=True, use_mlp=False,
                  kernel_shape=(3, 3), basis_type="harmonic", basis_norm_mode="mean", checkpointing_level=0, bias=False, backend=None):
         super().__init__()
-        backend = backend or _Backend()
+        backend = backend or _default_backend()
         self.inp_shape = (forward_transform.nlat, forward_transform.nlon)
         self.out_shape = (inverse_transform.nlat, inverse_transform.nlon)
         self.out_chans = out_chans
@@ -200,6 +260,7 @@ class NeuralOperatorBlock(nn.Module):
                                                                kernel_shape=kernel_shape, basis_type=basis_type, basis_norm_mode=basis_norm_mode,
                                                                groups=num_groups, grid_in=forward_transform.grid, grid_out=inverse_transform.grid,
                                                                bias=False, theta_cutoff=theta_cutoff)
+            _tag_spatial_conv(self.local_conv)
         elif conv_type == "global":
             self.global_conv = backend.SpectralConv(forward_transform, inverse_transform, inp_chans, inp_chans, operator_type="dhconv",
                                                     num_groups=num_groups, bias=bias, gain=1.0)
@@ -260,13 +321,18 @@ class AtmoSphericNeuralOperatorNet(nn.Module):
                  clamp_water=False, bias=False, checkpointing_level=0, freeze_encoder=False, freeze_processor=False, precision="auto", backend=None,
                  **kwargs):
         super().__init__()
-        backend = backend or _Backend(precision)
+        backend = backend or _default_backend(precision)
         self.inp_shape, self.out_shape = inp_shape, out_shape
         self.atmo_embed_dim, self.surf_embed_dim, self.aux_embed_dim = atmo_embed_dim, surf_embed_dim, aux_embed_dim
         self.big_skip, self.checkpointing_level = big_skip, checkpointing_level
         if n_history != 0:
             raise ValueError(f"this model currently does not support history, expected n_history == 0 but got {n_history}")
         self.h, self.w = int(self.inp_shape[0] // scale_factor), int(self.inp_shape[1] // scale_factor)
+        if _spatial_size() > 1:
+            modes_lat, modes_lon = self._modes(hard_thresholding_fraction, max_modes)
+            _refuse_oversplit({"inp_shape[0]": inp_shape[0], "out_shape[0]": out_shape[0], "model grid h": self.h, "modes_lat": modes_lat},
+                              {"inp_shape[1]": inp_shape[1], "out_shape[1]": out_shape[1], "model grid w": self.w, "modes_lon": modes_lon,
+                               "decoder SHT modes w // 2 + 1": self.w // 2 + 1})
         self._init_spectral_transforms(backend, sht_grid_type, hard_thresholding_fraction, max_modes)
         self._precompute_channel_groups(channel_names, aux_channel_names)
         self.n_out_chans = self.n_atmo_groups * self.n_atmo_chans + self.n_surf_chans
@@ -331,14 +397,16 @@ class AtmoSphericNeuralOperatorNet(nn.Module):
                 p.requires_grad = False
 
     def _init_spectral_transforms(self, backend, sht_grid_type, hard_thresholding_fraction, max_modes):
-        """the processor's SHT pair on the (h, w) grid; modes = max_modes, else int(h * frac), int((w // 2 + 1) * frac)"""
-        if max_modes is not None:
-            modes_lat, modes_lon = max_modes
-        else:
-            modes_lat = int(self.h * hard_thresholding_fraction)
-            modes_lon = int((self.w // 2 + 1) * hard_thresholding_fraction)
+        """the processor's SHT pair on the (h, w) grid"""
+        modes_lat, modes_lon = self._modes(hard_thresholding_fraction, max_modes)
         self.sht = backend.RealSHT(self.h, self.w, lmax=modes_lat, mmax=modes_lon, grid=sht_grid_type).float()
         self.isht = backend.InverseRealSHT(self.h, self.w, lmax=modes_lat, mmax=modes_lon, grid=sht_grid_type).float()
+
+    def _modes(self, hard_thresholding_fraction, max_modes):
+        """modes = max_modes, else int(h * frac), int((w // 2 + 1) * frac)"""
+        if max_modes is not None:
+            return tuple(max_modes)
+        return int(self.h * hard_thresholding_fraction), int((self.w // 2 + 1) * hard_thresholding_fraction)
 
     def _precompute_channel_groups(self, channel_names, aux_channel_names):
         atmo_chans, surf_chans, dyn_aux_chans, stat_aux_chans, pressure_lvls = get_channel_groups(channel_names, aux_channel_names)
